@@ -1,23 +1,30 @@
 #!/usr/bin/env python
 """bench.py -- BASELINE.json's metric on BASELINE.json's configuration.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--blocks B] [--cls E50]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--blocks B] [--cls E50] [--dump-outputs DIR]
 
 metric  : "GB/s encode+decode on batched 64KiB blocks" -- raw (uncompressed) bytes per second through one encode pass
           plus one decode pass over the batch (the reference's convention: throughput numerator = uncompressed bytes in
           both directions, src/LZ4.Tests.Helpers/TimedMethod.cs:66-69).  GB = 1e9 bytes.
 step    : one pass of the hot path over the whole batch: ONE fast-encode launch over all blocks (raw -> fixed-stride
           slots, both resident in HBM), then the known-size decode of every block (slots -> a reused wave buffer).
-workload: configs[1] of BASELINE.json: 2^20 x 64 KiB independent blocks per GPU (64 GiB raw, > 500x the L2, so every
-          timed iteration streams from HBM), synthetic entropy class E50 (SURVEY.md 8d) unless --cls says otherwise.
+workload: configs[1] of BASELINE.json: 2^18 x 64 KiB independent blocks per GPU (16 GiB raw, > 300x the H100's 50 MB L2,
+          so every timed iteration streams from HBM; raw + slots + decode buffer take 48 GiB of the 80), synthetic entropy
+          class E50 (SURVEY.md 8d) unless --cls says otherwise.
 value   : whole-job throughput over all ranks, device-timed (CUDA events, barrier + synchronize on both sides, max over
           ranks), inputs already in HBM.
 e2e     : the same metric through the reference-facing C ABI with HOST buffers (pinned), H2D/D2H inside the timed region.
 roofline: algorithmic bytes (raw + compressed, SURVEY.md 8d) / CUDA-event duration of the launches, for the kernel that
           dominates the step (the fast encoder -- latency-bound by the exact greedy parse) and, as "roofline_decode",
           for the decoder, the kernel north_star sets the HBM target on.
-cpu_baseline / --impl reference: the reference's own original/lz4.c (oracle/_ref, built from /root/reference by
+cpu_baseline / --impl reference: the reference's own original/lz4.c (oracle/_ref, built from a lz4net checkout by
           oracle/Makefile; the oracle port if that file is absent) timed on the host cores with a static block partition.
+--dump-outputs DIR: after the timed steps, what the last step handed its caller, as float64 / float32 .npy files (< 64 MB):
+          clen.npy and used.npy (compressed length and bytes consumed by the decoder of every block; of 2^20 blocks drawn
+          with a fixed seed, listed in length_blocks.npy, when the batch is larger), sample_blocks.npy
+          (64 block indices drawn with a fixed seed from the last decode wave), compressed_sample.npy (their compressed
+          bytes, zero past each length) and decoded_sample.npy (their decoded bytes).  Inputs are seeded: the same
+          arguments give the same inputs on every run.
 
 Multi-GPU: one process per GPU under torch.distributed.run; blocks are independent (doc/compatibility.md:4-7), so ranks
 own disjoint block ranges and there is no data-path collective -- "scaling": "weak" (per-GPU work fixed).
@@ -45,13 +52,13 @@ def parse():
     p.add_argument("--steps", type=int, default=5)
     p.add_argument("--warmup", type=int, default=3)
     p.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    p.add_argument("--blocks", type=int, default=1 << 20, help="64 KiB blocks per GPU (default 2^20 = BASELINE configs[1])")
+    p.add_argument("--blocks", type=int, default=1 << 18, help="64 KiB blocks per GPU (default 2^18 = BASELINE configs[1])")
     p.add_argument("--cls", default="E50", choices=["E0", "E50", "E100", "ETEXT"])
     p.add_argument("--wave", type=int, default=1 << 18, help="blocks per decode wave (output buffer reuse)")
     p.add_argument("--e2e-blocks", type=int, default=1 << 14)
     p.add_argument("--cpu-blocks", type=int, default=1 << 15)
     p.add_argument("--lanes", type=int, default=0, help="decode lanes per block (4/8/16/32, +100 staged, 1/2 lane-per-block); 0 = library default (picked per batch)")
-    p.add_argument("--stream-gib", type=float, default=16.0, help="BASELINE configs[3]: size of the stream that starts on rank 0")
+    p.add_argument("--stream-gib", type=float, default=8.0, help="BASELINE configs[3]: size of the stream that starts on rank 0")
     p.add_argument("--no-stream", action="store_true")
     p.add_argument("--no-numa", action="store_true")
     p.add_argument("--enc-ctas", type=int, default=0)
@@ -61,15 +68,16 @@ def parse():
     p.add_argument("--no-e2e", action="store_true")
     p.add_argument("--sweep-blocks", type=int, default=1 << 17)
     p.add_argument("--hc-blocks", type=int, default=1 << 17)
+    p.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs here (.npy)")
     return p.parse_args()
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md: sample DURING the timed region)
+# clocks sampler: sampled DURING the timed region; the card's name and power limit are part of every number
 # ------------------------------------------------------------------------------------------------------------------
 class Clocks:
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit")
 
     def __init__(self, index: int):
         self.index = index; self.samples = []; self.proc = None; self.th = None
@@ -95,20 +103,21 @@ class Clocks:
             self.proc.wait(timeout=5)
         except Exception:
             pass
-        sm, mx, reasons = [], None, set()
+        sm, mx, reasons, card = [], None, set(), {}
         for s in self.samples:
             f = [x.strip() for x in s.split(",")]
-            if len(f) < 7:
+            if len(f) < 9:
                 continue
             try:
                 sm.append(float(f[0])); mx = float(f[1])
             except ValueError:
                 continue
+            card = {"gpu": f[7], "power_limit_w": f[8]}
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
         sm.sort()
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm)}
+        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm), **card}
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -535,7 +544,7 @@ def main():
     ctx = lz4net_b200.Context(local)
     # The headline runs the library's DEFAULTS: for device batches the decoder is picked per batch on the device from the
     # compression ratio.  TUNED_LANES (tools/sweep.py) is what a caller who knows the data could set by hand; the entropy
-    # sweep reports both side by side.
+    # sweep reports both side by side (on H100 the default is at or above them on every class: profiles/README.md).
     TUNED_LANES = {"E0": 32, "E50": 108, "E100": 16, "ETEXT": 104}
     if args.lanes:
         ctx.set_option("decode_lanes", args.lanes)
@@ -546,7 +555,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_hbm = float(peaks.get("hbm_gbs", 6650.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak_hbm = float(peaks.get("hbm_gbs", 3350.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "H100 SXM data sheet: 3350 GB/s HBM3"
 
     # ---- headline workload -------------------------------------------------------------------------------------------
     from lz4net_b200 import shard
@@ -576,6 +585,8 @@ def main():
         dist.barrier()
     clk = clocks.stop()
     launches = ctx.launches - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(work, args.dump_outputs)
     elapsed = t_start.elapsed_time(t_end) * 1e-3
     t_enc = sum(e[0][0].elapsed_time(e[0][1]) for e in evs) * 1e-3 / args.steps
     t_dec = sum(sum(p[0].elapsed_time(p[1]) for p in e[1:]) for e in evs) * 1e-3 / args.steps
@@ -586,17 +597,9 @@ def main():
     enc_gbs = total_raw / t_enc / GB; dec_gbs = total_raw / t_dec / GB
     # roofline (per GPU): algorithmic bytes = raw + compressed, both directions of each kernel (SURVEY.md 8d)
     alg = (total_raw + csum_all) / world
-    # DRAM traffic per launch: NOT measured in this run -- scaled per block from the committed ncu --set full capture
-    # (profiles/ncu_traffic.json, class E50 only), labelled as such
+    # DRAM traffic per launch needs a hardware-counter profile; this run does not take one
     traffic_dec = traffic_enc = None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        if args.cls == "E50":
-            traffic_dec = int(tj["lz4_decode_kernel"]["dram_bytes"] / tj["blocks"] * min(args.wave, args.blocks))
-            traffic_enc = int(tj["lz4_encode_fast_kernel"]["dram_bytes"] / tj["blocks"] * args.blocks)
-    except Exception:
-        pass
-    tsrc = "static: profiles/ncu_traffic.json (ncu --set full, bytes per block x blocks per launch), not measured in this run"
+    tsrc = "not measured"
     roof_dec = {"kernel": "lz4_decode_lpb_kernel (whole waves of the batch) + lz4_decode_kernel<8> (the rest), as picked on the device", "bound": "hbm", "achieved": round(alg / t_dec / GB, 1), "peak": peak_hbm, "unit": "GB/s",
                 "frac": round(alg / t_dec / GB / peak_hbm, 4), "traffic": traffic_dec, "traffic_source": tsrc, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": int(alg / nw), "launch_ms": round(t_dec / nw * 1e3, 3)}
@@ -759,7 +762,7 @@ def main():
         "config": {"workload": f"{args.blocks} x 64KiB independent blocks per GPU, class {args.cls} (BASELINE configs[1]): one fast-encode launch + {nw} known-size decode launches per step",
                    "block_size": BLOCK, "class": args.cls, "blocks_per_gpu": args.blocks, "ratio": round(csum_all / total_raw, 4),
                    "decode_lanes": args.lanes or "library default: picked per batch on the device from the compression ratio",
-                   "decode_wave_blocks": work_wave(args), "l2": "inputs (64 GiB raw + slots per GPU) are far larger than the 126 MB L2; no flush needed",
+                   "decode_wave_blocks": work_wave(args), "l2": f"inputs ({raw_bytes / 2**30:g} GiB raw + slots per GPU) are far larger than the 50 MB L2; no flush needed",
                    "parallelism": f"independent blocks sharded over {world} GPU(s), no data-path collective", "gb": "1e9 bytes"},
         "encode_gbs": round(enc_gbs, 2), "decode_gbs": round(dec_gbs, 2),
         "roofline": roof_enc, "roofline_decode": roof_dec,
@@ -770,6 +773,35 @@ def main():
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+MAX_LENGTHS = 1 << 20
+
+
+def dump_outputs(work, out_dir, n_sample=64):
+    """What the last timed step computed (see --dump-outputs): lengths of every block, bytes of a seeded sample."""
+    import numpy as np
+    torch = work.torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    b0 = (work.n_waves - 1) * work.wave                       # the decode buffer holds the last wave
+    rng = np.random.default_rng(20240601)
+    idx = np.sort(rng.choice(np.arange(b0, work.n), size=min(n_sample, work.n - b0), replace=False))
+    clen = work.clen.cpu().numpy()
+    lidx = np.arange(work.n)
+    if work.n > MAX_LENGTHS:                                  # keeps the dump below 64 MB at any --blocks
+        lidx = np.sort(rng.choice(work.n, size=MAX_LENGTHS, replace=False))
+    slots = work.slots.view(work.n, work.slot)[torch.from_numpy(idx).cuda()].cpu().numpy()
+    comp = np.zeros(slots.shape, np.float32)
+    for j, i in enumerate(idx):
+        comp[j, :max(int(clen[i]), 0)] = slots[j, :max(int(clen[i]), 0)]
+    dec = work.out.view(work.wave, BLOCK)[torch.from_numpy((idx - b0) % work.wave).cuda()].cpu().numpy()
+    arrays = {"clen": clen[lidx].astype(np.float32), "used": work.used.cpu().numpy()[lidx].astype(np.float32),
+              "sample_blocks": idx.astype(np.float64), "compressed_sample": comp, "decoded_sample": dec.astype(np.float32)}
+    if work.n > MAX_LENGTHS:
+        arrays["length_blocks"] = lidx.astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def work_wave(args):

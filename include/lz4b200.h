@@ -1,5 +1,5 @@
 /*
- * lz4b200.h -- C ABI of liblz4b200.so: the B200 (sm_100a) LZ4 r93 block codec behind lz4net's service boundary.
+ * lz4b200.h -- C ABI of liblz4b200.so: the H100 (sm_90a) LZ4 r93 block codec behind lz4net's service boundary.
  *
  * This is the drop-in boundary of the path (SURVEY.md 8b).  lz4net's native services (LZ4mm / LZ4cc) reach the
  * codec through exactly four C functions (src/LZ4cc/LZ4Codec.64.cpp:35,88,95,143 -> original/lz4.h:59-60,101,116,
@@ -13,7 +13,7 @@
  *   - known-size decode returns bytes READ from the source, < 0 = malformed     (original/lz4.h:96-101)
  *   - unknown-size decode returns bytes WRITTEN, < 0 = malformed                (original/lz4.h:104-116)
  *   - compressed bytes are identical to lz4net's LZ4Codec.Encode / EncodeHC on the same input
- * There is no CPU fallback: every entry point fails (LZ4B200_E_*) when no sm_100 device / kernel image is usable.
+ * There is no CPU fallback: every entry point fails (LZ4B200_E_*) when no sm_90 device / kernel image is usable.
  */
 #ifndef LZ4B200_H
 #define LZ4B200_H
@@ -37,7 +37,7 @@ extern "C" {
 /* status codes (batch / context calls).  Per-block results are reported in out_len[], never here. */
 #define LZ4B200_OK            0
 #define LZ4B200_E_ARG        -1
-#define LZ4B200_E_NODEVICE   -2        /* no CUDA device, or not compute capability 10.x */
+#define LZ4B200_E_NODEVICE   -2        /* no CUDA device, or not compute capability 9.x */
 #define LZ4B200_E_CUDA       -3        /* a CUDA runtime call failed; see lz4b200_last_error() */
 #define LZ4B200_E_NOMEM      -4
 #define LZ4B200_E_FORMAT     -5        /* malformed LZ4Stream / Wrap framing, or a chunk that does not decode */
@@ -46,7 +46,7 @@ typedef struct lz4b200_ctx lz4b200_ctx;
 
 int         lz4b200_version(void);
 const char* lz4b200_last_error(void);                 /* thread-local, never NULL */
-int         lz4b200_device_count(void);               /* usable (cc 10.x) devices; 0 if none */
+int         lz4b200_device_count(void);               /* usable (cc 9.x) devices; 0 if none */
 
 /* A context owns one device's stream, scratch (HC chain tables, staging) and tuning knobs.  Unlike the reference
  * (stateless: tables are allocated per call, src/LZ4ps/LZ4Codec.Safe.cs:407) the GPU path has state.

@@ -32,8 +32,8 @@ struct ILZ4Service {                                                     // src/
 
 class CudaLZ4Service : public ILZ4Service {
 public:
-    CudaLZ4Service() { if (lz4b200_device_count() < 1) throw std::runtime_error("CudaLZ4Service: no sm_100 device"); }
-    std::string CodecName() const override { return "CUDA sm_100a"; }
+    CudaLZ4Service() { if (lz4b200_device_count() < 1) throw std::runtime_error("CudaLZ4Service: no sm_90 device"); }
+    std::string CodecName() const override { return "CUDA sm_90a"; }
     int Encode(const uint8_t* in, int io, int il, uint8_t* out, int oo, int ol) override
     {
         if (il == 0 || ol == 0) return 0;                                // src/LZ4ps/LZ4Codec.cs:156-160, Safe.cs:403

@@ -1,4 +1,4 @@
-// CudaLZ4Service.cs -- ILZ4Service over liblz4b200 (the B200 / sm_100a LZ4 block codec of this repository).
+// CudaLZ4Service.cs -- ILZ4Service over liblz4b200 (the H100 / sm_90a LZ4 block codec of this repository).
 //
 // Drop into src/LZ4/Services/ of lz4net next to CppMM64LZ4Service.cs (which this file mirrors in shape:
 // src/LZ4/Services/CppMM64LZ4Service.cs:38-51) and compile it into the LZ4 assembly -- ILZ4Service is internal
@@ -39,17 +39,17 @@ namespace LZ4.Services
         [DllImport(Library, CallingConvention = CallingConvention.Cdecl)]
         private static extern int lz4b200_uncompress_unknownOutputSize(byte* source, byte* dest, int isize, int maxOutputSize);
 
-        /// <summary>Throws unless a compute-capability 10.x device is usable: TryService() then discards this service,
+        /// <summary>Throws unless a compute-capability 9.x device is usable: TryService() then discards this service,
         /// exactly like a native service whose assembly fails to load (src/LZ4/LZ4Codec.cs:278-290).</summary>
         public CudaLZ4Service()
         {
             if (lz4b200_device_count() < 1)
-                throw new NotSupportedException("lz4b200: no sm_100 device");
+                throw new NotSupportedException("lz4b200: no sm_90 device");
         }
 
         public string CodecName
         {
-            get { return "CUDA B200"; }
+            get { return "CUDA H100"; }
         }
 
         // the argument rules of src/LZ4ps/LZ4Codec.cs:151-170 (negative length = to the end of the array)

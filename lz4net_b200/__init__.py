@@ -1,4 +1,4 @@
-"""lz4net_b200 -- a B200 (sm_100a) LZ4 r93 block codec behind lz4net's LZ4Codec / ILZ4Service / LZ4Stream surface.
+"""lz4net_b200 -- an H100 (sm_90a) LZ4 r93 block codec behind lz4net's LZ4Codec / ILZ4Service / LZ4Stream surface.
 
 Only the hot path lives here: hand-written CUDA kernels (csrc/), their C ABI (include/lz4b200.h, liblz4b200.so) and
 the host-side mirror of the reference interface (codec.py).  There is no CPU codec in this package.

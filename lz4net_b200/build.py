@@ -1,10 +1,10 @@
-"""Builds lz4net_b200/liblz4b200.so in-tree with nvcc for sm_100a (the only target: no multi-arch fallback).
+"""Builds lz4net_b200/liblz4b200.so in-tree with nvcc for sm_90a (H100; the only target: no multi-arch fallback).
 
     python -m lz4net_b200.build            # incremental
     python -m lz4net_b200.build --force
 
-nvcc cross-compiles without a GPU, so this also runs in the CPU-only build container.  The .so is git-ignored but
-travels to the GPU box with the gpurun snapshot.
+nvcc cross-compiles without a GPU, so this also runs on a build machine without one.  The .so and the objects under
+lz4net_b200/build/ are git-ignored build products.
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "liblz4b200.so")
 SOURCES = ["capi.cu", "decode.cu", "encode.cu", "util.cu", "framing.cpp"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -57,7 +57,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     vs = os.path.join(objdir, "exports.map")
     with open(vs, "w") as f:
         f.write("{ global: lz4b200_*; local: *; };\n")
-    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT] + objs + ["-Xlinker", f"--version-script={vs}", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
+    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", OUT] + objs + ["-Xlinker", f"--version-script={vs}", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
     subprocess.check_call(cmd)
     return OUT
 

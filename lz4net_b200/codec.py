@@ -171,7 +171,7 @@ def default_context() -> Context:
 class CudaLZ4Service:
     """ILZ4Service (src/LZ4/ILZ4Service.cs:30-36) over the single-block C entry points."""
 
-    CodecName = "CUDA sm_100a"
+    CodecName = "CUDA sm_90a"
 
     @staticmethod
     def _ptr(buf, offset):
@@ -207,7 +207,7 @@ class LZ4Codec:
     """Static facade, src/LZ4/LZ4Codec.cs.  Buffers are bytearray / numpy uint8 arrays (the byte[] of the original)."""
 
     _service = CudaLZ4Service()
-    CodecName = "CUDA sm_100a/CUDA sm_100a/CUDA sm_100aHC"
+    CodecName = "CUDA sm_90a/CUDA sm_90a/CUDA sm_90aHC"
 
     @staticmethod
     def MaximumOutputLength(inputLength: int) -> int:                # :313-316

@@ -34,7 +34,7 @@ int cuda_fail(cudaError_t e, const char* what)
 
 constexpr int NSLOT = 3;                       // pipeline depth of host-memory batches
 constexpr int NCOUNTER = 256;
-constexpr size_t HOST_CHUNK_BYTES_DEFAULT = 128u << 20; // src + dst bytes per pipeline stage (tools/e2e_sweep.py: 128 MiB is the best of 32..512 on B200)
+constexpr size_t HOST_CHUNK_BYTES_DEFAULT = 128u << 20; // src + dst bytes per pipeline stage (on H100 the best of 32..512 MiB: profiles/README.md)
 
 struct DevBuf {
     void* p = nullptr; size_t cap = 0;
@@ -65,7 +65,7 @@ struct PinBuf {
 };
 
 // Pageable host memory (a managed caller's `fixed` byte[]): cudaMemcpyAsync from / to it is staged by the driver through
-// its own small pinned buffers, synchronously (measured: 4.5 GB/s round trip against 21 from pinned memory).  The library
+// its own small pinned buffers, synchronously (several times slower than from pinned memory).  The library
 // stages such buffers itself, a pipeline chunk at a time, with a handful of host threads doing the memcpy into / out of
 // its pinned chunk buffers while the previous chunks are on the wire.
 constexpr int STAGE_THREADS = 8;
@@ -118,7 +118,7 @@ struct lz4b200_ctx {
     int encode_variant = 2;                // same-hash detection inside a round: 1 exact votes, 2 optimistic (default)
     int encode_tune[4] = {512, 12, 8, 24}; // prefetch distance, lane_copy_max, probe_max, wide_min (lz4_encode.cuh EncTune)
     size_t host_chunk_bytes = HOST_CHUNK_BYTES_DEFAULT;
-    int hc_concurrency = 131072;         // blocks in flight (one thread each, 256 KiB state): 16384 / 65536 / 131072 / 262144 -> 2.8 / 8.3 / 9.7 / 9.7 GB/s (E50)
+    int hc_concurrency = 131072;         // blocks in flight (one thread each, 256 KiB state: 32 GiB of arena at this default)
     int hc_kernel = -1;                  // -1: chosen per batch (encode.cu launch_encode_hc_auto); 0: one thread per block (any block size); one warp per block on a static index (blocks <= 64 KiB, the rest is handed to 0): 1 = block staged in shared memory, 2 = nothing in shared memory
     int hc_warps_per_sm = 0;             // warp kernels: blocks in flight per SM (0 = 3 for kernel 1, 32 for kernel 2)
     Slot slot[NSLOT];
@@ -467,7 +467,7 @@ int lz4b200_device_count(void)
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
     for (int i = 0; i < n; i++) {
         int major = 0;
-        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 10) ok++;
+        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 9) ok++;
     }
     return ok;
 }
@@ -483,7 +483,7 @@ int lz4b200_create(lz4b200_ctx** out, int device)
     if (device < 0 || device >= n) return fail(LZ4B200_E_ARG, "device index out of range");
     int major = 0;
     CU(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major != 10) return fail(LZ4B200_E_NODEVICE, "device is not compute capability 10.x (this library holds sm_100a code only)");
+    if (major != 9) return fail(LZ4B200_E_NODEVICE, "device is not compute capability 9.x (this library holds sm_90a code only)");
     DeviceGuard g(device);
     if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
     lz4b200_ctx* c = new lz4b200_ctx();

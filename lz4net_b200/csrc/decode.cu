@@ -96,10 +96,10 @@ static cudaError_t launch_g(const BatchArgs& a, bool known, bool staged, uint32_
 }
 
 // ---- lane-per-block decoder (lz4_decode_lpb.cuh): one CTA per SM, as many warps as shared memory holds rings for --------
-// Geometry (tools/sweep.py, round 2): 128-byte input ring, 256-byte output window, runs up to 32 bytes copied by the lane,
+// Geometry (tools/sweep.py): 128-byte input ring, 256-byte output window, runs up to 32 bytes copied by the lane,
 // requests waited for at the top of the next iteration, two sequences per iteration: 16 warps = 512 blocks in flight per SM.
-// (256 / 512-byte rings with 64-byte runs and one-iteration-ahead requests -- 8 warps -- measured 1078 vs 1406 GB/s on E50
-// and 173 vs 269 GB/s on ETEXT: this kernel lives on resident warps.)
+// (256 / 512-byte rings with 64-byte runs and one-iteration-ahead requests -- 8 warps -- were slower on E50 and ETEXT alike:
+// this kernel lives on resident warps.)
 typedef LpbGeom<128, 256, 32, 0, 2> LpbDefault;
 // Warps per CTA: what 227 KiB of shared memory hold rings for, rounded DOWN to a multiple of four -- ptxas budgets registers
 // for the block size rounded up to 128 threads (17 warps were given the 96 registers of 20 and spilled the copy loops).
@@ -117,7 +117,7 @@ lz4_decode_lpb_kernel(BatchArgs a, uint32_t* counter, const int* pick, int takes
     lpb_decode_warp<KNOWN, GEO>(sh, b, counter, (int)(threadIdx.x & 31));
 }
 
-// The lane-per-block decoder holds one block per lane (148 x 16 x 32 = 75 776 at a time) and blocks of one class take
+// The lane-per-block decoder holds one block per lane (on H100 132 x 16 x 32 = 67 584 at a time) and blocks of one class take
 // about equally long, so a batch is worked off in waves: below half a wave the group kernels are ahead; on token-dense
 // data (class 104) it is 1.4-1.6x the 4-lane group kernel and pays from there on; on the middle class (108) its edge over
 // the 8-lane kernel is ~11 %, which a last wave that is less than ~90 % full gives back.
@@ -157,7 +157,7 @@ cudaError_t launch_decode(const BatchArgs& a, bool known_len, int lanes, uint32_
     if (e != cudaSuccess) return e;
     if (launches) ++*launches;
     if (lanes == 0) {
-        // auto: pick on the device, enqueue the four candidates (three of them return at once: ~3 us of GPU time each)
+        // auto: pick on the device, enqueue the four candidates (three of them return at once)
         int* pick = (int*)(counter + 1);             // (the context hands out counters in fours: [block counter, pick, two more counters])
         lz4_decode_pick_kernel<<<1, 256, 0, stream>>>(a.src_len, a.dst_cap, a.n_blocks, pick);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;

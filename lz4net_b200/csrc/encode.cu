@@ -10,11 +10,10 @@ namespace lz4b200 {
 // All encoder warps of an SM live in ONE CTA (up to 14 warps x 16 KiB position tables = 224 KiB of dynamic shared
 // memory -- separate CTAs would each pay 1 KiB of system-reserved shared memory, which costs the 14th warp).  The warps
 // never synchronise with each other.  (The launch bound only tells ptxas how many registers it may use: 65536 / 448.)
-// Measured and dropped in round 2 (profiles/encoder_r02_history.md): more warp-per-block encoders with their tables in
-// an L2-resident global arena (18 / 20 / 24 / 28 warps per SM: 0.83 / 0.74 / 0.5 / 0.4 of the 14-warp kernel -- the
-// register cap spills the parse and a table round trip becomes an L2 round trip), and a 15th warp whose lanes each encode
-// a block of their own with the table in global memory (0.66 - 0.82 of the 14-warp kernel even with tagged table entries:
-// its scattered table and candidate traffic costs the 14 warps more L2 hits than its own blocks add).
+// Tried and dropped: more warp-per-block encoders with their tables in an L2-resident global arena (the register cap
+// spills the parse and a table round trip becomes an L2 round trip), and a 15th warp whose lanes each encode a block of
+// their own with the table in global memory (its scattered table and candidate traffic costs the 14 warps more L2 hits
+// than its own blocks add).  The same shared-memory budget holds on H100 (227 KiB per block, 228 KiB per SM).
 constexpr int ENC_MAX_WARPS = 14;
 
 template <int DUP>
@@ -143,8 +142,8 @@ lz4_encode_hcw_kernel(BatchArgs a, uint8_t* arena, uint32_t* counter, const uint
 // statistic (depth = sum(min(c, 255) * c) / sum(c) = the clamped bucket size an average position sees: E0 3.0, E50 3.9,
 // natural text and code 20 - 66, ETEXT 240) is computed as well: with the warp kernel capped at 8 resident warps per SM by a
 // shared-memory carve-out preference it separated the batches the index paid for (depth >= 8) from those it did not; at its
-// real residency the warp kernel is ahead on every class measured (profiles/hc_ab_r02e.json: E50 10.5 against 9.7), so the
-// threshold is 0 and the statistic is kept for the record only.
+// real residency the warp kernel was ahead on every class timed (tools/hc_ab.py compares the kernels), so the threshold is
+// 0 and the statistic is kept for the record only.
 // words: [0] block counter of the codec kernels (used as the ticket here and left zero), [1] pick (0 thread kernel,
 // 2 warp kernel), [2] sum(c), [3] sum(min(c,255)*c) / 16.
 constexpr int HC_PICK_SAMPLE = 32;
@@ -237,7 +236,7 @@ static cudaError_t launch_hc_warps(const BatchArgs& a, void* scratch, int varian
         // Residency below 32 CTAs per SM is a matter of the grid alone: CTAs are placed breadth-first over the SMs and the
         // kernel is persistent.  No shared-memory carve-out preference: asking for "all L1" (cudaSharedmemCarveoutMaxL1)
         // left room for the system-reserved KiB of only a handful of CTAs per SM -- 16 to 32 warps per SM all ran at the
-        // speed of 8 (profiles/hc_ab_r02d.json: identical times); the default lets the driver size it for the occupancy.
+        // speed of 8 (tools/hc_ab.py: identical times); the default lets the driver size it for the occupancy.
         if (warps <= 16) lz4_encode_hcw_kernel<false, 16><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter, pick);
         else             lz4_encode_hcw_kernel<false, 32><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter, pick);
     }
@@ -261,7 +260,7 @@ cudaError_t launch_encode_hcw(const BatchArgs& a, void* scratch, int variant, in
 
 // ---- HC, kernel chosen per batch -------------------------------------------------------------------------------------
 // Small batches (at most three blocks per SM): the shared-memory warp kernel, whose time per block is the shortest by far
-// (20 ms for a lone block of text; a lone thread of the thread kernel needs 0.23 s, and seconds inside a full batch).
+// (a lone thread of the thread kernel walks its block's chains one dependent load at a time).
 // Larger batches: the pick kernel looks at a sample, then both candidates are enqueued and the one not chosen returns at once.
 bool hc_auto_small(int32_t n_blocks, const DeviceInfo& dev) { return n_blocks <= 3 * dev.num_sms; }
 

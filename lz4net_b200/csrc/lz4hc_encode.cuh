@@ -5,7 +5,7 @@
 //
 // Why a thread and not a warp: the cost of HC is the hash-chain walk (<= 256 dependent hops per searched position,
 // :423-433) -- pointer chasing whose next address is only known when the previous hop returns.  A warp cannot make
-// one chain go faster; what a B200 can do is keep tens of thousands of independent chains in flight so that HBM/L2
+// one chain go faster; what a GPU can do is keep tens of thousands of independent chains in flight so that HBM/L2
 // latency is hidden by thread-level parallelism.  Each thread therefore owns one block and a private
 // 256 KiB state (heads u32[32768] + chain u16[65536], :231-237) in global memory, handed out from a scratch arena.
 // The parse (3-match look-ahead state machine, :557-742) is control flow only and is restated branch for branch.

@@ -1,6 +1,6 @@
 // simt.cuh -- the handful of warp / memory primitives the codec kernels are written against.
 //
-// Device build (nvcc, sm_100a): thin wrappers over the hardware instructions (SHFL / VOTE / MATCH, LDG/STG with
+// Device build (nvcc, sm_90a): thin wrappers over the hardware instructions (SHFL / VOTE / MATCH, LDG/STG with
 // cache hints, cp.async.bulk + mbarrier for TMA-style staging -> SASS UBLKCP / SYNCS).
 // Test build (-DLZ4B200_SIMT_EMU, g++): the same names come from tests/simt_emu/simt_emu.h, a coroutine emulation
 // of one warp used only by the CPU-side logic tests.  The product library is never built that way.

@@ -125,10 +125,10 @@ def encode_stream_sharded(raw_root, n_blocks: int, block_size: int, encode_local
     (None, None, None) elsewhere.
 
     Every rank's block range can be cut into `pieces` sub-ranges (all transfers posted up front, a piece encoded as soon
-    as it has arrived).  Measured on 2 and 4 B200s (tools/stream_ab.py) that buys nothing: a point-to-point transfer is a
+    as it has arrived).  That bought nothing when measured (tools/stream_ab.py): a point-to-point transfer is a
     KERNEL of the communication library, and it is not scheduled while the persistent encode kernel holds every SM's
     shared memory -- the pieces arrive back to back before the first encode or after the last one.  (Sending rank 1 its
-    range first, then rank 2's, ... is worse for the same reason: 133 instead of 191 GB/s at 4 GPUs.)  The transfers that
+    range first, then rank 2's, ... is worse for the same reason.)  The transfers that
     do overlap the kernels are the copy engines' -- StreamWindow below."""
     import torch
     import torch.distributed as dist

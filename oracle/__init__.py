@@ -4,10 +4,11 @@ Two interchangeable implementations, both loaded through ctypes:
 
 * ``port``  -- ``oracle/liblz4_oracle.so``: this repo's own plain-C restatement (``lz4_oracle.c``).
 * ``ref``   -- ``oracle/_ref/liblz4net_ref.so``: the reference's ``original/lz4.c`` + ``original/lz4hc.c``
-  compiled in place from ``/root/reference`` by ``oracle/Makefile`` with lz4net's 64-bit shim flags
+  compiled in place from the lz4net checkout named by ``$LZ4NET_REFERENCE`` by ``oracle/Makefile`` with lz4net's 64-bit shim flags
   (``src/adapters/cpp/lz4_64.h:5-9``).  lz4net's ConformanceTests assert this code byte-identical to every
   C# codec flavour (``src/LZ4.Tests/ConformanceTests.cs:59-68,125-132``), which is what makes it a valid
-  stand-in for ``LZ4Codec.Encode`` bytes.
+  stand-in for ``LZ4Codec.Encode`` bytes.  Optional: the tests read what it produced from ``tests/golden/``
+  (``tests/golden/make_golden.py``), so they run without a lz4net checkout.
 
 Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s CPU-baseline legs may import this module.
 The product package ``lz4net_b200`` never does.
@@ -23,19 +24,21 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _PORT_SO = os.path.join(_HERE, "liblz4_oracle.so")
 _REF_SO = os.path.join(_HERE, "_ref", "liblz4net_ref.so")
+REF_ENV = "LZ4NET_REFERENCE"                  # a MiloszKrajewski/lz4net checkout (only make_golden.py needs one)
 
 _port = None
 _ref = None
 
 
 def build(force: bool = False) -> None:
-    """Compile the port (always possible: gcc only) and, where /root/reference exists, oracle/_ref."""
+    """Compile the port (always possible: gcc only) and, where $LZ4NET_REFERENCE names a lz4net checkout, oracle/_ref."""
     if force or not os.path.exists(_PORT_SO) or \
             os.path.getmtime(_PORT_SO) < max(os.path.getmtime(os.path.join(_HERE, f))
                                              for f in ("lz4_oracle.c", "lz4_oracle.h", "oracle_mt.c")):
         subprocess.check_call(["make", "-C", _HERE, "liblz4_oracle.so"], stdout=subprocess.DEVNULL)
-    if os.path.exists("/root/reference/original/lz4.c") and (force or not os.path.exists(_REF_SO)):
-        subprocess.check_call(["make", "-C", _HERE, "ref"], stdout=subprocess.DEVNULL)
+    ref_dir = os.environ.get(REF_ENV, "")
+    if ref_dir and os.path.exists(os.path.join(ref_dir, "original", "lz4.c")) and (force or not os.path.exists(_REF_SO)):
+        subprocess.check_call(["make", "-C", _HERE, "ref", "REF=" + os.path.abspath(ref_dir)], stdout=subprocess.DEVNULL)
 
 
 def _u8p(a):
@@ -73,7 +76,7 @@ def ref():
     global _ref
     if _ref is None:
         if not have_ref():
-            raise RuntimeError("oracle/_ref/liblz4net_ref.so is absent (needs /root/reference to build)")
+            raise RuntimeError(f"oracle/_ref/liblz4net_ref.so is absent (set {REF_ENV} to a lz4net checkout to build it)")
         lib = C.CDLL(_REF_SO)
         cp = C.c_char_p
         for name in ("LZ4_compress_limitedOutput", "LZ4_compressHC_limitedOutput", "LZ4_uncompress_unknownOutputSize"):
@@ -159,7 +162,7 @@ def mt_run(kind: str, impl: str, src: np.ndarray, src_off, src_len, dst: np.ndar
         fn = {"encode": lib.LZ4_compress_limitedOutput, "encode_hc": lib.LZ4_compressHC_limitedOutput,
               "decode": lib.LZ4_uncompress}[kind]
     else:
-        fn = {"encode": p.lz4o_encode, "encode_hc": p.lz4o_encode_hc, "decode": p.lz4o_decode3}[kind]
+        fn = {"encode": p.lz4o_encode4, "encode_hc": p.lz4o_encode_hc4, "decode": p.lz4o_decode3}[kind]
     fnp = C.cast(fn, C.c_void_p)
     src_off = np.ascontiguousarray(src_off, dtype=np.int64)
     dst_off = np.ascontiguousarray(dst_off, dtype=np.int64)

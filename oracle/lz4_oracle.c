@@ -12,7 +12,7 @@
  * golden vectors in tests/golden/ (generated from oracle/_ref by tests/golden/make_golden.py).
  *
  * Every function cites the reference lines it restates.  All reference citations are relative to
- * /root/reference/.
+ * the root of a MiloszKrajewski/lz4net checkout.
  */
 #include "lz4_oracle.h"
 #include <string.h>
@@ -387,3 +387,8 @@ int lz4o_decode3(const char* src, char* dst, int osize)
 {
     return lz4o_decode_known((const uint8_t*)src, -1, (uint8_t*)dst, osize);
 }
+
+/* LZ4_compress[HC]_limitedOutput-shaped wrappers (src, dst, isize, cap) for oracle_mt.c: the port's own argument
+ * order is (src, isize, dst, cap) */
+int lz4o_encode4(const char* src, char* dst, int isize, int cap) { return lz4o_encode((const uint8_t*)src, isize, (uint8_t*)dst, cap); }
+int lz4o_encode_hc4(const char* src, char* dst, int isize, int cap) { return lz4o_encode_hc((const uint8_t*)src, isize, (uint8_t*)dst, cap); }

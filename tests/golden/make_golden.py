@@ -1,7 +1,11 @@
-"""Regenerates tests/golden/golden_v1.json from the REFERENCE's own code (oracle/_ref/liblz4net_ref.so, i.e.
-/root/reference/original/lz4.c + lz4hc.c compiled in place by oracle/Makefile).  Run only in the build container:
+"""Regenerates tests/golden/golden_v1.json and tests/golden/reference_v1.json from the REFERENCE's own code
+(oracle/_ref/liblz4net_ref.so, i.e. a lz4net checkout's original/lz4.c + lz4hc.c compiled in place by oracle/Makefile):
 
-    python tests/golden/make_golden.py
+    LZ4NET_REFERENCE=<lz4net checkout> python tests/golden/make_golden.py
+
+golden_v1.json: encoder outputs on named inputs.  reference_v1.json: the reference's side of tests/test_oracle.py's
+port-versus-reference checks (return values and output digests), and the one input on which r93's LZ4HC gives up at
+LZ4_compressBound (tests/test_kernels_emu.py).
 
 The reference ships no golden vectors of its own (SURVEY.md 8c); these are outputs of the reference itself on
 reproducible inputs (tests/cases.py), including the reference-defined AutoTest text (src/LZ4/LZ4Codec.cs:175-184).
@@ -47,6 +51,21 @@ def main():
     json.dump({"source": "oracle/_ref (reference original/lz4.c + lz4hc.c, LZ4_ARCH64=1, LZ4_MK_OPT)", "cases": out},
               open(path, "w"), indent=1)
     print("wrote", path, len(out), "cases")
+
+    from lz4net_b200 import synth
+    from tests import test_oracle as t
+    d = synth.make_blocks("E0", 1, 65536, seed=3, first_block=1268)[0].tobytes()
+    ref = {"source": "oracle/_ref (reference original/lz4.c + lz4hc.c, LZ4_ARCH64=1, LZ4_MK_OPT)",
+           "random_lengths": {m: t._digest(*t.records_random_lengths(m, "ref")) for m in cases.MODELS},
+           "accept_reject": t.digest_accept_reject(t.records_accept_reject("ref")),
+           "corrupt_streams": t.records_corrupt_streams("ref"),
+           "hc_gives_up_at_bound": {"class": "E0", "seed": 3, "first_block": 1268,
+                                    "ret": oracle.encode_hc(d, cap=oracle.bound(len(d)), impl="ref")[0]}}
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_v1.json")
+    with open(path, "w") as f:
+        json.dump(ref, f, separators=(",", ":"))
+        f.write("\n")
+    print("wrote", path)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): every check calls liblz4b200.so through its C ABI and compares with the oracle.
+"""GPU parity tests (H100): every check calls liblz4b200.so through its C ABI and compares with the oracle.
 
 Same shape as lz4net's ConformanceTests (src/LZ4.Tests/ConformanceTests.cs:57-148: all encoders byte-identical, all
 decoders round-trip), WrapTests.cs:11-48, StreamTests.cs:22-63 and the upstream fuzzer's +-1 invariants

@@ -1,6 +1,8 @@
-"""CPU-only: pins the port oracle (oracle/lz4_oracle.c) to the reference's own sources (oracle/_ref) and to the
-committed golden vectors.  Mirrors src/LZ4.Tests/ConformanceTests.cs (all encoders byte-identical, all decoders
-round-trip) and original/fuzzer.c:146-233 (size +-1 invariants)."""
+"""CPU-only: pins the port oracle (oracle/lz4_oracle.c) to the reference's own sources and to the committed golden
+vectors.  Mirrors src/LZ4.Tests/ConformanceTests.cs (all encoders byte-identical, all decoders round-trip) and
+original/fuzzer.c:146-233 (size +-1 invariants).  What the reference (oracle/_ref) returned on these inputs is stored in
+tests/golden/reference_v1.json (tests/golden/make_golden.py): the records below are computed with the port and compared
+with the reference's."""
 import hashlib
 import json
 import os
@@ -12,11 +14,88 @@ import oracle
 from tests import cases
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden", "golden_v1.json")
-needs_ref = pytest.mark.skipif(not oracle.have_ref(), reason="oracle/_ref not built (needs /root/reference)")
+REF = os.path.join(os.path.dirname(__file__), "golden", "reference_v1.json")
 
 
 def _sha(b: bytes) -> str:
     return hashlib.sha256(b).hexdigest()
+
+
+def _digest(*parts) -> str:
+    h = hashlib.sha256()
+    for p in parts:
+        h.update(p if isinstance(p, bytes) else str(p).encode())
+        h.update(b"|")
+    return h.hexdigest()[:12]
+
+
+def _stored(key):
+    return json.load(open(REF))[key]
+
+
+def records_random_lengths(model, impl):
+    """[n, ret fast, ret HC, digest of every return value and output, limited outputs included] per input."""
+    out = []
+    lens = cases.random_lengths(60, 200_000, seed=7) + list(cases.BOUNDARY_LENGTHS)
+    for i, n in enumerate(lens):
+        if model in ("mixed",) and n > 70_000:
+            n = n % 70_000
+        data = cases.content(model, n, seed=i).tobytes()
+        rets, parts = [], []
+        for fn in (oracle.encode, oracle.encode_hc):
+            r, o = fn(data, impl=impl)
+            rets.append(r); parts += [r, o]
+            # limited output: exactly enough, one short, and cap = n (fuzzer.c:212-227; LZ4Stream.cs:243-246)
+            for cap in sorted({r, r - 1, n, max(0, n - 1), r // 2}):
+                if cap >= 0:
+                    parts += [cap, *fn(data, cap=cap, impl=impl)]
+        out.append([n, *rets, _digest(*parts)])
+    return out
+
+
+def records_accept_reject(impl):
+    """fuzzer.c:176-210 on 48 inputs: the compressed stream, known-size verdicts for n, n-1, n+1, and unknown-size verdicts
+    (+ output digest) for the (input size, output capacity) pairs of _ACCEPT_REJECT_SIZES."""
+    rng = np.random.default_rng(3)
+    from lz4net_b200 import synth
+    out = []
+    for i in range(48):
+        fuz = i % 6 == 5      # the upstream generator: for it the +-1 invariants are strict (fuzzer.c:176-210)
+        data = (synth.fuz_block(i, 4096) if fuz else
+                cases.content(cases.MODELS[i % len(cases.MODELS)], int(rng.integers(20, 40000)), seed=100 + i)).tobytes()
+        n = len(data)
+        _, comp = oracle.encode(data, impl=impl)
+        clen = len(comp)
+        known = [oracle.decode_known(comp, osize, impl=impl)[0] for osize in (n, n - 1, n + 1)]
+        unknown = []
+        for isz, osz in ((clen, n + 1), (clen, n), (clen, n - 1), (clen - 1, n), (clen + 1, n)):
+            cc = comp if isz <= clen else comp + b"\x00"
+            r, o = oracle.decode_unknown(cc[:isz], osz, impl=impl)
+            unknown.append([r, _digest(o) if r >= 0 else None])
+        out.append({"n": n, "fuz": fuz, "clen": clen, "comp": _digest(comp), "known": known, "unknown": unknown})
+    return out
+
+
+def digest_accept_reject(records):
+    """What the port must share with the reference: every input, stream and verdict, and the value and output of every
+    accepted decode (the magnitude of an error result is not part of parity)."""
+    return _digest(*(json.dumps([r["n"], r["clen"], r["comp"], [max(a, -1) for a in r["known"]],
+                                 [[max(a, -1), d] for a, d in r["unknown"]]]) for r in records))
+
+
+def records_corrupt_streams(impl):
+    """300 bit-flipped streams: (digest of all the streams, [unknown-size verdict, output digest or None] per stream)."""
+    rng = np.random.default_rng(11)
+    out, streams = [], []
+    for i in range(300):
+        data = cases.content("mixed", 3000, seed=i).tobytes()
+        _, comp = oracle.encode(data, impl=impl)
+        c = bytearray(comp)
+        for _ in range(int(rng.integers(1, 4))):
+            c[int(rng.integers(0, len(c)))] ^= 1 << int(rng.integers(0, 8))
+        r, o = oracle.decode_unknown(bytes(c), len(data), impl=impl)
+        streams.append(bytes(c)); out.append([max(r, -1), _digest(o)[:8] if r >= 0 else None])
+    return _digest(*streams), out
 
 
 def test_bound():
@@ -45,76 +124,41 @@ def test_golden_vectors_port():
             assert r2 == c[mode]["len_cap_n"], (c["name"], mode)
 
 
-@needs_ref
 @pytest.mark.parametrize("model", cases.MODELS)
 def test_port_equals_reference_random_lengths(model):
-    lens = cases.random_lengths(60, 200_000, seed=7) + list(cases.BOUNDARY_LENGTHS)
-    for i, n in enumerate(lens):
-        if model in ("mixed",) and n > 70_000:
-            n = n % 70_000
+    got = records_random_lengths(model, "port")
+    assert _digest(*got) == _stored("random_lengths")[model], model
+    for i, (n, _, _, _) in enumerate(got):
         data = cases.content(model, n, seed=i).tobytes()
-        for fn in (oracle.encode, oracle.encode_hc):
-            if fn is oracle.encode_hc and n > 70_000 and model in ("E100", "runs", "periodic"):
-                pass
-            rr, ro = fn(data, impl="ref")
-            rp, po = fn(data, impl="port")
-            assert (rr, ro) == (rp, po), (model, n, fn.__name__)
-            # limited output: exactly enough, one short, and cap = n (fuzzer.c:212-227; LZ4Stream.cs:243-246)
-            for cap in {rr, rr - 1, n, max(0, n - 1), rr // 2}:
-                if cap < 0:
-                    continue
-                a = fn(data, cap=cap, impl="ref")
-                b = fn(data, cap=cap, impl="port")
-                assert a == b, (model, n, cap, fn.__name__)
-            d1 = oracle.decode_known(ro, n, impl="port")
-            d2 = oracle.decode_unknown(ro, n, impl="port")
-            assert d1 == (rr, data) and d2 == (n if n else d2[0], data)
+        r, o = oracle.encode(data)
+        d1 = oracle.decode_known(o, n, impl="port")
+        d2 = oracle.decode_unknown(o, n, impl="port")
+        assert d1 == (r, data) and d2 == (n if n else d2[0], data)
 
 
-@needs_ref
 def test_decoders_accept_reject_like_reference():
     """fuzzer.c:176-210: exact size works, size +-1 must fail; the port takes the same decisions as the reference."""
-    rng = np.random.default_rng(3)
-    from lz4net_b200 import synth
-    for i in range(48):
-        fuz = i % 6 == 5      # the upstream generator: for it the +-1 invariants are strict (fuzzer.c:176-210)
-        data = (synth.fuz_block(i, 4096) if fuz else
-                cases.content(cases.MODELS[i % len(cases.MODELS)], int(rng.integers(20, 40000)), seed=100 + i)).tobytes()
-        n = len(data)
-        _, comp = oracle.encode(data, impl="ref")
-        clen = len(comp)
-        for osize in (n, n - 1, n + 1):
-            a = oracle.decode_known(comp, osize, impl="ref")[0]
-            b = oracle.decode_known(comp, osize, impl="port")[0]
-            assert (a < 0) == (b < 0) and (a < 0 or a == b), (i, osize, a, b)
+    got = records_accept_reject("port")
+    assert digest_accept_reject(got) == _stored("accept_reject")          # the same decisions as the reference
+    for g in got:
+        n, clen = g["n"], g["clen"]
+        for osize, a in zip((n, n - 1, n + 1), g["known"]):
             assert (osize == n) == (a >= 0)
-        for isz, osz in ((clen, n + 1), (clen, n), (clen, n - 1), (clen - 1, n), (clen + 1, n)):
-            cc = comp if isz <= clen else comp + b"\x00"
-            a = oracle.decode_unknown(cc[:isz], osz, impl="ref")
-            b = oracle.decode_unknown(cc[:isz], osz, impl="port")
-            assert (a[0] < 0) == (b[0] < 0), (i, isz, osz, a[0], b[0])
-            if a[0] >= 0:
-                assert a == b
-            if fuz or isz == clen:
+        sizes = ((clen, n + 1), (clen, n), (clen, n - 1), (clen - 1, n), (clen + 1, n))
+        for (isz, osz), a in zip(sizes, g["unknown"]):
+            if g["fuz"] or isz == clen:
                 # (on arbitrary data a truncated stream can, rarely, still parse: the match-length loop stops at
                 #  iend-6 and re-reads its last byte as a token, original/lz4.c:986-999)
                 assert (a[0] >= 0) == (isz == clen and osz >= n)
 
 
-@needs_ref
 def test_corrupt_streams_same_verdict():
     """Bit-flipped streams: the port must never crash and must agree with the reference on accept/reject
     (and on the bytes when both accept), except for offset-0 matches which the port rejects by design."""
-    rng = np.random.default_rng(11)
     agree = 0
-    for i in range(300):
-        data = cases.content("mixed", 3000, seed=i).tobytes()
-        _, comp = oracle.encode(data, impl="ref")
-        c = bytearray(comp)
-        for _ in range(int(rng.integers(1, 4))):
-            c[int(rng.integers(0, len(c)))] ^= 1 << int(rng.integers(0, 8))
-        a = oracle.decode_unknown(bytes(c), len(data), impl="ref")
-        b = oracle.decode_unknown(bytes(c), len(data), impl="port")
+    (want_streams, want), (got_streams, got) = _stored("corrupt_streams"), records_corrupt_streams("port")
+    assert got_streams == want_streams                 # the same corrupted streams
+    for a, b in zip(want, got):
         if (a[0] < 0) == (b[0] < 0):
             agree += 1
             if a[0] >= 0:
@@ -133,3 +177,22 @@ def test_fuz_generator_roundtrip():
         assert oracle.decode_known(c, len(data)) == (r, data)
         assert oracle.decode_known(ch, len(data)) == (rh, data)
         assert oracle.decode_known(c, len(data) - 1)[0] < 0 and oracle.decode_known(c, len(data) + 1)[0] < 0
+
+
+def test_mt_run_port_matches_single_calls():
+    """bench.py's CPU baseline times the port through oracle.mt_run when oracle/_ref is absent (a default build)."""
+    from lz4net_b200 import synth
+    n, bs = 12, 65536
+    raw = synth.make_blocks("E50", n, bs, seed=5).reshape(-1)
+    slot = oracle.bound(bs)
+    so = np.arange(n, dtype=np.int64) * bs; do = np.arange(n, dtype=np.int64) * slot
+    sl = np.full(n, bs, np.int32); dc = np.full(n, slot, np.int32)
+    for kind, fn in (("encode", oracle.encode), ("encode_hc", oracle.encode_hc)):
+        comp = np.zeros(n * slot + 64, np.uint8)
+        _, clen = oracle.mt_run(kind, "port", raw, so, sl, comp, do, dc, 3)
+        for i in range(n):
+            r, o = fn(raw[i * bs:(i + 1) * bs])
+            assert clen[i] == r and comp[do[i]:do[i] + r].tobytes() == o, (kind, i)
+        out = np.zeros(n * bs + 64, np.uint8)
+        _, used = oracle.mt_run("decode", "port", comp, do, clen, out, so, sl, 3)
+        assert np.array_equal(used, clen) and np.array_equal(out[:n * bs], raw), kind

@@ -1,4 +1,4 @@
-"""Device-timed decode/encode sweep over entropy classes and tuning knobs (one gpurun call).
+"""Device-timed decode/encode sweep over entropy classes and tuning knobs (one GPU process).
 usage: python tools/sweep.py [blocks]"""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -8,7 +8,7 @@ from bench import Workload, measure_pair, BLOCK, GB
 
 nb = int(sys.argv[1]) if len(sys.argv) > 1 else 65536
 ctx = lz4net_b200.Context(0)
-peak = 6587.0
+peak = 3350.0                       # H100 SXM HBM3, data sheet
 res = {}
 CLASSES = sys.argv[2].split(",") if len(sys.argv) > 2 else ("E0", "E50", "E100", "ETEXT")
 ENC = len(sys.argv) <= 3 or sys.argv[3] == "enc"

@@ -1,5 +1,5 @@
-// ubench.cu -- single-warp latency probes for the primitives the encoder's parse chain is built from (B200, sm_100a).
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench tools/ubench.cu ; run on the GPU box.
+// ubench.cu -- single-warp latency probes for the primitives the encoder's parse chain is built from (H100, sm_90a).
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench tools/ubench.cu ; run on an H100.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
