@@ -34,6 +34,7 @@
 #pragma once
 #include "simt.cuh"
 #include "lz4_copy.cuh"
+#include "enc_prof.cuh"
 
 namespace lz4b200 {
 
@@ -52,19 +53,6 @@ struct EncTune {
 // flags kept above the 16-bit offset of a parked sequence
 constexpr uint32_t SEQ_NOCHK = 0x10000u;                           // zero-literal `goto _next_match` sequence: no :663 check
 constexpr uint32_t SEQ_LAST  = 0x20000u;                           // the last literal run (no match part)
-
-// Lanes whose hash equals mine (bit mask, always contains me): one vote per hash bit.  Invalid lanes match nobody.
-template <int BITS>
-SIMT_DEV uint32_t hash_peers(uint32_t h, bool valid, uint32_t vmask, int lane)
-{
-    uint32_t m = vmask;
-#pragma unroll
-    for (int b = 0; b < BITS; b++) {
-        const uint32_t v = simt::ballot(0xFFFFFFFFu, (h >> b) & 1u);
-        m &= ((h >> b) & 1u) ? v : ~v;
-    }
-    return valid ? m : (1u << lane);
-}
 
 // A long literal run (> 32 bytes), copied by the whole warp with pipelined 128-bit moves.  Kept out of line: it is the
 // rare path of the emission, and inlined its eight vector registers pairs would spill the parse loop.
@@ -95,9 +83,10 @@ struct EncTable {
 // once more: now the winner learns about a loser, and a loser that loses again knows the bucket has three or more
 // sharers.  Two sharers (by far the common case: a match whose source lies inside the round) are resolved exactly from
 // that -- the later iteration's candidate is the earlier one's position and its candidate word is the earlier one's
-// input word, moved by SHFL, no load; three or more take the exact path (one vote per hash bit) over the first 32
-// iterations.  At the end every bucket gets its final value: the position of the last sharer whose iteration really
-// ran (index <= f), or its old entry if none did.
+// input word, moved by SHFL, no load; three or more take the exact path (one vote per hash bit and half) over all the
+// iterations of the round, so its result is final as well.  At the end every bucket gets its final value: the position
+// of the last sharer whose iteration really ran (index <= f), or its old entry if none did.
+// f: the first iteration that hits or runs past mflimit; 32*W when none does.
 struct RoundOut { int f; bool finished; int ip, ref; };
 
 // SIMPLE: every attempt of the round still has step 1 and lies inside the block (known from two warp-uniform tests):
@@ -108,6 +97,9 @@ SIMT_DEV RoundOut find_round(const EncTable<GENERAL>& T, const InWords& in, int 
 {
     constexpr uint32_t FULL = 0xFFFFFFFFu;
     constexpr int HSHIFT = GENERAL ? 20 : 19;                      // :185-187 / :566-569
+    ENC_PROF_T0(tp);
+    ENC_PROF_EVENT(EP_ROUND);
+    ENC_PROF_EVENT_IF(EP_ROUND_WIDE, W == 2);
     int pos[W]; bool valid[W]; uint32_t v[W], h[W]; int t[W]; uint32_t vmask[W];
     InWords::Raw rp[W], rc[W];
     const int p0 = org + (int)A0 - 64;                             // SIMPLE: attempt A0 + i sits at p0 + i (S(a) = a - 64 up to a = 128)
@@ -132,6 +124,7 @@ SIMT_DEV RoundOut find_round(const EncTable<GENERAL>& T, const InWords& in, int 
     for (int s = 0; s < W; s++) t[s] = T.get(h[s]);
 #pragma unroll
     for (int s = 0; s < W; s++) rc[s] = in.raw<LDP>(t[s]);          // candidate words for the table entries: in flight from here
+    ENC_PROF_LAP(EP_C_LOADHASH, tp);
 
     RoundOut o; o.finished = false; o.ip = o.ref = 0;
     int partner[W];
@@ -162,6 +155,7 @@ SIMT_DEV RoundOut find_round(const EncTable<GENERAL>& T, const InWords& in, int 
             multi = simt::ballot(FULL, m);
         }
     }
+    ENC_PROF_LAP(EP_C_SAMEHASH, tp);
     if (DUP == 2 && multi == 0u) {
         uint32_t hitm[W]; int cand[W];
 #pragma unroll
@@ -211,9 +205,10 @@ SIMT_DEV RoundOut find_round(const EncTable<GENERAL>& T, const InWords& in, int 
                 o.ref = (int)simt::shfl(FULL, (uint32_t)(hi ? cand[W - 1] : cand[0]), f & 31);
             }
         }
+        ENC_PROF_LAP(EP_C_VOTE, tp);
         return o;
     }
-    // ---- exact path over the first 32 iterations (three or more iterations share a bucket, or DUP == 1) ----
+    // ---- exact path over the whole round (three or more iterations share a bucket, or DUP == 1) ----
     if (DUP == 2) {
         simt::syncwarp(FULL);
 #pragma unroll
@@ -221,26 +216,68 @@ SIMT_DEV RoundOut find_round(const EncTable<GENERAL>& T, const InWords& in, int 
         simt::syncwarp(FULL);
     }
     {
-        const uint32_t same = hash_peers<GENERAL ? 12 : 13>(h[0], valid[0], vmask[0], lane);
-        const uint32_t lower = same & lt_mask;
-        const int from = lower ? 31 - simt::clz(lower) : lane;
-        const int fwd = (int)simt::shfl(FULL, (uint32_t)pos[0], from);
-        const uint32_t fv = simt::shfl(FULL, v[0], from);
-        const int cand = lower ? fwd : t[0];
-        const uint32_t w0 = lower ? fv : InWords::word(rc[0]);
-        const bool hit = valid[0] && !(fused && lane == 0) && (!GENERAL || cand >= pos[0] - 65535) && w0 == v[0];
-        const uint32_t stop = simt::ballot(FULL, !valid[0] || hit);
-        const int f = stop ? simt::ffs(stop) - 1 : 32;
-        // commit the table writes of the serial iterations that really happened (lanes <= f), last writer per bucket
-        const uint32_t cmask = f >= 31 ? vmask[0] : (vmask[0] & ((2u << f) - 1u));
-        const uint32_t above = same & cmask & ~((2u << lane) - 1u);
-        if (((cmask >> lane) & 1u) && !above) T.put(h[0], pos[0]);
-        simt::syncwarp(FULL);
-        o.f = f < 32 ? f : -1;                                      // -1: nothing happened, and only 32 iterations were evaluated
-        if (f < 32) {
-            if (!((cmask >> f) & 1u)) o.finished = true;
-            else { o.ip = (int)simt::shfl(FULL, (uint32_t)pos[0], f); o.ref = (int)simt::shfl(FULL, (uint32_t)cand, f); }
+        // same[s][u]: the lanes whose iteration in half u has the hash of my iteration in half s (invalid ones: nobody)
+        uint32_t same[W][W];
+#pragma unroll
+        for (int s = 0; s < W; s++)
+#pragma unroll
+            for (int u = 0; u < W; u++) same[s][u] = vmask[u];
+#pragma unroll
+        for (int b = 0; b < (GENERAL ? 12 : 13); b++) {
+            uint32_t vb[W];
+#pragma unroll
+            for (int u = 0; u < W; u++) vb[u] = simt::ballot(FULL, (h[u] >> b) & 1u);
+#pragma unroll
+            for (int s = 0; s < W; s++)
+#pragma unroll
+                for (int u = 0; u < W; u++) same[s][u] &= ((h[s] >> b) & 1u) ? vb[u] : ~vb[u];
         }
+        // the candidate: the position of the latest earlier sharer (in my half, else in the first), else the table entry
+        int cand[W]; uint32_t stop[W];
+#pragma unroll
+        for (int s = 0; s < W; s++) {
+            const uint32_t own = valid[s] ? same[s][s] & lt_mask : 0u;
+            const uint32_t lower = own ? own : (s == 1 && valid[s] ? same[W - 1][0] : 0u);
+            const int from = lower ? 31 - simt::clz(lower) : lane;
+            int fwd = (int)simt::shfl(FULL, (uint32_t)pos[0], from);
+            uint32_t fv = simt::shfl(FULL, v[0], from);
+            if (s == 1) {
+                const int fwd1 = (int)simt::shfl(FULL, (uint32_t)pos[W - 1], from);
+                const uint32_t fv1 = simt::shfl(FULL, v[W - 1], from);
+                if (own) { fwd = fwd1; fv = fv1; }
+            }
+            cand[s] = lower ? fwd : t[s];
+            const uint32_t w = lower ? fv : InWords::word(rc[s]);
+            const bool hit = valid[s] && !(fused && s == 0 && lane == 0) && (!GENERAL || cand[s] >= pos[s] - 65535) && w == v[s];
+            stop[s] = simt::ballot(FULL, !valid[s] || hit);
+        }
+        int f = stop[0] ? simt::ffs(stop[0]) - 1 : 32;
+        if (W == 2 && !stop[0]) f = stop[W - 1] ? 32 + simt::ffs(stop[W - 1]) - 1 : 64;
+        // commit the table writes of the serial iterations that really happened (index <= f), last writer per bucket
+        uint32_t cmask[W];
+#pragma unroll
+        for (int u = 0; u < W; u++) {
+            const int fu = f - 32 * u;
+            cmask[u] = fu < 0 ? 0u : (fu >= 31 ? vmask[u] : (vmask[u] & ((2u << fu) - 1u)));
+        }
+#pragma unroll
+        for (int s = 0; s < W; s++) {
+            uint32_t later = same[s][s] & cmask[s] & ~((2u << lane) - 1u);
+            if (s == 0 && W == 2) later |= same[0][W - 1] & cmask[W - 1];
+            if (valid[s] && ((cmask[s] >> lane) & 1u) && !later) T.put(h[s], pos[s]);
+        }
+        simt::syncwarp(FULL);
+        o.f = f;
+        if (f < 32 * W) {
+            const bool hi = W == 2 && f >= 32;
+            if (!((cmask[hi ? W - 1 : 0] >> (f & 31)) & 1u)) o.finished = true;
+            else {
+                o.ip = (int)simt::shfl(FULL, (uint32_t)(hi ? pos[W - 1] : pos[0]), f & 31);
+                o.ref = (int)simt::shfl(FULL, (uint32_t)(hi ? cand[W - 1] : cand[0]), f & 31);
+            }
+        }
+        ENC_PROF_EVENT(EP_EXACT);
+        ENC_PROF_LAP(EP_C_EXACT, tp);
         return o;
     }
 }
@@ -251,6 +288,9 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
     constexpr uint32_t FULL = 0xFFFFFFFFu;
     const int mflimit = n - 12, matchlimit = n - 5;                // :361,:366 / :590,:596
     const uint32_t lt_mask = (1u << lane) - 1u;
+    ENC_PROF_T0(tb);
+    ENC_PROF_T0(tp);
+    ENC_PROF_EVENT(EP_BLOCK);
     InWords in; in.init(src);
     EncTable<GENERAL> T; T.bind(table);
 
@@ -262,6 +302,7 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
     const uint64_t spol = LDP == 1 ? simt::l2_policy_stream() : 0;
     auto st8 = [&](uint8_t* p, uint32_t v) { if (LDP == 1) simt::stg_hint_u8(p, v, spol); else simt::stg_u8(p, (uint8_t)v); };
     auto flush = [&]() -> bool {
+        ENC_PROF_EVENT(EP_FLUSH);
         const bool act = lane < q;
         const int L = sq_L, M = sq_M;
         const bool last = (sq_off & SEQ_LAST) != 0, nochk = (sq_off & SEQ_NOCHK) != 0;
@@ -326,17 +367,20 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
                 for (int i = s; i < s + 4 && i < q; i++) {
                     const uint8_t* const sp = src + (int)simt::shfl(FULL, (uint32_t)sq_anchor, i);
                     uint8_t* const dp = dst + (int)simt::shfl(FULL, (uint32_t)litpos, i);
+                    ENC_PROF_EVENT(EP_LONG_LIT);
                     copy_long_literals(dp, sp, simt::shfl(FULL, (uint32_t)Lq, i), lane);
                 }
             }
         }
         op += (int)simt::shfl(FULL, (uint32_t)incl, 31);
         q = 0;
+        ENC_PROF_LAP(EP_C_EMIT, tp);
         return true;
     };
 
     for (int i = lane; i < 1024; i += 32) ((uint4*)table)[i] = uint4{0, 0, 0, 0};
     simt::syncwarp(FULL);
+    ENC_PROF_RESTART(tp);
 
     int anchor = 0;
     if (n >= 13) {                                                 // :387 / :615 (MINLENGTH)
@@ -372,19 +416,20 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
                 simt::syncwarp(FULL);
                 if ((!GENERAL || t > mp - 65536) && w == vi) { ip = mp; ref = t; again = true; have = true; }
                 else { org = mp + 1 - 3; A0 = 67; fused = false; wide = false; pre = false; }
+                ENC_PROF_EVENT(EP_PROBE);
+                ENC_PROF_EVENT_IF(EP_PROBE_HIT, have);
+                ENC_PROF_LAP(EP_C_PROBE, tp);
             }
             while (!have) {
                 RoundOut r;
-                int consumed;
                 const bool w2 = wide && DUP == 2;
-                consumed = w2 ? 64 : 32;
+                const int consumed = w2 ? 64 : 32;
                 // step 1 up to attempt 128 (and 2 for attempt 128 itself), everything inside the block?
                 const bool simple = A0 + (uint32_t)consumed - 1u <= 128u && org + (int)A0 - 64 + consumed + 1 <= mflimit;
                 if (w2) r = simple ? find_round<GENERAL, 2, DUP, LDP, true>(T, in, org, A0, fused, mflimit, lane, lt_mask)
                                    : find_round<GENERAL, 2, DUP, LDP, false>(T, in, org, A0, fused, mflimit, lane, lt_mask);
                 else    r = simple ? find_round<GENERAL, 1, DUP, LDP, true>(T, in, org, A0, fused, mflimit, lane, lt_mask)
                                    : find_round<GENERAL, 1, DUP, LDP, false>(T, in, org, A0, fused, mflimit, lane, lt_mask);
-                if (r.f < 0) { r.f = 32; consumed = 32; }           // exact path: only the first 32 iterations were evaluated
                 if (r.f >= consumed) {                              // no hit: the find-match loop goes on
                     A0 += (uint32_t)consumed; fused = false; wide = true;
                     if (tune.pf_dist != 0) {                        // incompressible stretch: fetch what the round after next will read
@@ -398,6 +443,7 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
                 ip = r.ip; ref = r.ref; have = true;
                 again = fused && r.f == 1;                          // zero-literal sequence (:531 / :751)
             }
+            ENC_PROF_RESTART(tp);                                   // (the rounds count their own cycles)
             if (finished) break;
 
             // ---------------- catch up (:432 / :657) and count the match (:475-494 / :701-716): all loads first -------
@@ -421,6 +467,7 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
                         ip -= c; ref -= c;
                     }
                 }
+                ENC_PROF_LAP(EP_C_CATCHUP, tp);
                 const uint32_t x = InWords::word(ra) ^ InWords::word(rr);
                 cnt = x ? (simt::ffs(x) - 1) >> 3 : 4;
                 if (cnt > room) cnt = room;
@@ -452,12 +499,15 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
                 const int pl = simt::ffs(part) - 1;
                 mp += 4 * pl + (int)simt::shfl(FULL, (uint32_t)cnt, pl);
             }
+            ENC_PROF_LAP(EP_C_COUNT, tp);
             // ---------------- park the sequence ----------------
             const int L = ip - anchor;
             if (lane == q) {
                 sq_anchor = anchor; sq_L = L; sq_M = mp - (ip + 4);
                 sq_off = (uint32_t)(ip - ref) | (again ? SEQ_NOCHK : 0u);
             }
+            ENC_PROF_EVENT(EP_SEQ);
+            ENC_PROF_LAP(EP_C_PARK, tp);
             if (++q == 32 && !flush()) return 0;
             anchor = mp;
             if (mp > mflimit) break;                                // :516 / :736
@@ -472,13 +522,17 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
             probe_first = L < tune.probe_max;
             org = mp - 2; A0 = 65; fused = true;
             wide = L >= tune.wide_min;                                      // long literal runs: the next match is probably > 30 bytes away
+            ENC_PROF_LAP(EP_C_PARK, tp);
         }
     }
 
     // ---------------- last literals (:540-551 / :760-767) ----------------
     if (lane == q) { sq_anchor = anchor; sq_L = n - anchor; sq_off = SEQ_LAST; sq_M = 0; }
     ++q;
+    ENC_PROF_EVENT(EP_SEQ);
+    ENC_PROF_RESTART(tp);
     if (!flush()) return 0;
+    ENC_PROF_LAP(EP_C_BLOCK, tb);
     return op;
 }
 
