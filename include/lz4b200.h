@@ -78,6 +78,30 @@ int lz4b200_decode_batch(lz4b200_ctx* ctx,
                          void* dst, const int64_t* dst_off, const int32_t* dst_cap,
                          int32_t* out_len, int32_t n_blocks, int known_len, int mem, void* stream);
 
+/* ---- decoded sizes without decoding, and a decode whose output the library sizes itself ---------------------------
+ * Raw LZ4 blocks do not store their decoded size (lz4net's LZ4Codec.Decode(..., knownOutputLength: false) leaves the
+ * capacity to the caller).  The decoders' accept / reject decisions depend on the stream's structure alone, so a pass
+ * over the headers that skips the payload predicts their result exactly, and validates a batch before any output
+ * buffer is committed.
+ *
+ * measure_batch: out_len[i] = what lz4b200_decode_batch (same arguments) would store; nothing is decoded or written.
+ *   Non-negative values are equal, negative ones agree in sign.  dst_cap may be NULL when known_len == 0 (capacity
+ *   INT32_MAX per block; LZ4B200_E_ARG otherwise).  MEM_DEVICE: asynchronous on `stream`; MEM_HOST: synchronous. */
+int lz4b200_measure_batch(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                          const int32_t* dst_cap, int32_t* out_len, int32_t n_blocks, int known_len, int mem, void* stream);
+
+/* decode_batch_packed (device memory only, asynchronous on `stream`, no host synchronisation): unknown-size decode into
+ * PACKED output.  Every block is measured (capacity INT32_MAX); out_off[0..n] (int64, n_blocks+1 entries) = exclusive
+ * prefix sum of max(size, 0), out_off[n] the total.  If out_off[n] <= dst_total_cap, block i is decoded to
+ * dst + out_off[i] with capacity = its measured size and out_len[i] is the decoder's result (a malformed block reports a
+ * negative value and occupies no bytes).  Otherwise dst is not touched and out_len[i] holds the measured sizes: allocate
+ * out_off[n] bytes and call again.
+ * There is no host-memory form: the host pipeline sizes its chunks by decoded bytes, which this call learns only on the
+ * device.  Host callers use lz4b200_measure_batch, then lz4b200_decode_batch. */
+int lz4b200_decode_batch_packed(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n_blocks,
+                                void* stream);
+
 /* Host-memory encode with PACKED output: block i's compressed bytes land at dst + out_off[i] (out_off has n_blocks+1
  * entries; out_off[n_blocks] = total bytes written <= dst_total_cap), back to back in block order -- the layout the
  * LZ4Stream chunk writer (src/LZ4/LZ4Stream.cs:262-266) and any transport want, and the one that moves only compLen

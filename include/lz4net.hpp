@@ -66,6 +66,16 @@ public:
     ~Context() { lz4b200_destroy(h_); }
     Context(const Context&) = delete; Context& operator=(const Context&) = delete;
     lz4b200_ctx* handle() const { return h_; }
+    // What a host-memory decode of these blocks would return per block (bytes written; with known sizes: bytes read), without
+    // decoding.  dst_cap may be null for unknown sizes: no limit.
+    std::vector<int32_t> measure(const uint8_t* src, const int64_t* src_off, const int32_t* src_len, const int32_t* dst_cap,
+                                 int32_t n, bool known = false)
+    {
+        std::vector<int32_t> out((size_t)std::max(n, 0));
+        if (lz4b200_measure_batch(h_, src, src_off, src_len, dst_cap, out.data(), n, known ? 1 : 0, LZ4B200_MEM_HOST, nullptr) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+        return out;
+    }
 private:
     lz4b200_ctx* h_ = nullptr;
 };

@@ -50,6 +50,12 @@ namespace LZ4
         private static extern unsafe int lz4b200_decode_batch(IntPtr ctx, byte* src, long* srcOff, int* srcLen, byte* dst, long* dstOff,
                                                               int* dstCap, int* outLen, int nBlocks, int knownLen, int mem, IntPtr stream);
         [DllImport(Library, CallingConvention = CallingConvention.Cdecl)]
+        private static extern unsafe int lz4b200_measure_batch(IntPtr ctx, byte* src, long* srcOff, int* srcLen, int* dstCap, int* outLen,
+                                                               int nBlocks, int knownLen, int mem, IntPtr stream);
+        [DllImport(Library, CallingConvention = CallingConvention.Cdecl)]
+        private static extern unsafe int lz4b200_decode_batch_packed(IntPtr ctx, byte* src, long* srcOff, int* srcLen, byte* dst,
+                                                                     long dstTotalCap, long* outOff, int* outLen, int nBlocks, IntPtr stream);
+        [DllImport(Library, CallingConvention = CallingConvention.Cdecl)]
         private static extern unsafe int lz4b200_wrap_batch(IntPtr ctx, byte* src, long* srcOff, int* srcLen, int highCompression,
                                                             byte* dst, long* dstOff, int* dstCap, int* outLen, int n);
 
@@ -101,6 +107,20 @@ namespace LZ4
             for (var i = 0; i < n; i++)
                 if (consumed[i] != inputLengths[i])
                     throw new ArgumentException("LZ4 block is corrupted, or invalid length has been given.");
+        }
+
+        /// <summary>The decoded size of each of n raw LZ4 blocks (input[inputOffsets[i], +inputLengths[i])) without decoding them:
+        /// sizes[i] is what <see cref="Decode(byte[],int,int,byte[],int,int,bool)"/> with knownOutputLength = false and an
+        /// unlimited output would return, or a negative value for a corrupt block.  Allocate, then decode with exact sizes.</summary>
+        public static unsafe void MeasureBlocks(byte[] input, long[] inputOffsets, int[] inputLengths, int[] sizes)
+        {
+            var n = inputOffsets.Length;
+            if (inputLengths.Length < n || sizes.Length < n) throw new ArgumentException("length arrays too small");
+            fixed (byte* src = input) fixed (long* so = inputOffsets) fixed (int* sl = inputLengths) fixed (int* ol = sizes)
+            {
+                var rc = lz4b200_measure_batch(CudaContext(), src, so, sl, null, ol, n, 0, 0, IntPtr.Zero);
+                if (rc != 0) throw new InvalidOperationException("lz4b200_measure_batch failed: " + rc);
+            }
         }
 
         #endregion

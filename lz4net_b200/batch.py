@@ -45,6 +45,22 @@ def decode(ctx: Context, comp: torch.Tensor, src_off, src_len, out: torch.Tensor
                          src_off.numel(), known=known, device=True, stream=_stream())
 
 
+def measure(ctx: Context, comp: torch.Tensor, src_off, src_len, out_len, dst_cap=None, known: bool = False):
+    """out_len[i] = what decode(..., dst_cap, out_len, known) would store, without decoding; dst_cap=None (unknown size only)
+    = no limit.  Asynchronous on the current torch stream."""
+    ctx.measure_batch_ptr(_p(comp), _p(src_off), _p(src_len), _p(dst_cap) if dst_cap is not None else None, _p(out_len),
+                          src_off.numel(), known=known, device=True, stream=_stream())
+
+
+def decode_packed(ctx: Context, comp: torch.Tensor, src_off, src_len, out: torch.Tensor, out_off, out_len):
+    """Unknown-size decode into packed output (lz4b200_decode_batch_packed): block i lands at out + out_off[i] (int64[n+1],
+    out_off[n] = the total) when the total fits out.numel() bytes; otherwise out is untouched and out_len holds the sizes.
+    Asynchronous on the current torch stream: read out_off[n] after a synchronise to learn which happened."""
+    native.check(native.lib().lz4b200_decode_batch_packed(ctx.handle, _p(comp), _p(src_off), _p(src_len), _p(out), out.numel(),
+                                                          _p(out_off), _p(out_len), src_off.numel(), _stream()),
+                 "decode_batch_packed")
+
+
 def compact(ctx: Context, slots: torch.Tensor, slot_off, lens, packed, out_off):
     """out_off: int64[n+1]; packed may be None to compute only the offsets."""
     native.check(native.lib().lz4b200_compact(ctx.handle, _p(slots), _p(slot_off), _p(lens),

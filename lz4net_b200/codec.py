@@ -83,6 +83,10 @@ class Context:
                                                        1 if known else 0,
                                                        native.MEM_DEVICE if device else native.MEM_HOST, stream), "decode_batch")
 
+    def measure_batch_ptr(self, src, src_off, src_len, dst_cap, out_len, n, known=False, device=True, stream=0):
+        native.check(native.lib().lz4b200_measure_batch(self._h, src, src_off, src_len, dst_cap, out_len, int(n), 1 if known else 0,
+                                                        native.MEM_DEVICE if device else native.MEM_HOST, stream), "measure_batch")
+
     def encode_batch_packed_ptr(self, src, src_off, src_len, dst_cap, dst, dst_total_cap, out_off, out_len, n, hc=False):
         native.check(native.lib().lz4b200_encode_batch_packed(self._h, src, src_off, src_len, dst_cap, dst, int(dst_total_cap),
                                                               out_off, out_len, int(n),
@@ -131,6 +135,20 @@ class Context:
             m = int(c) if known else max(int(r), 0)
             outs.append(dst[int(o):int(o) + m].tobytes())
         return res, outs
+
+    def measure_blocks(self, blocks, caps=None, known=False):
+        """What decode_blocks(blocks, caps, known) would return as out_len, without decoding: one host-memory batch call.
+        caps=None (unknown size only): no limit on the decoded size (INT32_MAX per block)."""
+        if caps is None and known:
+            raise ValueError("known-size measuring needs the decoded sizes (caps)")
+        n = len(blocks)
+        src, lens, src_off = _pack(blocks)
+        caps = None if caps is None else np.array(caps, np.int32)
+        out = np.zeros(n, np.int32)
+        if n:
+            self.measure_batch_ptr(src.ctypes.data, src_off.ctypes.data, lens.ctypes.data, None if caps is None else caps.ctypes.data,
+                                   out.ctypes.data, n, known=known, device=False)
+        return out.tolist()
 
     # ---- framing ----------------------------------------------------------------------------------------------
     def stream_encode(self, data: bytes, block_size: int = 1 << 20, high_compression: bool = False) -> bytes:

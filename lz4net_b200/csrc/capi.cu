@@ -1,6 +1,6 @@
 // capi.cu -- the C ABI of liblz4b200.so (include/lz4b200.h): context, batched entry points, single-block entry points.
 //
-// Every call on host memory (the batches with LZ4B200_MEM_HOST, the packed encode, the single-block entry points and the
+// Every call on host memory (the batches with LZ4B200_MEM_HOST, the packed encode, the measure pass, the single-block entry points and the
 // framing in framing.cpp) goes through one software pipeline, run_host: the block list is cut into chunks, and for each
 // chunk H2D(inputs) -> kernel -> D2H(outputs) is enqueued on one of NSLOT streams, so that the copy engines (both PCIe
 // directions) and the SMs work on different chunks at the same time.  There is no CPU codec in this library: if the
@@ -118,6 +118,7 @@ struct lz4b200_ctx {
     uint32_t* counters = nullptr;
     int next_counter = 0;
     DevBuf hc_arena, compact_tmp;
+    DevBuf packed_caps;                    // lz4b200_decode_batch_packed: per-block capacities + the "fits" flag (serialised like compact_tmp)
     cudaEvent_t hc_done = nullptr;         // the HC state arena is shared: HC launches are chained through this event
     cudaEvent_t compact_done = nullptr;    // likewise the scan scratch of lz4b200_compact
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
@@ -155,7 +156,8 @@ int lanes_for_ratio(double ratio, int64_t n_blocks, const DeviceInfo& dev)
     return g == 104 && n_blocks >= (int64_t)dev.num_sms * 32 * 8 ? 1 : g;
 }
 
-int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc, 2 dec known, 3 dec unknown*/, cudaStream_t st, int lanes = 0)
+int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc, 2 dec known, 3 dec unknown, 4 / 5 measure known / unknown*/,
+               cudaStream_t st, int lanes = 0)
 {
     if (!lanes && !c->decode_lanes_auto) lanes = c->decode_lanes;       // (0 = auto: the decoder is picked on the device)
     cudaError_t e = cudaSuccess;
@@ -179,7 +181,8 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
         break;
     }
     case 2: e = launch_decode(a, true, lanes, c->counter(), c->dev, st, &c->launches); break;
-    default: e = launch_decode(a, false, lanes, c->counter(), c->dev, st, &c->launches); break;
+    case 3: e = launch_decode(a, false, lanes, c->counter(), c->dev, st, &c->launches); break;
+    default: e = launch_measure(a, op == 4, c->dev, st, &c->launches); break;
     }
     if (e != cudaSuccess) return cuda_fail(e, "kernel launch");
     return LZ4B200_OK;
@@ -188,7 +191,8 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
 // Host-memory batch: chunks of at most host_chunk_bytes (src + dst bytes) go through the slots in turn, and a slot's
 // outputs land in the caller's memory when the slot comes round again, so chunks overlap and land in block order.  On the
 // device the output slots of a chunk are dense: block i starts at the sum of dst_cap over the earlier blocks of its
-// chunk, so slots adjacent in dst are adjacent there too.
+// chunk, so slots adjacent in dst are adjacent there too.  The measure pass (op 4 / 5) has no output: its chunks are
+// weighed by src_len alone, dst_cap may be null (INT32_MAX per block), and only out_len comes back (NONE).
 // Only bytes a block PRODUCED ever reach the caller's buffer (the reference's safe codec leaves everything behind the
 // return value untouched, its native ones spill at most 7 bytes).  A chunk's outputs land in one of four ways:
 //  PER_BLOCK  chunks of at most 8 blocks: one copy per block to dst + dst_off[i];
@@ -202,10 +206,11 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
              const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op,
              int64_t* out_off, int64_t dst_total_cap)
 {
+    const bool measure = op >= 4;
     for (int32_t i = 0; i < n; i++)
-        if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
-    const bool src_pageable = is_pageable(src), dst_pageable = is_pageable(dst);
-    enum Mode { PER_BLOCK, RUNS, SCATTER, APPEND };
+        if (src_len[i] < 0 || (dst_cap && dst_cap[i] < 0)) return fail(LZ4B200_E_ARG, "negative block length");
+    const bool src_pageable = is_pageable(src), dst_pageable = !measure && is_pageable(dst);
+    enum Mode { NONE, PER_BLOCK, RUNS, SCATTER, APPEND };
     struct Pending { int32_t b0, b1; Mode mode; };
     Pending pend[NSLOT]; bool busy[NSLOT] = {false, false, false};
     int32_t b0 = 0; int k = 0; int64_t written = 0;
@@ -278,7 +283,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         // ---- pick the chunk [b0, b1): bounded src + dst bytes ----
         int64_t bytes = 0; int32_t b1 = b0;
         while (b1 < n) {
-            const int64_t w = (int64_t)src_len[b1] + dst_cap[b1];
+            const int64_t w = (int64_t)src_len[b1] + (measure ? 0 : dst_cap[b1]);
             if (b1 > b0 && bytes + w > (int64_t)c->host_chunk_bytes) break;
             bytes += w; b1++;
         }
@@ -286,14 +291,14 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         int rc = retire(s); if (rc) return rc;
         Slot& sl = c->slot[s];
         const int32_t m = b1 - b0;
-        const Mode mode = !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == 2 ? RUNS : SCATTER;
+        const Mode mode = measure ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == 2 ? RUNS : SCATTER;
         CU(sl.meta.reserve((size_t)m * 28)); CU(sl.hmeta.reserve((size_t)m * 28 + sizeof(int64_t) * (size_t)(m + 2)));
         const Meta h(sl.hmeta.p, m), d(sl.meta.p, m);
         int64_t slo = INT64_MAX, shi = INT64_MIN, dsum = 0;
         for (int32_t i = b0; i < b1; i++) { slo = std::min(slo, src_off[i]); shi = std::max(shi, src_off[i] + src_len[i]); }
         for (int32_t i = 0; i < m; i++) {
-            h.so[i] = src_off[b0 + i] - slo; h.dof[i] = dsum; dsum += dst_cap[b0 + i];
-            h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap[b0 + i];
+            h.so[i] = src_off[b0 + i] - slo; h.dof[i] = dsum; dsum += measure ? 0 : dst_cap[b0 + i];
+            h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap ? dst_cap[b0 + i] : INT32_MAX;
         }
         const size_t sbytes = (size_t)(shi - slo);
         CU(sl.src.reserve(sbytes + 64)); CU(sl.dst.reserve((size_t)dsum + 64));
@@ -305,7 +310,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         }
         const BatchArgs a{(const uint8_t*)sl.src.p, d.so, d.sl, (uint8_t*)sl.dst.p, d.dof, d.dc, d.out, m};
         int lanes = 0;
-        if (op >= 2 && c->decode_lanes_auto) {
+        if ((op == 2 || op == 3) && c->decode_lanes_auto) {
             double cs = 0, rs = 0;
             for (int32_t i = b0; i < b1; i++) { cs += src_len[i]; rs += dst_cap[i]; }
             lanes = lanes_for_ratio(rs > 0 ? cs / rs : 1.0, m, c->dev);
@@ -338,7 +343,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
 }
 
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
-// packed host encode (lz4b200_encode_batch_packed).
+// packed host encode (lz4b200_encode_batch_packed); the measure pass (op 4 / 5) has no dst, dst_off or out_off.
 int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
           const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op, int mem, void* stream,
           int64_t* out_off = nullptr, int64_t dst_total_cap = 0)
@@ -346,7 +351,9 @@ int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0) return fail(LZ4B200_E_ARG, "negative block count");
     if (n == 0) return LZ4B200_OK;
-    if (!src_off || !src_len || !(dst_off || out_off) || !dst_cap || !out_len || !src || !dst) return fail(LZ4B200_E_ARG, "null argument");
+    const bool measure = op >= 4;
+    if (!src_off || !src_len || !out_len || !src || (!measure && (!(dst_off || out_off) || !dst_cap || !dst)))
+        return fail(LZ4B200_E_ARG, "null argument");
     std::lock_guard<std::mutex> lock(c->mu);
     DeviceGuard g(c->device);
     if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
@@ -449,7 +456,7 @@ void lz4b200_destroy(lz4b200_ctx* c)
         if (s.done) cudaEventDestroy(s.done);
         if (s.stream) cudaStreamDestroy(s.stream);
     }
-    c->hc_arena.release(); c->compact_tmp.release();
+    c->hc_arena.release(); c->compact_tmp.release(); c->packed_caps.release();
     if (c->hc_done) cudaEventDestroy(c->hc_done);
     if (c->compact_done) cudaEventDestroy(c->compact_done);
     if (c->counters) cudaFree(c->counters);
@@ -487,6 +494,48 @@ int lz4b200_decode_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off
                          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int known_len, int mem, void* stream)
 {
     return batch(c, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, known_len ? 2 : 3, mem, stream);
+}
+
+int lz4b200_measure_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, const int32_t* dst_cap,
+                          int32_t* out_len, int32_t n, int known_len, int mem, void* stream)
+{
+    if (known_len && !dst_cap) return fail(LZ4B200_E_ARG, "dst_cap may be NULL only when known_len == 0");
+    return batch(c, src, src_off, src_len, nullptr, nullptr, dst_cap, out_len, n, known_len ? 4 : 5, mem, stream);
+}
+
+// measure -> scan -> capacities + "fits" -> decode, all enqueued on `stream`: the decoders leave at once (pick gate)
+// when the total does not fit, so out_len keeps the measured sizes and dst is untouched.
+int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n, void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    std::lock_guard<std::mutex> lock(c->mu);
+    DeviceGuard g(c->device);
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
+    if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
+    const size_t caps_bytes = sizeof(int32_t) * ((size_t)n + 1);
+    if (compact_tmp_bytes(n) > c->compact_tmp.cap || caps_bytes > c->packed_caps.cap) {
+        CU(cudaDeviceSynchronize());               // both scratch buffers may still be in use by an earlier call
+        CU(c->compact_tmp.reserve(compact_tmp_bytes(n))); CU(c->packed_caps.reserve(caps_bytes));
+    }
+    // the scan scratch and the capacities are the context's: calls on different streams are serialised on them
+    CU(cudaStreamWaitEvent(st, c->compact_done, 0));
+    int32_t* caps = (int32_t*)c->packed_caps.p;
+    int* fits = (int*)(caps + n);
+    const BatchArgs m{(const uint8_t*)src, src_off, src_len, nullptr, nullptr, nullptr, out_len, n};
+    cudaError_t e = launch_measure(m, false, c->dev, st, &c->launches);
+    if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, out_len, nullptr, out_off, n, c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
+    if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, caps, fits, st, &c->launches);
+    if (e == cudaSuccess) {
+        const BatchArgs d{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, caps, out_len, n};
+        e = launch_decode(d, false, c->decode_lanes_auto ? 0 : c->decode_lanes, c->counter(), c->dev, st, &c->launches, fits);
+    }
+    if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
+    CU(cudaEventRecord(c->compact_done, st));
+    return LZ4B200_OK;
 }
 
 int lz4b200_compact(lz4b200_ctx* c, const void* slots, const int64_t* slot_off, const int32_t* len, void* packed,

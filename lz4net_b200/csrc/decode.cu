@@ -2,6 +2,7 @@
 #include "kernels.h"
 #include "lz4_decode.cuh"
 #include "lz4_decode_lpb.cuh"
+#include "lz4_measure.cuh"
 
 namespace lz4b200 {
 
@@ -54,7 +55,10 @@ lz4_decode_kernel(BatchArgs a, uint32_t* counter, const int* pick, int code)
 // the first blocks of the batch -> the same rule as lanes_for_ratio() on the host (capi.cu, tools/sweep.py): incompressible
 // data is long literal runs (whole warps, 128-bit copies), nearly-empty streams are long matches, everything between is
 // sequence-dense (the denser, the smaller the group; both output-staged).
-__global__ void __launch_bounds__(256) lz4_decode_pick_kernel(const int32_t* src_len, const int32_t* dst_cap, int32_t n, int* pick)
+// gate (may be null): a device flag; 0 makes the pick 0, which no decoder kernel answers to (the packed decode when its
+// output does not fit).  fixed != 0: the code of the one kernel a pinned decode_lanes setting launched.
+__global__ void __launch_bounds__(256) lz4_decode_pick_kernel(const int32_t* src_len, const int32_t* dst_cap, int32_t n, int* pick,
+                                                              const int* gate, int fixed)
 {
     __shared__ unsigned long long sc[8], sr[8];
     unsigned long long c = 0, r = 0;
@@ -67,7 +71,7 @@ __global__ void __launch_bounds__(256) lz4_decode_pick_kernel(const int32_t* src
         c = r = 0;
         for (int i = 0; i < 8; i++) { c += sc[i]; r += sr[i]; }
         const double ratio = r ? (double)c / (double)r : 1.0;
-        *pick = decode_lanes_for_ratio(ratio);
+        *pick = gate && !*gate ? 0 : (fixed ? fixed : decode_lanes_for_ratio(ratio));
     }
 }
 
@@ -150,16 +154,31 @@ static cudaError_t launch_lpb(const BatchArgs& a, uint32_t* counter, const Devic
 }
 
 cudaError_t launch_decode(const BatchArgs& a, bool known_len, int lanes, uint32_t* counter,
-                          const DeviceInfo& dev, cudaStream_t stream, int64_t* launches)
+                          const DeviceInfo& dev, cudaStream_t stream, int64_t* launches, const int* gate)
 {
     if (a.n_blocks <= 0) return cudaSuccess;
     cudaError_t e = cudaMemsetAsync(counter, 0, 4 * sizeof(uint32_t), stream);     // [block counter, decoder pick, two more block counters]
     if (e != cudaSuccess) return e;
     if (launches) ++*launches;
+    int* pick = (int*)(counter + 1);                 // (the context hands out counters in fours: [block counter, pick, two more counters])
+    if (lanes != 0 && gate) {
+        // a pinned decoder behind a gate: the pick kernel passes the gate on as that kernel's code (or 0)
+        const int code = lanes == 1 ? 104 : lanes;
+        lz4_decode_pick_kernel<<<1, 256, 0, stream>>>(a.src_len, a.dst_cap, a.n_blocks, pick, gate, code);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+        if (launches) ++*launches;
+        const bool staged = lanes >= 100;
+        switch (lanes % 100) {
+        case 1:  return known_len ? launch_lpb<true, LpbDefault>(a, counter, dev, stream, pick, 0) : launch_lpb<false, LpbDefault>(a, counter, dev, stream, pick, 0);
+        case 4:  return launch_g<4>(a, known_len, staged, counter, dev, stream, pick, code);
+        case 8:  return launch_g<8>(a, known_len, staged, counter, dev, stream, pick, code);
+        case 16: return launch_g<16>(a, known_len, staged, counter, dev, stream, pick, code);
+        default: return launch_g<32>(a, known_len, staged, counter, dev, stream, pick, code);
+        }
+    }
     if (lanes == 0) {
         // auto: pick on the device, enqueue the four candidates (three of them return at once)
-        int* pick = (int*)(counter + 1);             // (the context hands out counters in fours: [block counter, pick, two more counters])
-        lz4_decode_pick_kernel<<<1, 256, 0, stream>>>(a.src_len, a.dst_cap, a.n_blocks, pick);
+        lz4_decode_pick_kernel<<<1, 256, 0, stream>>>(a.src_len, a.dst_cap, a.n_blocks, pick, gate, 0);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
         if (launches) *launches += 2;
         if ((e = launch_g<32>(a, known_len, false, counter, dev, stream, pick, 32)) != cudaSuccess) return e;
@@ -192,6 +211,48 @@ cudaError_t launch_decode(const BatchArgs& a, bool known_len, int lanes, uint32_
     case 16: return launch_g<16>(a, known_len, staged, counter, dev, stream);
     default: return launch_g<32>(a, known_len, staged, counter, dev, stream);
     }
+}
+
+// ---- measure pass (lz4_measure.cuh): one thread per block, no shared memory ---------------------------------------------
+constexpr int MEASURE_THREADS = 128;
+
+template <bool KNOWN>
+__global__ void __launch_bounds__(MEASURE_THREADS)
+lz4_measure_kernel(BatchArgs a)
+{
+    const int64_t i = (int64_t)blockIdx.x * MEASURE_THREADS + threadIdx.x;
+    if (i >= a.n_blocks) return;
+    const int cap = a.dst_cap ? a.dst_cap[i] : 0x7FFFFFFF;          // no capacities: INT32_MAX for every block
+    a.out_len[i] = measure_block<KNOWN>(a.src + a.src_off[i], a.src_len[i], cap);
+}
+
+cudaError_t launch_measure(const BatchArgs& a, bool known_len, const DeviceInfo&, cudaStream_t stream, int64_t* launches)
+{
+    if (a.n_blocks <= 0) return cudaSuccess;
+    const unsigned grid = (unsigned)(((int64_t)a.n_blocks + MEASURE_THREADS - 1) / MEASURE_THREADS);
+    if (known_len) lz4_measure_kernel<true><<<grid, MEASURE_THREADS, 0, stream>>>(a);
+    else           lz4_measure_kernel<false><<<grid, MEASURE_THREADS, 0, stream>>>(a);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+// Between the scan and the decode of lz4b200_decode_batch_packed: block i's capacity is its measured size (0 for a
+// malformed block: the decoder rejects it without writing a byte), and *fits = whether the total fits the destination.
+__global__ void __launch_bounds__(256) lz4_packed_prep_kernel(const int32_t* size, const int64_t* out_off, int32_t n,
+                                                              int64_t total_cap, int32_t* cap, int* fits)
+{
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i < n) cap[i] = size[i] > 0 ? size[i] : 0;
+    if (i == 0) *fits = out_off[n] <= total_cap;
+}
+
+cudaError_t launch_packed_prep(const int32_t* size, const int64_t* out_off, int32_t n, int64_t total_cap, int32_t* cap, int* fits,
+                               cudaStream_t stream, int64_t* launches)
+{
+    if (n <= 0) return cudaSuccess;
+    lz4_packed_prep_kernel<<<(unsigned)(((int64_t)n + 255) / 256), 256, 0, stream>>>(size, out_off, n, total_cap, cap, fits);
+    if (launches) ++*launches;
+    return cudaGetLastError();
 }
 
 }  // namespace lz4b200

@@ -18,8 +18,15 @@ struct DeviceInfo { int num_sms; int smem_per_sm; int smem_optin; };
 // lanes_per_block: 32 | 16 | 8 | 4 (+100 = output-staged), 1 | 2 = the lane-per-block decoder, 0 = chosen on the device from
 // the batch's compression ratio.  `counter` points at FOUR device words the launcher owns (block counter, pick, two more counters).
 int         decode_lanes_for_ratio(double ratio);
+// gate (optional): a device int; when it reads 0 at run time every decoder kernel of the launch returns at once.
 cudaError_t launch_decode(const BatchArgs& a, bool known_len, int lanes_per_block, uint32_t* counter,
-                          const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
+                          const DeviceInfo& dev, cudaStream_t stream, int64_t* launches, const int* gate = nullptr);
+// out_len[i] = what launch_decode would store for block i, nothing else is written (a.dst / a.dst_off unused; a.dst_cap
+// may be null when !known_len: INT32_MAX for every block).
+cudaError_t launch_measure(const BatchArgs& a, bool known_len, const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
+// cap[i] = max(size[i], 0); *fits = out_off[n] <= total_cap
+cudaError_t launch_packed_prep(const int32_t* size, const int64_t* out_off, int32_t n, int64_t total_cap, int32_t* cap, int* fits,
+                               cudaStream_t stream, int64_t* launches);
 cudaError_t launch_encode_fast(const BatchArgs& a, uint32_t* counter, int warps_per_sm, const int* tune4 /* prefetch, lane_copy_max, probe_max, wide_min */, int variant,
                                const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 size_t      hc_scratch_bytes(int concurrency);
