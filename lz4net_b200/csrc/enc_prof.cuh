@@ -19,16 +19,17 @@ enum EncProfSlot {
     EP_EXACT,                               // rounds on the exact path
     EP_PROBE, EP_PROBE_HIT,                 // post-match probes tried alone, of which hit
     EP_FLUSH, EP_LONG_LIT,                  // EMIT calls, literal runs copied by copy_long_literals
+    EP_CATCHUP_LONG,                        // catch-ups finished by the whole warp (longer than EMIT's per-lane steps)
     // clock64 cycles
     EP_C_LOADHASH,                          // round: positions, input words, hashes, table reads, candidate loads issued
     EP_C_SAMEHASH,                          // round: same-hash resolution through the table
     EP_C_VOTE,                              // round: candidate words, hit vote, final table writes
     EP_C_EXACT,                             // round: exact path
     EP_C_PROBE,                             // post-match probe alone
-    EP_C_CATCHUP,                           // backward catch-up (and the match count's first loads issued)
+    EP_C_CATCHUP,                           // EMIT: backward catch-up of the 32 parked sequences
     EP_C_COUNT,                             // forward match count
     EP_C_PARK,                              // park the record, prefetch, next round's set-up
-    EP_C_EMIT,                              // EMIT: prefix sum, limit checks, token / length stores, literal copy
+    EP_C_EMIT,                              // EMIT after the catch-up: prefix sum, limit checks, token / length stores, literal copy
     EP_C_BLOCK,                             // the whole of encode_block_t, table clear included
     EP_N
 };

@@ -69,6 +69,17 @@ struct InWords {
         return r;
     }
     static SIMT_MEM uint32_t word(const Raw& r) { return simt::funnel_r(r.lo, r.hi, r.sh); }
+    // The 4 bytes [p-4, p) (byte p-1 in the top byte), for the backward catch-up.  The caller passes 1 <= p < n: the word
+    // holding byte p is read when part of it is wanted, the word before it only when that is not the first word of the
+    // block, so no word without an input byte -- and none in front of src -- is ever touched.  Bytes in front of src
+    // come back as zeros (tests/test_encode_deferred_catchup.py::test_catchup_never_reads_before_the_input).
+    SIMT_MEM uint32_t back(int p) const
+    {
+        const uint32_t q = (uint32_t)p + sk, i = q >> 2, sh = (q & 3u) * 8u;
+        const uint32_t lo = i ? simt::ldg_nc_u32(w + i - 1) : 0u;
+        const uint32_t hi = sh ? simt::ldg_nc_u32(w + i) : 0u;
+        return simt::funnel_r(lo, hi, sh);
+    }
 };
 
 // ---- source policies -------------------------------------------------------------------------------------------

@@ -17,11 +17,14 @@
 //     step: they ride in lanes 0 and 1 of the next round ("fused round"), whose remaining 30 lanes are the first 30
 //     iterations of the find-match loop that starts at ip+1.  A hit in lane 1 is the reference's zero-literal
 //     `goto _next_match`;
-//   * the backward catch-up (:657) and the forward match-length count (:701-716) are independent once (ip, ref) are
-//     known: their loads are issued together, before the first vote;
-//   * nothing is written during the parse: each found sequence is one record (anchor, literal length, offset, match
-//     length) parked in the registers of one lane.
+//   * the forward match-length count (:701-716) starts at ip + 4 as the round found it.  The backward catch-up (:657)
+//     is not on this chain: it moves ip and ref back together over matching bytes, so the match end mp, the offset and
+//     everything the next round needs (org = mp - 2, anchor = mp, the mflimit test) are the same without it;
+//   * nothing is written during the parse: each found sequence is one record (anchor, literal length up to the ip the
+//     round found, offset, match length from there) parked in the registers of one lane.
 // EMIT (every 32 sequences, fully lane-parallel):
+//   * catch-up: lane k moves sequence k's split point back, 4 bytes per word compare; the rare catch-ups longer than a
+//     few words finish with the whole warp on one sequence, 32 bytes per step;
 //   * sizes -> warp prefix sum -> every sequence's output position; the reference's output-limit checks (:663, :728,
 //     :762) are evaluated for all 32 sequences at once from those positions;
 //   * lane k writes token, length bytes and offset of sequence k; literal runs are copied by the whole warp, four
@@ -304,8 +307,46 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
     auto flush = [&]() -> bool {
         ENC_PROF_EVENT(EP_FLUSH);
         const bool act = lane < q;
-        const int L = sq_L, M = sq_M;
+        int L = sq_L, M = sq_M;
         const bool last = (sq_off & SEQ_LAST) != 0, nochk = (sq_off & SEQ_NOCHK) != 0;
+        // ---- catch up (:432 / :657), lane k for sequence k.  Parked as found: ip = anchor + L, ref = ip - offset.  Word
+        // compares backwards, 4 bytes per step and lane; the few catch-ups longer than CU_LANE_STEPS words finish with
+        // the whole warp on one sequence at a time, 32 bytes per step.  ip - c >= anchor and ref - c >= 0 bound c.
+        {
+            constexpr int CU_LANE_STEPS = 4;
+            const int ip = sq_anchor + L, ref = ip - (int)(sq_off & 0xFFFFu);
+            const int lim = L < ref ? L : ref;
+            int c = 0;
+            bool go = act && !last && lim > 0;
+#pragma unroll 1
+            for (int s = 0; s < CU_LANE_STEPS && simt::ballot(FULL, go); s++) {
+                if (go) {
+                    const uint32_t x = in.back(ip - c) ^ in.back(ref - c);
+                    const int e = x ? simt::clz(x) >> 3 : 4;
+                    c += e;
+                    go = e == 4 && c < lim;
+                }
+            }
+            for (uint32_t lg = simt::ballot(FULL, go); lg; lg &= lg - 1u) {
+                const int k = simt::ffs(lg) - 1;
+                const int ipk = (int)simt::shfl(FULL, (uint32_t)ip, k), refk = (int)simt::shfl(FULL, (uint32_t)ref, k);
+                const int limk = (int)simt::shfl(FULL, (uint32_t)lim, k);
+                int ck = (int)simt::shfl(FULL, (uint32_t)c, k);
+                ENC_PROF_EVENT(EP_CATCHUP_LONG);
+                for (;;) {
+                    const int j = ck + lane + 1;
+                    const bool eq = j <= limk && simt::ldg_nc_u8(src + (ipk - j)) == simt::ldg_nc_u8(src + (refk - j));
+                    const uint32_t ne = ~simt::ballot(FULL, eq);
+                    const int e = ne ? simt::ffs(ne) - 1 : 32;
+                    ck += e;
+                    if (e < 32) break;
+                }
+                if (lane == k) c = ck;
+            }
+            if (c > lim) c = lim;
+            L -= c; M += c;
+        }
+        ENC_PROF_LAP(EP_C_CATCHUP, tp);
         const int extL = L >= 15 ? 1 + (L - 15) / 255 : 0;
         const int extM = (!last && M >= 15) ? 1 + (M - 15) / 255 : 0;
         const int size = act ? 1 + extL + L + (last ? 0 : 2 + extM) : 0;
@@ -446,28 +487,15 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
             ENC_PROF_RESTART(tp);                                   // (the rounds count their own cycles)
             if (finished) break;
 
-            // ---------------- catch up (:432 / :657) and count the match (:475-494 / :701-716): all loads first -------
+            // ---------------- count the match (:475-494 / :701-716) -------------------------------------------------
+            // The backward catch-up (:657) is left to EMIT: it moves ip and ref back together over bytes that match, so
+            // the match end mp, the offset and everything the next round needs are the same without it.
             int mp = ip + 4, mr = ref + 4;                          // forward cursors
             int cnt;
             {
                 const int a = mp + 4 * lane;
                 int room = matchlimit - a; room = room < 0 ? 0 : (room > 4 ? 4 : room);
                 const InWords::Raw ra = pre ? pre_ra : in.raw<LDP>(room > 0 ? a : 0), rr = pre ? pre_rr : in.raw<LDP>(room > 0 ? mr + 4 * lane : 0);
-                if (ip > anchor) {                                  // (never after a zero-literal probe hit: ip == anchor)
-                    const int k = lane + 1;
-                    const bool okb = ip - k >= anchor && ref - k >= 0;
-                    const uint8_t ba = simt::ldg_nc_u8(src + (okb ? ip - k : 0)), bb = simt::ldg_nc_u8(src + (okb ? ref - k : 0));
-                    const uint32_t ne = ~simt::ballot(FULL, okb && ba == bb);
-                    int c = ne ? simt::ffs(ne) - 1 : 32;
-                    ip -= c; ref -= c;
-                    while (c == 32) {                               // (a catch-up of 32 or more bytes: rare)
-                        const bool eq = ip - k >= anchor && ref - k >= 0 && simt::ldg_nc_u8(src + ip - k) == simt::ldg_nc_u8(src + ref - k);
-                        const uint32_t ne2 = ~simt::ballot(FULL, eq);
-                        c = ne2 ? simt::ffs(ne2) - 1 : 32;
-                        ip -= c; ref -= c;
-                    }
-                }
-                ENC_PROF_LAP(EP_C_CATCHUP, tp);
                 const uint32_t x = InWords::word(ra) ^ InWords::word(rr);
                 cnt = x ? (simt::ffs(x) - 1) >> 3 : 4;
                 if (cnt > room) cnt = room;
@@ -500,7 +528,7 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
                 mp += 4 * pl + (int)simt::shfl(FULL, (uint32_t)cnt, pl);
             }
             ENC_PROF_LAP(EP_C_COUNT, tp);
-            // ---------------- park the sequence ----------------
+            // ---------------- park the sequence, not caught up (EMIT catches it up) ----------------
             const int L = ip - anchor;
             if (lane == q) {
                 sq_anchor = anchor; sq_L = L; sq_M = mp - (ip + 4);
@@ -519,7 +547,7 @@ SIMT_DEV int encode_block_t(void* table, const uint8_t* src, int n, uint8_t* dst
             // What follows a match (:519-534 / :739-755): insert ip-2, probe + insert ip, then the find-match loop from
             // ip+1.  Short literal runs predict another immediate hit: do the probe alone first.  Otherwise all of it
             // is one fused round: attempts 65, 66 = ip-2, ip; 67.. = the loop.  S(66) = 2, so org = mp - 2.
-            probe_first = L < tune.probe_max;
+            probe_first = L < tune.probe_max;                      // (L before the catch-up: at least the emitted one)
             org = mp - 2; A0 = 65; fused = true;
             wide = L >= tune.wide_min;                                      // long literal runs: the next match is probably > 30 bytes away
             ENC_PROF_LAP(EP_C_PARK, tp);

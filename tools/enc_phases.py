@@ -27,7 +27,7 @@ from lz4net_b200 import synth  # noqa: E402
 CSRC = os.path.join(ROOT, "lz4net_b200", "csrc")
 EMU = os.path.join(ROOT, "tests", "simt_emu")
 # the order of enum EncProfSlot
-EVENTS = ["blocks", "seqs", "rounds", "rounds_wide", "exact", "probes", "probe_hits", "flushes", "long_lit"]
+EVENTS = ["blocks", "seqs", "rounds", "rounds_wide", "exact", "probes", "probe_hits", "flushes", "long_lit", "catchup_long"]
 PHASES = ["loadhash", "samehash", "vote", "exact", "probe", "catchup", "count", "park", "emit", "block"]
 BLOCK = 65536
 
