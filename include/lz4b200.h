@@ -180,10 +180,10 @@ int lz4b200_synth_fill(lz4b200_ctx* ctx, void* dst, int64_t n_blocks, int32_t bl
  * "encode_prefetch" (bytes of input kept prefetched ahead of the parse; 0 off, < 0 L2 only), "encode_lane_copy_max" /
  * "encode_probe_max" / "encode_wide_min" (path-selection heuristics of the fast encoder, lz4_encode.cuh EncTune: they
  * never change the emitted bytes), "hc_kernel" (which LZ4HC kernel encodes a batch: -1 = chosen per batch, the default -- at most
- * three blocks per SM: kernel 1, larger batches: kernel 2, batches made mostly of blocks above 64 KiB: kernel 0; 0 = one
- * thread per block, any block size; 1 / 2 = one warp per block on a static index of the block's hash buckets, blocks of at
- * most 64 KiB -- 1 stages the block in shared memory, 2 reads it through L1 -- larger blocks and the rare block whose chains
- * depend on the parse go to kernel 0 inside the same call), "hc_warps_per_sm" (kernels 1 / 2: blocks in flight per SM,
+ * three blocks per SM: kernel 1, larger batches: kernel 2; 0 = one thread per block, any block size; 1 / 2 = one warp per
+ * block: blocks of at most 64 KiB on a static index of the block's hash buckets -- 1 stages the block in shared memory, 2
+ * reads it through L1 -- and larger blocks, with either value, over a sliding 64 KiB window of index segments; the rare
+ * block whose chains depend on the parse goes to kernel 0 inside the same call), "hc_warps_per_sm" (kernels 1 / 2: blocks of at most 64 KiB in flight per SM,
  * 0 = the default: 3 / 32),
  * "hc_concurrency" (kernel 0: blocks in flight), "host_chunk_mb" (bytes per pipeline stage of host-memory batches).
  * Returns LZ4B200_OK or LZ4B200_E_ARG. */

@@ -128,7 +128,7 @@ struct lz4b200_ctx {
     int encode_tune[4] = {512, 12, 8, 24}; // prefetch distance, lane_copy_max, probe_max, wide_min (lz4_encode.cuh EncTune)
     size_t host_chunk_bytes = HOST_CHUNK_BYTES_DEFAULT;
     int hc_concurrency = 131072;         // blocks in flight (one thread each, 256 KiB state: 32 GiB of arena at this default)
-    int hc_kernel = -1;                  // -1: chosen per batch (encode.cu launch_encode_hc_auto); 0: one thread per block (any block size); one warp per block on a static index (blocks <= 64 KiB, the rest is handed to 0): 1 = block staged in shared memory, 2 = nothing in shared memory
+    int hc_kernel = -1;                  // -1: chosen per batch (encode.cu launch_encode_hc_auto); 0: one thread per block (any block size); one warp per block (on a static index for blocks <= 64 KiB, over a sliding 64 KiB window above; what neither describes goes to 0): 1 = block <= 64 KiB staged in shared memory, 2 = nothing in shared memory
     int hc_warps_per_sm = 0;             // warp kernels: blocks in flight per SM (0 = 3 for kernel 1, 32 for kernel 2)
     Slot slot[NSLOT];
     int64_t launches = 0;
@@ -156,26 +156,26 @@ int lanes_for_ratio(double ratio, int64_t n_blocks, const DeviceInfo& dev)
     return g == 104 && n_blocks >= (int64_t)dev.num_sms * 32 * 8 ? 1 : g;
 }
 
+// hc_large: blocks above 64 KiB in an HC batch (-1 = not known: a device-memory batch)
 int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc, 2 dec known, 3 dec unknown, 4 / 5 measure known / unknown*/,
-               cudaStream_t st, int lanes = 0)
+               cudaStream_t st, int lanes = 0, int32_t hc_large = -1)
 {
     if (!lanes && !c->decode_lanes_auto) lanes = c->decode_lanes;       // (0 = auto: the decoder is picked on the device)
     cudaError_t e = cudaSuccess;
     switch (op) {
     case 0: e = launch_encode_fast(a, c->counter(), c->encode_ctas_per_sm, c->encode_tune, c->encode_variant, c->dev, st, &c->launches); break;
     case 1: {
-        // (chosen per batch: the thread kernel only runs for batches of blocks above 64 KiB -- 4 GiB of state at most there)
-        const int conc = (int)std::min<int64_t>(c->hc_kernel < 0 ? std::min(c->hc_concurrency, 16384) : c->hc_concurrency, std::max(a.n_blocks, 1));
-        const size_t need = c->hc_kernel < 0 ? hc_auto_scratch_bytes(a.n_blocks, conc, c->dev)
-                          : (c->hc_kernel ? hcw_scratch_bytes(a.n_blocks, c->hc_kernel, c->hc_warps_per_sm, c->dev) : hc_scratch_bytes(conc));
+        const int conc = (int)std::min<int64_t>(c->hc_concurrency, std::max(a.n_blocks, 1));
+        const size_t need = c->hc_kernel < 0 ? hc_auto_scratch_bytes(a.n_blocks, hc_large, c->dev)
+                          : (c->hc_kernel ? hcw_scratch_bytes(a.n_blocks, hc_large, c->hc_kernel, c->hc_warps_per_sm, c->dev) : hc_scratch_bytes(conc));
         if (need > c->hc_arena.cap) {
             CU(cudaDeviceSynchronize());           // the arena may still be in use by an earlier launch
             CU(c->hc_arena.reserve(need));
         }
         // one arena per context: an HC launch may not overlap the previous one, whatever stream it was given
         CU(cudaStreamWaitEvent(st, c->hc_done, 0));
-        e = c->hc_kernel < 0 ? launch_encode_hc_auto(a, c->hc_arena.p, conc, c->counter(), c->dev, st, &c->launches)
-          : c->hc_kernel ? launch_encode_hcw(a, c->hc_arena.p, c->hc_kernel, c->hc_warps_per_sm, c->counter(), c->dev, st, &c->launches)
+        e = c->hc_kernel < 0 ? launch_encode_hc_auto(a, c->hc_arena.p, hc_large, c->counter(), c->dev, st, &c->launches)
+          : c->hc_kernel ? launch_encode_hcw(a, c->hc_arena.p, c->hc_kernel, c->hc_warps_per_sm, hc_large, c->counter(), c->dev, st, &c->launches)
                               : launch_encode_hc(a, c->hc_arena.p, conc, c->counter(), c->dev, st, &c->launches);
         if (e == cudaSuccess) e = cudaEventRecord(c->hc_done, st);
         break;
@@ -315,7 +315,9 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
             for (int32_t i = b0; i < b1; i++) { cs += src_len[i]; rs += dst_cap[i]; }
             lanes = lanes_for_ratio(rs > 0 ? cs / rs : 1.0, m, c->dev);
         }
-        rc = run_device(c, a, op, sl.stream, lanes); if (rc) return rc;
+        int32_t hc_large = 0;
+        if (op == 1) for (int32_t i = b0; i < b1; i++) hc_large += src_len[i] > 65536;
+        rc = run_device(c, a, op, sl.stream, lanes, hc_large); if (rc) return rc;
         if (mode >= SCATTER) {
             CU(sl.packed.reserve((size_t)dsum + 64)); CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
             cudaError_t e = launch_compact(a.dst, a.dst_off, a.out_len, (uint8_t*)sl.packed.p, (int64_t*)sl.offs.p, m,
@@ -594,7 +596,7 @@ int lz4b200_set_option(lz4b200_ctx* c, const char* key, int64_t value)
         c->hc_arena.release();
         c->hc_concurrency = (int)value;
     }
-    else if (k == "hc_kernel") { if (value < -1 || value > 2) return fail(LZ4B200_E_ARG, "hc_kernel must be -1 (chosen per batch), 0 (thread per block), 1 or 2 (warp per block on a static index: block in shared memory / read through L1)"); c->hc_kernel = (int)value; }
+    else if (k == "hc_kernel") { if (value < -1 || value > 2) return fail(LZ4B200_E_ARG, "hc_kernel must be -1 (chosen per batch), 0 (thread per block), 1 or 2 (warp per block: blocks <= 64 KiB in shared memory / read through L1)"); c->hc_kernel = (int)value; }
     else if (k == "hc_warps_per_sm") { if (value < 0 || value > 32) return fail(LZ4B200_E_ARG, "hc_warps_per_sm must be 0..32"); c->hc_warps_per_sm = (int)value; }
     else if (k == "host_chunk_mb") { if (value < 1 || value > 4096) return fail(LZ4B200_E_ARG, "host_chunk_mb out of range"); c->host_chunk_bytes = (size_t)value << 20; }
     else return fail(LZ4B200_E_ARG, "unknown option");

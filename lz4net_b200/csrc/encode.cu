@@ -3,6 +3,9 @@
 #include "lz4_encode.cuh"
 #include "lz4hc_encode.cuh"
 #include "lz4hc_warp.cuh"
+#include "lz4hc_window.cuh"
+
+#include <algorithm>
 
 namespace lz4b200 {
 
@@ -72,9 +75,8 @@ cudaError_t launch_encode_fast(const BatchArgs& a, uint32_t* counter, int warps_
 constexpr int HC_THREADS = 32;
 
 __global__ void __launch_bounds__(HC_THREADS)
-lz4_encode_hc_kernel(BatchArgs a, uint8_t* arena, uint32_t* counter, const uint32_t* pick)
+lz4_encode_hc_kernel(BatchArgs a, uint8_t* arena, uint32_t* counter)
 {
-    if (pick && *pick != 0u) return;                       // auto mode: the pick kernel chose the warp kernel for this batch
     const size_t slot = (size_t)blockIdx.x * HC_THREADS + threadIdx.x;
     void* state = arena + slot * HC_STATE_BYTES;
     for (;;) {
@@ -90,14 +92,14 @@ size_t hc_scratch_bytes(int concurrency)
     return slots * HC_STATE_BYTES;
 }
 
-static cudaError_t launch_hc_threads(const BatchArgs& a, void* scratch, int concurrency, uint32_t* counter, const uint32_t* pick,
+static cudaError_t launch_hc_threads(const BatchArgs& a, void* scratch, int concurrency, uint32_t* counter,
                                      cudaStream_t stream, int64_t* launches)
 {
     long long ctas = ((long long)concurrency + HC_THREADS - 1) / HC_THREADS;
     long long want = ((long long)a.n_blocks + HC_THREADS - 1) / HC_THREADS;
     if (ctas > want) ctas = want;
     if (ctas < 1) ctas = 1;
-    lz4_encode_hc_kernel<<<(unsigned)ctas, HC_THREADS, 0, stream>>>(a, (uint8_t*)scratch, counter, pick);
+    lz4_encode_hc_kernel<<<(unsigned)ctas, HC_THREADS, 0, stream>>>(a, (uint8_t*)scratch, counter);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
@@ -108,7 +110,7 @@ cudaError_t launch_encode_hc(const BatchArgs& a, void* scratch, int concurrency,
     if (a.n_blocks <= 0) return cudaSuccess;
     cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(uint32_t), stream);
     if (e != cudaSuccess) return e;
-    return launch_hc_threads(a, scratch, concurrency, counter, nullptr, stream, launches);
+    return launch_hc_threads(a, scratch, concurrency, counter, stream, launches);
 }
 
 // ---- HC encoder, blocks <= 64 KiB: one WARP per block on a static index (lz4hc_warp.cuh) -----------------------------
@@ -120,7 +122,7 @@ template <bool SMEM, int MINB>
 __global__ void __launch_bounds__(32, MINB)
 lz4_encode_hcw_kernel(BatchArgs a, uint8_t* arena, uint32_t* counter, const uint32_t* pick)
 {
-    if (pick && *pick == 0u) return;                       // auto mode: the pick kernel chose the thread kernel for this batch
+    if (pick && *pick == 0u) return;                       // (launched with pick = nullptr: the gate is kept only so that these kernels' instructions stay those profiled)
     extern __shared__ __align__(16) uint8_t smem[];
     const simt::smem_ref sm = simt::smem_ref_of(smem);
     void* index = arena + (size_t)blockIdx.x * HCW_INDEX_BYTES;
@@ -133,57 +135,6 @@ lz4_encode_hcw_kernel(BatchArgs a, uint8_t* arena, uint32_t* counter, const uint
         const int r = hcw_encode_block<SMEM>(sm, index, a.src + a.src_off[b], a.src_len[b], a.dst + a.dst_off[b], a.dst_cap[b], lane);
         if (lane == 0) a.out_len[b] = r;
         simt::syncwarp(0xFFFFFFFFu);                       // the next block reuses the shared memory and the index
-    }
-}
-
-// Auto mode, large batches: a sample of the batch (up to 32 blocks, evenly spaced; one CTA each) is looked at on the device.
-// What decides today is the block size alone -- the warp kernel takes blocks of at most 64 KiB and hands the others to a
-// few thousand threads, so a batch made mostly of larger blocks goes to the thread kernel.  The sample's hash-bucket
-// statistic (depth = sum(min(c, 255) * c) / sum(c) = the clamped bucket size an average position sees: E0 3.0, E50 3.9,
-// natural text and code 20 - 66, ETEXT 240) is computed as well: with the warp kernel capped at 8 resident warps per SM by a
-// shared-memory carve-out preference it separated the batches the index paid for (depth >= 8) from those it did not; at its
-// real residency the warp kernel was ahead on every class timed (tools/hc_ab.py compares the kernels), so the threshold is
-// 0 and the statistic is kept for the record only.
-// words: [0] block counter of the codec kernels (used as the ticket here and left zero), [1] pick (0 thread kernel,
-// 2 warp kernel), [2] sum(c), [3] sum(min(c,255)*c) / 16.
-constexpr int HC_PICK_SAMPLE = 32;
-constexpr uint32_t HC_PICK_DEPTH_X16 = 0;                  // warp kernel from this average bucket size (x16) on: always
-
-__global__ void __launch_bounds__(256)
-lz4_hc_pick_kernel(BatchArgs a, uint32_t* words)
-{
-    extern __shared__ __align__(16) uint32_t buckets[];    // 16384 words of two u16 counters
-    const int nsample = gridDim.x;
-    const int b = (int)(((long long)blockIdx.x * a.n_blocks) / nsample);
-    const uint8_t* src = a.src + a.src_off[b];
-    int n = a.src_len[b];
-    const bool big = n > HCW_MAX_BLOCK;
-    if (n > HCW_MAX_BLOCK) n = HCW_MAX_BLOCK;
-    for (int i = threadIdx.x; i < 16384; i += blockDim.x) buckets[i] = 0;
-    __syncthreads();
-    for (int p = threadIdx.x; p + 4 <= n; p += blockDim.x) {
-        const uint32_t h = hcw_hash(in32(src, p));
-        atomicAdd(&buckets[h >> 1], (h & 1u) ? 0x10000u : 1u);
-    }
-    __syncthreads();
-    uint32_t s1 = 0, s2 = 0;
-    for (int i = threadIdx.x; i < 16384; i += blockDim.x) {
-        const uint32_t v = buckets[i], lo = v & 0xFFFFu, hi = v >> 16;
-        s1 += lo + hi; s2 += (lo < 255u ? lo : 255u) * lo + (hi < 255u ? hi : 255u) * hi;
-    }
-    for (int d = 16; d; d >>= 1) { s1 += __shfl_xor_sync(0xFFFFFFFFu, s1, d); s2 += __shfl_xor_sync(0xFFFFFFFFu, s2, d); }
-    if ((threadIdx.x & 31) == 0) { atomicAdd(&words[2], s1); atomicAdd(&words[3], s2 >> 4); }      // (s2 / 16: 32 blocks fit 32 bits)
-    if (big && threadIdx.x == 0) atomicAdd(&words[1], 1u);                  // blocks the warp kernel cannot take
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        if (atomicAdd(&words[0], 1u) == (uint32_t)nsample - 1u) {           // the last CTA decides
-            __threadfence();
-            const uint32_t t1 = atomicAdd(&words[2], 0u), t2 = atomicAdd(&words[3], 0u), nbig = atomicAdd(&words[1], 0u);
-            const bool deep = t1 && (unsigned long long)t2 * 256ull >= (unsigned long long)HC_PICK_DEPTH_X16 * t1;   // t2*16/t1 >= depth
-            atomicExch(&words[1], (deep && 2u * nbig < (uint32_t)nsample) ? 2u : 0u);
-            atomicExch(&words[0], 0u);
-        }
     }
 }
 
@@ -202,6 +153,37 @@ lz4_encode_hc_marked_kernel(BatchArgs a, uint8_t* arena)
 
 constexpr int HCW_FALLBACK_THREADS = 4096;                 // thread-per-block slots kept for handed-back blocks (1 GiB of state)
 
+// ---- HC encoder, blocks > 64 KiB: one WARP per block over a sliding 64 KiB window (lz4hc_window.cuh) --------------------
+// Takes the blocks the warp kernel handed back for their size; whatever it hands back itself stays marked for the thread
+// kernel.  One 32-thread CTA per warp, nothing in shared memory, HCWW_INDEX_BYTES of the arena per CTA.  HCWW_WARPS CTAs
+// per SM: the launch bound lets ptxas use 128 registers, and it needs 120 without spilling or local memory (-Xptxas -v).
+constexpr int HCWW_WARPS = 16;
+
+__global__ void __launch_bounds__(32, HCWW_WARPS)
+lz4_encode_hcw_window_kernel(BatchArgs a, uint8_t* arena, uint32_t* counter)
+{
+    void* index = arena + (size_t)blockIdx.x * HCWW_INDEX_BYTES;
+    const int lane = threadIdx.x;
+    for (;;) {
+        uint32_t b = 0;
+        if (lane == 0) b = atomicAdd(counter, 1u);
+        b = simt::shfl(0xFFFFFFFFu, b, 0);
+        if (b >= (uint32_t)a.n_blocks) break;
+        if (a.out_len[b] != HCW_FALLBACK || a.src_len[b] <= HCW_MAX_BLOCK) continue;      // (the same values in every lane)
+        const int r = hcww_encode_block(index, a.src + a.src_off[b], a.src_len[b], a.dst + a.dst_off[b], a.dst_cap[b], lane);
+        if (lane == 0) a.out_len[b] = r;
+        simt::syncwarp(0xFFFFFFFFu);                       // the next block reuses the index
+    }
+}
+
+// CTAs of the window kernel: one per block above 64 KiB up to HCWW_WARPS per SM (n_large < 0: not known on the host, the
+// batch's block count stands for it)
+static int hcww_grid(int32_t n_blocks, int32_t n_large, const DeviceInfo& dev)
+{
+    long long g = (long long)dev.num_sms * HCWW_WARPS, want = n_large < 0 ? n_blocks : n_large;
+    return (int)(g < want ? g : want);
+}
+
 static int hcw_warps(int variant, int warps_per_sm) { const int mx = variant == 1 ? 3 : 32; return warps_per_sm < 1 || warps_per_sm > mx ? mx : warps_per_sm; }
 
 static int hcw_grid(int32_t n_blocks, int variant, int warps_per_sm, const DeviceInfo& dev)
@@ -211,15 +193,19 @@ static int hcw_grid(int32_t n_blocks, int variant, int warps_per_sm, const Devic
     return g < 1 ? 1 : (int)g;
 }
 
-size_t hcw_scratch_bytes(int32_t n_blocks, int variant, int warps_per_sm, const DeviceInfo& dev)
+size_t hcw_scratch_bytes(int32_t n_blocks, int32_t n_large, int variant, int warps_per_sm, const DeviceInfo& dev)
 {
+    // the three kernels run one after the other on the same arena
     const size_t index = (size_t)hcw_grid(n_blocks, variant, warps_per_sm, dev) * HCW_INDEX_BYTES;
+    const size_t window = (size_t)hcww_grid(n_blocks, n_large, dev) * HCWW_INDEX_BYTES;
     const size_t back = hc_scratch_bytes((int)(n_blocks < HCW_FALLBACK_THREADS ? (n_blocks < 1 ? 1 : n_blocks) : HCW_FALLBACK_THREADS));
-    return index > back ? index : back;                    // the two kernels run one after the other on the same arena
+    return std::max(index, std::max(window, back));
 }
 
-// variant 1: block staged in shared memory (<= 3 warps per SM); 2: nothing in shared memory (<= 32 warps per SM)
-static cudaError_t launch_hc_warps(const BatchArgs& a, void* scratch, int variant, int warps_per_sm, uint32_t* counter, const uint32_t* pick,
+// variant 1: block staged in shared memory (<= 3 warps per SM); 2: nothing in shared memory (<= 32 warps per SM).
+// Then the window kernel over the blocks above 64 KiB, then the thread kernel over whatever is still handed back.
+// counter: four words, zero on entry (the warp kernel's ticket, the window kernel's).
+static cudaError_t launch_hc_warps(const BatchArgs& a, void* scratch, int variant, int warps_per_sm, int32_t n_large, uint32_t* counter,
                                    const DeviceInfo& dev, cudaStream_t stream, int64_t* launches)
 {
     const int warps = hcw_warps(variant, warps_per_sm);
@@ -231,60 +217,54 @@ static cudaError_t launch_hc_warps(const BatchArgs& a, void* scratch, int varian
         if (warps < 3) { const int share = dev.smem_per_sm / warps - 2048; if (share > dyn) dyn = share < dev.smem_optin ? share : dev.smem_optin; }
         e = cudaFuncSetAttribute(lz4_encode_hcw_kernel<true, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn);
         if (e != cudaSuccess) return e;
-        lz4_encode_hcw_kernel<true, 3><<<(unsigned)grid, 32, dyn, stream>>>(a, (uint8_t*)scratch, counter, pick);
+        lz4_encode_hcw_kernel<true, 3><<<(unsigned)grid, 32, dyn, stream>>>(a, (uint8_t*)scratch, counter, nullptr);
     } else {
         // Residency below 32 CTAs per SM is a matter of the grid alone: CTAs are placed breadth-first over the SMs and the
         // kernel is persistent.  No shared-memory carve-out preference: asking for "all L1" (cudaSharedmemCarveoutMaxL1)
         // left room for the system-reserved KiB of only a handful of CTAs per SM -- 16 to 32 warps per SM all ran at the
         // speed of 8 (tools/hc_ab.py: identical times); the default lets the driver size it for the occupancy.
-        if (warps <= 16) lz4_encode_hcw_kernel<false, 16><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter, pick);
-        else             lz4_encode_hcw_kernel<false, 32><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter, pick);
+        if (warps <= 16) lz4_encode_hcw_kernel<false, 16><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter, nullptr);
+        else             lz4_encode_hcw_kernel<false, 32><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter, nullptr);
     }
     if (launches) ++*launches;
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
+    if (n_large != 0) {
+        lz4_encode_hcw_window_kernel<<<(unsigned)hcww_grid(a.n_blocks, n_large, dev), 32, 0, stream>>>(a, (uint8_t*)scratch, counter + 1);
+        if (launches) ++*launches;
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
     const int back = a.n_blocks < HCW_FALLBACK_THREADS ? a.n_blocks : HCW_FALLBACK_THREADS;
     lz4_encode_hc_marked_kernel<<<(unsigned)((back + HC_THREADS - 1) / HC_THREADS), HC_THREADS, 0, stream>>>(a, (uint8_t*)scratch);
     if (launches) ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t launch_encode_hcw(const BatchArgs& a, void* scratch, int variant, int warps_per_sm, uint32_t* counter,
+cudaError_t launch_encode_hcw(const BatchArgs& a, void* scratch, int variant, int warps_per_sm, int32_t n_large, uint32_t* counter,
                               const DeviceInfo& dev, cudaStream_t stream, int64_t* launches)
 {
     if (a.n_blocks <= 0) return cudaSuccess;
-    cudaError_t e = cudaMemsetAsync(counter, 0, sizeof(uint32_t), stream);
+    cudaError_t e = cudaMemsetAsync(counter, 0, 2 * sizeof(uint32_t), stream);
     if (e != cudaSuccess) return e;
-    return launch_hc_warps(a, scratch, variant, warps_per_sm, counter, nullptr, dev, stream, launches);
+    return launch_hc_warps(a, scratch, variant, warps_per_sm, n_large, counter, dev, stream, launches);
 }
 
 // ---- HC, kernel chosen per batch -------------------------------------------------------------------------------------
 // Small batches (at most three blocks per SM): the shared-memory warp kernel, whose time per block is the shortest by far
-// (a lone thread of the thread kernel walks its block's chains one dependent load at a time).
-// Larger batches: the pick kernel looks at a sample, then both candidates are enqueued and the one not chosen returns at once.
-bool hc_auto_small(int32_t n_blocks, const DeviceInfo& dev) { return n_blocks <= 3 * dev.num_sms; }
+// (a lone thread of the thread kernel walks its block's chains one dependent load at a time); larger batches: the warp
+// kernel with nothing in shared memory at 32 warps per SM.  Blocks above 64 KiB go to the window kernel either way: it
+// was ahead of the thread kernel on every batch of such blocks timed (profiles/README.md).
+static int hc_auto_variant(int32_t n_blocks, const DeviceInfo& dev) { return n_blocks <= 3 * dev.num_sms ? 1 : 2; }
 
-size_t hc_auto_scratch_bytes(int32_t n_blocks, int concurrency, const DeviceInfo& dev)
+size_t hc_auto_scratch_bytes(int32_t n_blocks, int32_t n_large, const DeviceInfo& dev)
 {
-    if (hc_auto_small(n_blocks, dev)) return hcw_scratch_bytes(n_blocks, 1, 0, dev);
-    const size_t a = hc_scratch_bytes(concurrency), b = hcw_scratch_bytes(n_blocks, 2, 32, dev);
-    return a > b ? a : b;
+    return hcw_scratch_bytes(n_blocks, n_large, hc_auto_variant(n_blocks, dev), 0, dev);
 }
 
-cudaError_t launch_encode_hc_auto(const BatchArgs& a, void* scratch, int concurrency, uint32_t* counter /* four words */,
+cudaError_t launch_encode_hc_auto(const BatchArgs& a, void* scratch, int32_t n_large, uint32_t* counter /* four words */,
                                   const DeviceInfo& dev, cudaStream_t stream, int64_t* launches)
 {
-    if (a.n_blocks <= 0) return cudaSuccess;
-    cudaError_t e = cudaMemsetAsync(counter, 0, 4 * sizeof(uint32_t), stream);
-    if (e != cudaSuccess) return e;
-    if (hc_auto_small(a.n_blocks, dev)) return launch_hc_warps(a, scratch, 1, 0, counter, nullptr, dev, stream, launches);
-    e = cudaFuncSetAttribute(lz4_hc_pick_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536);
-    if (e != cudaSuccess) return e;
-    lz4_hc_pick_kernel<<<a.n_blocks < HC_PICK_SAMPLE ? a.n_blocks : HC_PICK_SAMPLE, 256, 65536, stream>>>(a, counter);
-    if (launches) ++*launches;
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    if ((e = launch_hc_threads(a, scratch, concurrency, counter, counter + 1, stream, launches)) != cudaSuccess) return e;
-    return launch_hc_warps(a, scratch, 2, 32, counter, counter + 1, dev, stream, launches);
+    return launch_encode_hcw(a, scratch, hc_auto_variant(a.n_blocks, dev), 0, n_large, counter, dev, stream, launches);
 }
 
 }  // namespace lz4b200

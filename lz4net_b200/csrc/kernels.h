@@ -32,15 +32,17 @@ cudaError_t launch_encode_fast(const BatchArgs& a, uint32_t* counter, int warps_
 size_t      hc_scratch_bytes(int concurrency);
 cudaError_t launch_encode_hc(const BatchArgs& a, void* scratch, int concurrency, uint32_t* counter,
                              const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
-// blocks <= 64 KiB: one warp per block on a static index, followed by the thread-per-block kernel over the blocks it handed back
-// (variant 1: the block staged in shared memory, <= 3 warps per SM; 2: nothing in shared memory, <= 32 warps per SM)
-size_t      hcw_scratch_bytes(int32_t n_blocks, int variant, int warps_per_sm, const DeviceInfo& dev);
-cudaError_t launch_encode_hcw(const BatchArgs& a, void* scratch, int variant, int warps_per_sm, uint32_t* counter,
+// one warp per block on a static index for blocks <= 64 KiB (variant 1: the block staged in shared memory, <= 3 warps per
+// SM; 2: nothing in shared memory, <= 32 warps per SM), then one warp per block over a sliding 64 KiB window for the blocks
+// above 64 KiB, then the thread-per-block kernel over whatever is still handed back.  n_large = the number of blocks above
+// 64 KiB, -1 = not known (device-memory batches: the arena is sized as if every block were one).
+size_t      hcw_scratch_bytes(int32_t n_blocks, int32_t n_large, int variant, int warps_per_sm, const DeviceInfo& dev);
+cudaError_t launch_encode_hcw(const BatchArgs& a, void* scratch, int variant, int warps_per_sm, int32_t n_large, uint32_t* counter,
                               const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
-// kernel chosen per batch: small batches -> the shared-memory warp kernel; large ones -> a sample of the batch decides on
-// the device between the thread kernel and the warp kernel (`counter` = four words)
-size_t      hc_auto_scratch_bytes(int32_t n_blocks, int concurrency, const DeviceInfo& dev);
-cudaError_t launch_encode_hc_auto(const BatchArgs& a, void* scratch, int concurrency, uint32_t* counter,
+// kernel chosen per batch: small batches -> the shared-memory warp kernel, larger ones -> the one with nothing in shared
+// memory (`counter` = four words)
+size_t      hc_auto_scratch_bytes(int32_t n_blocks, int32_t n_large, const DeviceInfo& dev);
+cudaError_t launch_encode_hc_auto(const BatchArgs& a, void* scratch, int32_t n_large, uint32_t* counter,
                                   const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 cudaError_t launch_compact(const uint8_t* slots, const int64_t* slot_off, const int32_t* len, uint8_t* packed,
                            int64_t* out_off, int32_t n_blocks, void* scan_tmp, size_t scan_tmp_bytes,
