@@ -7,6 +7,8 @@
 #include "lz4_encode.cuh"
 #include "lz4hc_encode.cuh"
 #include "lz4hc_warp.cuh"
+#include "lz4hc_window.cuh"
+#include "lz4_measure.cuh"
 #include <stdlib.h>
 #include <vector>
 
@@ -76,10 +78,8 @@ void lpb_entry(int lane, void* arg)
     }
 }
 
-int g_enc_variant = 2;
-EncTune g_enc_tune;
-
 struct EncJob {
+    int variant; EncTune tune;
     int nblocks; const uint8_t* const* src; const int* n; uint8_t* const* dst; const int* cap; int* result;
     EncShared* sh;
 };
@@ -88,9 +88,25 @@ void enc_entry(int lane, void* arg)
 {
     EncJob* j = (EncJob*)arg;
     for (int b = 0; b < j->nblocks; b++) {
-        int r = g_enc_variant == 1 ? encode_block<1>(j->sh, j->src[b], j->n[b], j->dst[b], j->cap[b], lane, g_enc_tune)
-                                   : encode_block<2>(j->sh, j->src[b], j->n[b], j->dst[b], j->cap[b], lane, g_enc_tune);
+        int r = j->variant == 1 ? encode_block<1>(j->sh, j->src[b], j->n[b], j->dst[b], j->cap[b], lane, j->tune)
+                                : encode_block<2>(j->sh, j->src[b], j->n[b], j->dst[b], j->cap[b], lane, j->tune);
         if (lane == 0) j->result[b] = r;
+    }
+}
+
+// measure pass: one lane per block like the kernel; the lanes take blocks with a stride and meet after every round of
+// 32 blocks, so the scheduler interleaves them in its seeded order
+struct MeasureJob { int known, nblocks; const uint8_t* const* src; const int* isize; const int* cap; int* result; };
+void measure_entry(int lane, void* arg)
+{
+    MeasureJob* j = (MeasureJob*)arg;
+    for (int b0 = 0; b0 < j->nblocks; b0 += 32) {
+        const int b = b0 + lane;
+        if (b < j->nblocks) {
+            const int cap = j->cap ? j->cap[b] : 0x7FFFFFFF;
+            j->result[b] = j->known ? measure_block<true>(j->src[b], j->isize[b], cap) : measure_block<false>(j->src[b], j->isize[b], cap);
+        }
+        simt::syncwarp(0xFFFFFFFFu);
     }
 }
 
@@ -151,18 +167,40 @@ int emu_encode_hcw(const uint8_t* src, int n, uint8_t* dst, int cap, uint64_t sc
     return j.result;
 }
 
-void emu_set_encode_variant(int v) { g_enc_variant = v; }
-void emu_set_encode_tune(int lane_copy_max, int probe_max, int wide_min)
+// the warp-per-block HC encoder over a sliding 64 KiB window (blocks above 64 KiB); returns the bytes written, 0 (did not
+// fit) or HCW_FALLBACK (handed back to the thread-per-block kernel)
+struct WinJob { const uint8_t* src; int n; uint8_t* dst; int cap; int result; void* index; };
+static void win_entry(int lane, void* arg)
 {
-    g_enc_tune.lane_copy_max = lane_copy_max; g_enc_tune.probe_max = probe_max; g_enc_tune.wide_min = wide_min;
+    WinJob* j = (WinJob*)arg;
+    const int r = hcww_encode_block(j->index, j->src, j->n, j->dst, j->cap, lane);
+    if (lane == 0) j->result = r;
+}
+int emu_encode_hcw_window(const uint8_t* src, int n, uint8_t* dst, int cap, uint64_t sched_seed)
+{
+    WinJob j{src, n, dst, cap, 0, aligned_alloc(16, HCWW_INDEX_BYTES)};
+    memset(j.index, 0xA5, HCWW_INDEX_BYTES);                          // stale garbage, like a reused arena slot
+    simt_emu::run_warp(win_entry, &j, sched_seed);
+    free(j.index);
+    return j.result;
 }
 
-void emu_encode(int nblocks, const uint8_t* const* src, const int* n, uint8_t* const* dst, const int* cap,
-                int* result, uint64_t sched_seed)
+// variant: how the round finds same-hash lanes (1 always exact votes, 2 optimistic); the last three are EncTune's fields
+void emu_encode(int variant, int lane_copy_max, int probe_max, int wide_min, int nblocks, const uint8_t* const* src,
+                const int* n, uint8_t* const* dst, const int* cap, int* result, uint64_t sched_seed)
 {
-    EncJob j{nblocks, src, n, dst, cap, result, (EncShared*)aligned_alloc(16, sizeof(EncShared))};
+    EncTune tune;
+    tune.lane_copy_max = lane_copy_max; tune.probe_max = probe_max; tune.wide_min = wide_min;
+    EncJob j{variant, tune, nblocks, src, n, dst, cap, result, (EncShared*)aligned_alloc(16, sizeof(EncShared))};
     simt_emu::run_warp(enc_entry, &j, sched_seed);
     free(j.sh);
+}
+
+// cap may be null: INT32_MAX for every block (the unknown-size mode's "no limit")
+void emu_measure(int known, int nblocks, const uint8_t* const* src, const int* isize, const int* cap, int* result, uint64_t sched_seed)
+{
+    MeasureJob j{known, nblocks, src, isize, cap, result};
+    simt_emu::run_warp(measure_entry, &j, sched_seed);
 }
 
 }

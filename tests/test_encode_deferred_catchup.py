@@ -6,9 +6,6 @@ probes with a growing step, so the positions between two probes are never insert
 in front of an inserted probe position x to the bytes in front of a later probe position y gives a match found at y
 whose catch-up is exactly as long as the copy (or is stopped by the anchor, or by ref reaching position 0).  A small
 model of the reference's greedy parse (checked against the oracle's bytes) confirms every planted catch-up."""
-import ctypes as C
-import mmap
-
 import numpy as np
 import pytest
 
@@ -310,39 +307,8 @@ def test_catchups_unaligned_buffers(planted, skew):
 def test_catchups_under_every_heuristic(planted, tune):
     """probe_max and wide_min see the literal length before the catch-up; they still only choose between equivalent
     paths."""
-    lib = emu.lib()
-    lib.emu_set_encode_tune(*tune)
-    try:
-        _check([b for b, _ in planted[:5]] + [cases.content(m, 30000, seed=5).tobytes() for m in ("E50", "ETEXT")],
-               sched_seed=6)
-    finally:
-        lib.emu_set_encode_tune(12, 8, 24)
-
-
-def _encode_front_guarded(block, pad):
-    """Encode one block that starts `pad` bytes after the start of a page whose preceding page is PROT_NONE: any read
-    of a word in front of the block faults.  Returns (result, bytes)."""
-    page = mmap.PAGESIZE
-    n = len(block)
-    npages = (pad + n + 64 + page - 1) // page
-    m = mmap.mmap(-1, (npages + 1) * page)
-    base = C.addressof(C.c_char.from_buffer(m))
-    libc = C.CDLL(None, use_errno=True)
-    libc.mprotect.argtypes = [C.c_void_p, C.c_size_t, C.c_int]
-    assert libc.mprotect(base, page, 0) == 0
-    start = page + pad
-    m[start:start + n] = block
-    cap = n + n // 255 + 16
-    dst = np.full(cap + 96, 0xCD, np.uint8)
-    ns = np.array([n], np.int32); cps = np.array([cap], np.int32); res = np.zeros(1, np.int32)
-    sp = (C.c_void_p * 1)(base + start); dp = (C.c_void_p * 1)(dst.ctypes.data + 32)
-    emu.lib().emu_set_encode_variant(2)
-    emu.lib().emu_encode(1, sp, ns.ctypes.data_as(C.c_void_p), dp, cps.ctypes.data_as(C.c_void_p),
-                         res.ctypes.data_as(C.c_void_p), C.c_uint64(3))
-    assert libc.mprotect(base, page, 3) == 0
-    del sp
-    r = int(res[0])
-    return r, dst[32:32 + max(r, 0)].tobytes()
+    _check([b for b, _ in planted[:5]] + [cases.content(m, 30000, seed=5).tobytes() for m in ("E50", "ETEXT")],
+           sched_seed=6, tune=tune)
 
 
 def test_catchup_never_reads_before_the_input():
@@ -351,4 +317,5 @@ def test_catchup_never_reads_before_the_input():
     blocks = [build_ref0(16000, c, seed=200 + c)[0] for c in (1, 2, 3, 4, 5, 9)] + [build_ref0(70000, 6, seed=7)[0]]
     for b in blocks:
         for pad in range(4):
-            assert _encode_front_guarded(b, pad) == oracle.encode(b), (len(b), pad)
+            res, outs = emu.encode([b], sched_seed=3, fence="front", pad=pad)
+            assert (res[0], outs[0]) == oracle.encode(b), (len(b), pad)

@@ -5,15 +5,14 @@ import numpy as np
 import pytest
 
 import oracle
-from tests import cases
-from tests import emu_hcw_window as win
+from tests import cases, emu
 
-FB = win.HCW_FALLBACK
+FB = emu.HCW_FALLBACK
 
 
 def _check(d, cap=None, **kw):
     """True = encoded like the reference, False = handed back."""
-    r, o = win.encode(d, cap=cap, **kw)
+    r, o = emu.encode_hcw_window(d, cap=cap, **kw)
     if r == FB:
         return False
     assert (r, o) == oracle.encode_hc(d, cap=cap), (len(d), cap, kw)
@@ -109,7 +108,7 @@ def test_window_hands_back_the_colliding_triple():
             if found: break
         if found: break
     d = _rand(70000, 3) + bytes(found) * 200 + _rand(500, 4)
-    assert win.encode(d)[0] == FB
+    assert emu.encode_hcw_window(d)[0] == FB
     assert _check(_rand(70000, 3) + bytes([1, 2, 3]) * 200 + _rand(500, 4))
 
 
@@ -137,4 +136,4 @@ def test_window_reads_no_word_outside_the_block(behind):
     """A PROT_NONE page directly behind the block's last byte / in front of its first: no word without an input byte is read."""
     for n in (65537, 131074):
         d = cases.content("mixed", n, seed=n).tobytes()
-        assert win.encode_fenced(d, behind=behind) == oracle.encode_hc(d), (n, behind)
+        assert emu.encode_hcw_window(d, fence="behind" if behind else "front") == oracle.encode_hc(d), (n, behind)

@@ -62,6 +62,11 @@ def test_encode_output_limit_inside_every_emission_batch():
         _enc_check([d] * len(caps), caps, sched_seed=8)
 
 
+def _encode_fenced(d, **kw):
+    res, outs = emu.encode([d], **kw)
+    return res[0], outs[0]
+
+
 def test_encode_never_reads_past_the_input():
     """The block ends on the last byte of a mapped page (next page PROT_NONE): a load of any word that holds no input
     byte would fault.  Covers the unaligned 32-bit reads of the parse, the match-length count up to matchlimit, the
@@ -69,14 +74,15 @@ def test_encode_never_reads_past_the_input():
     for model, n in (("E50", 65536), ("ETEXT", 65536), ("E100", 65536), ("E0", 8192), ("lowent", 4096), ("periodic", 65536),
                      ("runs", 20000), ("mixed", 12), ("mixed", 16), ("ETEXT", 70000)):
         d = cases.content(model, n, seed=n % 97).tobytes()
-        assert emu.encode_guarded(d, sched_seed=3) == oracle.encode(d), (model, n)
-    # every source alignment and every position of the block end inside its last word
+        assert _encode_fenced(d, sched_seed=3, fence="behind") == oracle.encode(d), (model, n)
+    # every source alignment and every position of the block end inside its last word: e (0..3) readable bytes stay
+    # between the block and the fence, the rest of its last aligned 32-bit word (the kernels read whole aligned words)
     for n in (4093, 4094, 4095, 4096, 13, 14, 15):
         for pad in range(4):
             if (n + pad) % 4 == 0 or pad == 0:
                 d = cases.content("lowent", n, seed=n + pad).tobytes()
                 e = (4 - n % 4) % 4 if pad else 0
-                assert emu.encode_guarded(d, sched_seed=4, end_pad=e) == oracle.encode(d), (n, e)
+                assert _encode_fenced(d, sched_seed=4, fence="behind", pad=e) == oracle.encode(d), (n, e)
 
 
 def test_encode_general_variant_above_64k():

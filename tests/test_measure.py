@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 import oracle
-from tests import cases, emu_measure
+from tests import cases, emu
 
 
 def _agree(got, want, what=""):
@@ -76,7 +76,7 @@ def test_measure_matches_oracle_decoders(known):
     pairs = _corpus()
     comp = [c for c, _ in pairs]
     caps = [len(d) for _, d in pairs]
-    res = emu_measure.measure(comp, caps, known=known, sched_seed=3)
+    res = emu.measure(comp, caps, known=known, sched_seed=3)
     for (c, d), cap, r in zip(pairs, caps, res):
         _agree(r, _expect(c, cap, known), len(d))
         if r >= 0:
@@ -84,7 +84,7 @@ def test_measure_matches_oracle_decoders(known):
     if not known:                                                # capacity one byte more / less than the decoded size
         for delta in (1, -1):
             caps2 = [max(len(d) + delta, 0) for _, d in pairs]
-            for (c, d), cap, r in zip(pairs, caps2, emu_measure.measure(comp, caps2, known=False, sched_seed=4)):
+            for (c, d), cap, r in zip(pairs, caps2, emu.measure(comp, caps2, known=False, sched_seed=4)):
                 _agree(r, _expect(c, cap, False), (len(d), cap))
 
 
@@ -92,7 +92,7 @@ def test_measure_size_invariants():
     sc = _size_cases()
     for known in (True, False):
         sel = [(c, cap) for c, cap, k in sc if k == known]
-        res = emu_measure.measure([c for c, _ in sel], [cap for _, cap in sel], known=known, sched_seed=11)
+        res = emu.measure([c for c, _ in sel], [cap for _, cap in sel], known=known, sched_seed=11)
         expect = [_expect(c, cap, known) for c, cap in sel]
         for r, e in zip(res, expect):
             _agree(r, e)
@@ -102,14 +102,14 @@ def test_measure_size_invariants():
 @pytest.mark.parametrize("known", [True, False])
 def test_measure_corrupt_streams(known):
     comp, caps = _corrupt()
-    res = emu_measure.measure(comp, caps, known=known, sched_seed=13)
+    res = emu.measure(comp, caps, known=known, sched_seed=13)
     expect = [_expect(c, cap, known) for c, cap in zip(comp, caps)]
     for r, e in zip(res, expect):
         _agree(r, e)
     assert sum(e < 0 for e in expect) > 50 and sum(e >= 0 for e in expect) > 20
     # unlimited capacity: the verdicts at INT32_MAX are those at 256 * len + 64 (no stream of len bytes writes more)
     if not known:
-        res = emu_measure.measure(comp, None, known=False, sched_seed=15)
+        res = emu.measure(comp, None, known=False, sched_seed=15)
         for c, r in zip(comp, res):
             _agree(r, oracle.decode_unknown(c, 256 * len(c) + 64)[0])
 
@@ -118,14 +118,14 @@ def test_measure_length_overflow_inputs():
     for bad in (OVERFLOW, LONG_LITERAL, OVERFLOW[:3], bytes([0xF0])):
         for known in (True, False):
             cap = 1 << 20
-            _agree(emu_measure.measure([bad], [cap], known=known)[0], _expect(bad, cap, known), (len(bad), known))
-        assert emu_measure.measure([bad], None)[0] < 0
+            _agree(emu.measure([bad], [cap], known=known)[0], _expect(bad, cap, known), (len(bad), known))
+        assert emu.measure([bad], None)[0] < 0
 
 
 def test_measure_unlimited_capacity():
     pairs = _corpus(lens=(0, 1, 13, 300, 65536, 65546))
     comp = [c for c, _ in pairs]
-    res = emu_measure.measure(comp, None, known=False, sched_seed=7)
+    res = emu.measure(comp, None, known=False, sched_seed=7)
     for (c, d), r in zip(pairs, res):
         _agree(r, oracle.decode_unknown(c, 256 * len(c) + 64)[0], len(d))
         assert r == len(d)
@@ -137,7 +137,7 @@ def test_measure_unaligned_streams_and_lane_schedules(skew):
     comp = [c for c, _ in pairs]
     for seed in (skew, 100 + skew):
         for known in (True, False):
-            res = emu_measure.measure(comp, [len(d) for _, d in pairs], known=known, sched_seed=seed, src_skew=skew)
+            res = emu.measure(comp, [len(d) for _, d in pairs], known=known, sched_seed=seed, src_skew=skew)
             assert res == [len(c) if known else len(d) for c, d in pairs]
 
 
@@ -150,10 +150,10 @@ def test_measure_never_reads_past_the_last_unit():
             c = fn(d)[1]
             for cc in (c, c[:-1], c[: len(c) // 2], c[:1]):
                 for known in (True, False):
-                    _agree(emu_measure.measure_guarded(cc, len(d), known=known), _expect(cc, len(d), known), (m, n, len(cc), known))
-                _agree(emu_measure.measure_guarded(cc), oracle.decode_unknown(cc, 256 * len(cc) + 64)[0], (m, n, len(cc)))
+                    _agree(emu.measure([cc], [len(d)], known=known, fence="behind")[0], _expect(cc, len(d), known), (m, n, len(cc), known))
+                _agree(emu.measure([cc], fence="behind")[0], oracle.decode_unknown(cc, 256 * len(cc) + 64)[0], (m, n, len(cc)))
     for bad in (OVERFLOW, LONG_LITERAL):
-        assert emu_measure.measure_guarded(bad) < 0 and emu_measure.measure_guarded(bad, 1 << 20, known=True) < 0
+        assert emu.measure([bad], fence="behind")[0] < 0 and emu.measure([bad], [1 << 20], known=True, fence="behind")[0] < 0
 
 
 def test_entry_points_reject_bad_arguments():

@@ -23,25 +23,21 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from lz4net_b200 import synth  # noqa: E402
+from tests import emu  # noqa: E402
 
 CSRC = os.path.join(ROOT, "lz4net_b200", "csrc")
-EMU = os.path.join(ROOT, "tests", "simt_emu")
 # the order of enum EncProfSlot
 EVENTS = ["blocks", "seqs", "rounds", "rounds_wide", "exact", "probes", "probe_hits", "flushes", "long_lit", "catchup_long"]
 PHASES = ["loadhash", "samehash", "vote", "exact", "probe", "catchup", "count", "park", "emit", "block"]
 BLOCK = 65536
 
 
-def _build(tmp: str, emu: bool, prof: bool) -> C.CDLL:
-    so = os.path.join(tmp, f"enc_phases_{'emu' if emu else 'gpu'}_{int(prof)}.so")
-    if emu:
-        cmd = ["g++", "-O2", "-shared", "-fPIC", "-std=c++17", "-I" + EMU, "-I" + CSRC, "-o", so,
-               os.path.join(EMU, "simt_emu.cpp"), os.path.join(ROOT, "tools", "enc_phases_emu.cpp")]
-    else:
-        nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-shared", "-Xcompiler", "-fPIC",
-               "-I" + CSRC, "-o", so, os.path.join(ROOT, "tools", "enc_phases.cu")] + (["-DLZ4B200_ENC_PROF"] if prof else [])
-    subprocess.check_call(cmd)
+def _build(tmp: str, prof: bool) -> C.CDLL:
+    so = os.path.join(tmp, f"enc_phases_gpu_{int(prof)}.so")
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-shared", "-Xcompiler",
+                           "-fPIC", "-I" + CSRC, "-o", so, os.path.join(ROOT, "tools", "enc_phases.cu")]
+                          + (["-DLZ4B200_ENC_PROF"] if prof else []))
     return C.CDLL(so)
 
 
@@ -70,8 +66,10 @@ def main():
     nb = a.blocks or (8 if a.emu else 32768)
     res = {}
     with tempfile.TemporaryDirectory() as tmp:
-        libs = {True: _build(tmp, a.emu, True)} if a.emu else {True: _build(tmp, False, True), False: _build(tmp, False, False)}
-        if not a.emu:
+        if a.emu:
+            libs = {True: C.CDLL(emu.build(os.path.join(ROOT, "tools", "enc_phases_emu.cpp"), ["-DLZ4B200_ENC_PROF"]))}
+        else:
+            libs = {True: _build(tmp, True), False: _build(tmp, False)}
             import torch
             res["device"] = torch.cuda.get_device_name(0)
             try:
