@@ -120,9 +120,8 @@ cudaError_t launch_encode_hc(const BatchArgs& a, void* scratch, int concurrency,
 // MINB = CTAs per SM the register budget is cut for (SMEM: 3; global variant: 16 -> <= 128 registers, 32 -> 64)
 template <bool SMEM, int MINB>
 __global__ void __launch_bounds__(32, MINB)
-lz4_encode_hcw_kernel(BatchArgs a, uint8_t* arena, uint32_t* counter, const uint32_t* pick)
+lz4_encode_hcw_kernel(BatchArgs a, uint8_t* arena, uint32_t* counter)
 {
-    if (pick && *pick == 0u) return;                       // (launched with pick = nullptr: the gate is kept only so that these kernels' instructions stay those profiled)
     extern __shared__ __align__(16) uint8_t smem[];
     const simt::smem_ref sm = simt::smem_ref_of(smem);
     void* index = arena + (size_t)blockIdx.x * HCW_INDEX_BYTES;
@@ -217,14 +216,14 @@ static cudaError_t launch_hc_warps(const BatchArgs& a, void* scratch, int varian
         if (warps < 3) { const int share = dev.smem_per_sm / warps - 2048; if (share > dyn) dyn = share < dev.smem_optin ? share : dev.smem_optin; }
         e = cudaFuncSetAttribute(lz4_encode_hcw_kernel<true, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn);
         if (e != cudaSuccess) return e;
-        lz4_encode_hcw_kernel<true, 3><<<(unsigned)grid, 32, dyn, stream>>>(a, (uint8_t*)scratch, counter, nullptr);
+        lz4_encode_hcw_kernel<true, 3><<<(unsigned)grid, 32, dyn, stream>>>(a, (uint8_t*)scratch, counter);
     } else {
         // Residency below 32 CTAs per SM is a matter of the grid alone: CTAs are placed breadth-first over the SMs and the
         // kernel is persistent.  No shared-memory carve-out preference: asking for "all L1" (cudaSharedmemCarveoutMaxL1)
         // left room for the system-reserved KiB of only a handful of CTAs per SM -- 16 to 32 warps per SM all ran at the
         // speed of 8 (tools/hc_ab.py: identical times); the default lets the driver size it for the occupancy.
-        if (warps <= 16) lz4_encode_hcw_kernel<false, 16><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter, nullptr);
-        else             lz4_encode_hcw_kernel<false, 32><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter, nullptr);
+        if (warps <= 16) lz4_encode_hcw_kernel<false, 16><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter);
+        else             lz4_encode_hcw_kernel<false, 32><<<(unsigned)grid, 32, 0, stream>>>(a, (uint8_t*)scratch, counter);
     }
     if (launches) ++*launches;
     e = cudaGetLastError();

@@ -18,7 +18,8 @@
 //      reference's "first candidate that beats everything before it" = first maximum, one REDUX);
 //   3. scans literal stretches 64 positions per round, a lane per position (the index is static: no insert hazard).
 // The 3-match look-ahead parse (:557-742) and LZ4_encodeSequence (:521-550) are control flow over those searches and are
-// restated branch for branch, warp-uniformly.
+// restated branch for branch, warp-uniformly.  The search, the scan and the parse are written against a small index
+// interface (HcwIndex below); lz4hc_window.cuh runs the same three on its segmented index for blocks above 64 KiB.
 //
 // The two places where r93's state DOES depend on the parse are detected and the block is handed to the exact scalar
 // kernel (HCW_FALLBACK; both are conservative, neither has been seen on the test corpora except when constructed):
@@ -46,15 +47,13 @@ constexpr uint32_t HCW_FULL      = 0xFFFFFFFFu;
 //                 three warps (blocks) per SM;
 //   SMEM = false: the block is read through the read-only path (L1 / L2), the counters live in the warp's arena slot
 //                 (global atomics): no shared memory, as many warps per SM as the launch asks for.
+// HcwBlock is the block as the search, the scan and the parse read it (lz4hc_window.cuh uses it with SMEM = false).
 template <bool SMEM>
-struct Hcw {
+struct HcwBlock {
     simt::smem_ref sm;            // SMEM: HCW_SMEM_BYTES
-    uint32_t* cnt;                // !SMEM: 16384 words of packed u16 counters
     InWords in;                   // the input through aligned 32-bit words (the build; !SMEM: every read)
-    uint16_t* rank;               // rank[p]: index of position p in `sorted` (positions 1 .. mflimit-1)
-    uint16_t* sorted;             // positions ordered by (hash, position)
     const uint8_t* src; int n, lane, mflimit, matchlimit;
-    uint32_t v0;                  // the four bytes at position 0 (the end of every walk)
+    uint32_t v0;                  // the four bytes at position 0 (the end of every walk that reaches it)
 
     // four bytes / one byte at position p of the block (p + 3 < n)
     SIMT_MEM uint32_t rd32(uint32_t p) const
@@ -63,7 +62,15 @@ struct Hcw {
         return in.at((int)p);
     }
     SIMT_MEM uint32_t rd8(uint32_t p) const { return SMEM ? simt::lds_u8(sm, p) : (uint32_t)simt::ldg_nc_u8(src + p); }
-    // the build's counters: u16, two to a word, word w at byte 4w
+};
+
+// The build's bucket counters: u16, two to a word, word w at byte 4w (SMEM: at the start of the shared memory; !SMEM: the
+// 16384 words at `cnt`)
+template <bool SMEM>
+struct HcwCounters {
+    simt::smem_ref sm;
+    uint32_t* cnt;
+    int lane;
     SIMT_MEM void cnt_zero() const
     {
         if (SMEM) for (uint32_t i = (uint32_t)lane * 16u; i < 65536u; i += 512u) simt::sts_v4(sm, i, uint4{0, 0, 0, 0});
@@ -91,9 +98,39 @@ struct Hcw {
 
 SIMT_DEV uint32_t hcw_hash(uint32_t v) { return (v * 2654435761u) >> 17; }                   // :245-246 HASH_LOG 15
 
+// The static index of a block of <= 64 KiB (built by hcw_build): candidate k of q is sorted[rank[q]-1-k] while that entry
+// is in q's bucket, then position 0.  The search, the scan and the parse reach an index only through these members
+// (lz4hc_window.cuh's HcwwIndex is the other implementation):
+//   At                   q's place in the index, with shfl(l) = lane l's place
+//   at(w, q)             q's place
+//   cand(at, q, k)       candidate k of q: a position, or -1 for none
+//   ends_at_0(q)         whether the walk from q ends at position 0 once its candidates run out
+//   prepare(w, q)        before a scan round at q and before a wider search at q (warp-uniform q)
+//   round_end(ip, mfl)   the end of the scan round that starts at ip
+struct HcwAt {                    // q's place in the index: rank[q]
+    int r;
+    SIMT_MEM HcwAt shfl(int l) const { return HcwAt{(int)simt::shfl(HCW_FULL, (uint32_t)r, l)}; }
+};
+
+struct HcwIndex {
+    typedef HcwAt At;
+    uint16_t* rank;               // rank[p]: index of position p in `sorted` (positions 1 .. mflimit-1)
+    uint16_t* sorted;             // positions ordered by (hash, position)
+
+    template <bool SMEM>
+    SIMT_MEM At at(const HcwBlock<SMEM>&, int q) const { return At{(int)simt::ldg_u16(rank + q)}; }
+    // candidate k of q: a position, or -1 below the first entry.  An entry of another bucket comes back as a position:
+    // the caller's hash test ends the walk there.
+    SIMT_MEM int cand(const At& a, int, int k) const { const int idx = a.r - 1 - k; return idx >= 0 ? (int)simt::ldg_u16(sorted + idx) : -1; }
+    SIMT_MEM bool ends_at_0(int) const { return true; }                             // every walk ends at position 0
+    template <bool SMEM>
+    SIMT_MEM void prepare(const HcwBlock<SMEM>&, int) {}                       // (the whole index is built up front)
+    SIMT_MEM int round_end(int ip, int mflimit) const { return ip + 64 < mflimit ? ip + 64 : mflimit; }
+};
+
 // equal bytes of [a..) and [b..), a < limit  (== the 8/4/2/1 scheme of :376-391); one lane
 template <bool SMEM>
-SIMT_DEV int hcw_common(const Hcw<SMEM>& w, int a, int b, int limit)
+SIMT_DEV int hcw_common(const HcwBlock<SMEM>& w, int a, int b, int limit)
 {
     const int a0 = a;
     while (a + 4 <= limit) {
@@ -108,7 +145,7 @@ SIMT_DEV int hcw_common(const Hcw<SMEM>& w, int a, int b, int limit)
 // the same count by the whole warp for ONE pair (a, b, limit identical in every lane): 128 bytes per step, the first
 // differing word found with one vote.  Same value as hcw_common (the common prefix, capped at limit).
 template <bool SMEM>
-SIMT_DEV int hcw_common_warp(const Hcw<SMEM>& w, int a, int b, int limit)
+SIMT_DEV int hcw_common_warp(const HcwBlock<SMEM>& w, int a, int b, int limit)
 {
     for (int done = 0; ; done += 128) {
         const int pa = a + done + 4 * w.lane;
@@ -146,11 +183,11 @@ struct HcwInputSrc {
 
 // ---- 1. the index ---------------------------------------------------------------------------------------------------
 template <bool SMEM>
-SIMT_DEV void hcw_build(const Hcw<SMEM>& w)
+SIMT_DEV void hcw_build(const HcwBlock<SMEM>& w, const HcwIndex& x, const HcwCounters<SMEM>& ct)
 {
     const int lane = w.lane, P = w.mflimit;                               // positions 1 .. P-1 are ever searched or walked to
     const InWords& in = w.in;
-    w.cnt_zero();
+    ct.cnt_zero();
     simt::syncwarp(HCW_FULL);
     // bucket sizes: u16 counters, two to a word, atomic adds on the word (a bucket never holds 65536 positions: no carry).
     // 128 positions per iteration, their input words requested together; the hashes are parked in rank[] for the scatter.
@@ -161,7 +198,7 @@ SIMT_DEV void hcw_build(const Hcw<SMEM>& w)
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             const int p = base + 32 * j + lane;
-            if (p < P) { const uint32_t h = hcw_hash(InWords::word(raw[j])); simt::stg_u16(w.rank + p, h); w.cnt_add(h); }
+            if (p < P) { const uint32_t h = hcw_hash(InWords::word(raw[j])); simt::stg_u16(x.rank + p, h); ct.cnt_add(h); }
         }
     }
     simt::syncwarp(HCW_FULL);
@@ -172,25 +209,25 @@ SIMT_DEV void hcw_build(const Hcw<SMEM>& w)
         const uint32_t wi = w0 + 4u * (uint32_t)lane;
         uint32_t v[4], s = 0;
 #pragma unroll
-        for (int j = 0; j < 4; j++) { v[j] = w.cnt_word(wi + j); s += (v[j] & 0xFFFFu) + (v[j] >> 16); }
-        uint32_t x = s;
+        for (int j = 0; j < 4; j++) { v[j] = ct.cnt_word(wi + j); s += (v[j] & 0xFFFFu) + (v[j] >> 16); }
+        uint32_t xs = s;
 #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = simt::shfl(HCW_FULL, x, lane >= d ? lane - d : lane); if (lane >= d) x += y; }
-        uint32_t run = x - s + carry;
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t y = simt::shfl(HCW_FULL, xs, lane >= d ? lane - d : lane); if (lane >= d) xs += y; }
+        uint32_t run = xs - s + carry;
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             const uint32_t lo = v[j] & 0xFFFFu, hi = v[j] >> 16;
-            w.cnt_word_set(wi + j, (run & 0xFFFFu) | ((run + lo) << 16));
+            ct.cnt_word_set(wi + j, (run & 0xFFFFu) | ((run + lo) << 16));
             run += lo + hi;
         }
-        carry += simt::shfl(HCW_FULL, x, 31);
+        carry += simt::shfl(HCW_FULL, xs, 31);
     }
     simt::syncwarp(HCW_FULL);
     // stable scatter, 32 consecutive positions per step (eight steps' hashes requested together)
     for (int base8 = 1; base8 < P; base8 += 256) {
         uint32_t hh[8];
 #pragma unroll
-        for (int j = 0; j < 8; j++) { const int p = base8 + 32 * j + lane; hh[j] = p < P ? simt::ldg_u16(w.rank + p) : 0xFFFFFFFFu; }
+        for (int j = 0; j < 8; j++) { const int p = base8 + 32 * j + lane; hh[j] = p < P ? simt::ldg_u16(x.rank + p) : 0xFFFFFFFFu; }
 #pragma unroll
         for (int j = 0; j < 8; j++) {
             const int base = base8 + 32 * j;
@@ -203,10 +240,10 @@ SIMT_DEV void hcw_build(const Hcw<SMEM>& w)
                 // counters at LDS / ATOMS latency: every lane adds for itself; lanes that share a hash inside the step get
                 // their indices from the atomic in no particular order, so such a step (one lane sees a counter that is not
                 // the value every lane read before) re-ranks the sharing lanes by position
-                const uint32_t c0 = act ? w.cnt_get(h) : 0u;
+                const uint32_t c0 = act ? ct.cnt_get(h) : 0u;
                 simt::syncwarp(HCW_FULL);
                 idx = c0;
-                if (act) idx = w.cnt_add(h);
+                if (act) idx = ct.cnt_add(h);
                 uint32_t pend = simt::ballot(HCW_FULL, act && idx != c0);
                 while (pend) {
                     const uint32_t hl = simt::shfl(HCW_FULL, h, simt::ffs(pend) - 1);
@@ -220,18 +257,18 @@ SIMT_DEV void hcw_build(const Hcw<SMEM>& w)
                 const uint32_t same = simt::match_any(HCW_FULL, h);
                 const int leader = simt::ffs(same) - 1;
                 uint32_t first = 0;
-                if (act && lane == leader) first = w.cnt_add_n(h, (uint32_t)simt::popc(same));
+                if (act && lane == leader) first = ct.cnt_add_n(h, (uint32_t)simt::popc(same));
                 first = simt::shfl(HCW_FULL, first, leader);
                 idx = first + (uint32_t)simt::popc(same & ((1u << lane) - 1u));
             }
-            if (act) { simt::stg_u16(w.sorted + idx, (uint32_t)p); simt::stg_u16(w.rank + p, idx); }
+            if (act) { simt::stg_u16(x.sorted + idx, (uint32_t)p); simt::stg_u16(x.rank + p, idx); }
             simt::syncwarp(HCW_FULL);
         }
     }
 }
 
 // the block's bytes into shared memory (aligned 16-byte reads of words that hold at least one input byte)
-SIMT_DEV void hcw_stage(const Hcw<true>& w)
+SIMT_DEV void hcw_stage(const HcwBlock<true>& w)
 {
     for (uint32_t i = (uint32_t)w.lane * 16u; i < (uint32_t)w.n; i += 512u) {
         const uintptr_t a = (uintptr_t)(w.src + i), al = a & ~(uintptr_t)15;
@@ -252,11 +289,12 @@ struct HcwHit { int len, ref, start, repl, delta; };
 
 // WIDER = false: LZ4HC_InsertAndFindBestMatch (:394-459) at q (len 0 = no match).
 // WIDER = true : LZ4HC_InsertAndGetWiderMatch (:462-518) at q with start_limit / longest; len <= longest = nothing better.
-// r = rank[q].  Candidate k is sorted[r-1-k] while that entry is in q's bucket, then position 0, then nothing; at most 256
-// are examined (:403, :471), one more when the first one lies within 4 bytes (:411-420 consumes it without an attempt).
-// The reference's byte filters (:426, :480) only skip candidates that cannot win; the 4-byte test implies them.
-template <bool WIDER, bool SMEM>
-SIMT_DEV HcwHit hcw_search(const Hcw<SMEM>& w, int q, int r, int start_limit, int longest)
+// `at` = x.at(w, q).  Candidate k is x.cand(at, q, k) while that position is in q's bucket, then position 0 where the
+// index says the walk ends there, then nothing; at most 256 are examined (:403, :471), one more when the first one lies
+// within 4 bytes (:411-420 consumes it without an attempt).  The reference's byte filters (:426, :480) only skip
+// candidates that cannot win; the 4-byte test implies them.
+template <bool WIDER, bool SMEM, class X>
+SIMT_DEV HcwHit hcw_search(const HcwBlock<SMEM>& w, const X& x, int q, const typename X::At& at, int start_limit, int longest)
 {
     const int lane = w.lane;
     const uint32_t vq = w.rd32((uint32_t)q), h = hcw_hash(vq);
@@ -264,25 +302,28 @@ SIMT_DEV HcwHit hcw_search(const Hcw<SMEM>& w, int q, int r, int start_limit, in
     int K = 256;
     HcwHit out{0, 0, 0, 0, 0};
     for (int b0 = 0; ; b0 += 4) {
-        uint32_t cc[4];
+        int cc[4];
 #pragma unroll
         for (int j = 0; j < 4; j++) {                                     // four batches requested at once
-            const int idx = r - 1 - (32 * (b0 + j) + lane);
-            cc[j] = (idx >= 0 && 32 * (b0 + j) + lane < 257) ? simt::ldg_u16(w.sorted + idx) : 0u;
+            const int k = 32 * (b0 + j) + lane;
+            cc[j] = k < 257 ? x.cand(at, q, k) : -1;
         }
         bool ended = false;
 #pragma unroll 1
         for (int j = 0; j < 4 && !ended; j++) {                           // (one copy of the scoring code: the kernel is large enough)
-            const int k = 32 * (b0 + j) + lane, idx = r - 1 - k;
-            uint32_t c = j == 0 ? cc[0] : (j == 1 ? cc[1] : (j == 2 ? cc[2] : cc[3])), vc = 0;
+            const int k = 32 * (b0 + j) + lane;
+            int c = j == 0 ? cc[0] : (j == 1 ? cc[1] : (j == 2 ? cc[2] : cc[3]));
+            uint32_t vc = 0;
             bool inb = false;
-            if (idx >= 0 && k < K) { vc = w.rd32(c); inb = hcw_hash(vc) == h; }
+            if (c >= 0 && k < K) { vc = w.rd32((uint32_t)c); inb = hcw_hash(vc) == h; }
             const uint32_t outm = simt::ballot(HCW_FULL, !inb);
             const int first_out = outm ? simt::ffs(outm) - 1 : 32;
             bool valid = lane < first_out;
-            if (lane == first_out && k < K) { valid = true; c = 0; vc = w.v0; }      // the walk ends at position 0
+            if (lane == first_out && k < K && x.ends_at_0(q)) { valid = true; c = 0; vc = w.v0; }    // the walk ends at position 0
             if (!WIDER && b0 == 0 && j == 0) {
-                const int c_first = (int)simt::shfl(HCW_FULL, c, 0);                  // lane 0 is valid in the first batch
+                // (lane 0 is valid unless the walk ends before its first candidate: then neither K nor the repeat
+                // detector below is used)
+                const int c_first = (int)simt::shfl(HCW_FULL, (uint32_t)c, 0);
                 if (c_first >= q - 4) K = 257;
             }
             uint32_t key = 0, back = 0;
@@ -291,7 +332,7 @@ SIMT_DEV HcwHit hcw_search(const Hcw<SMEM>& w, int q, int r, int start_limit, in
             if (eqm && !(eqm & (eqm - 1u))) {
                 // one matching candidate in the batch (sparse data): the whole warp counts its length, 128 bytes a step
                 const int f = simt::ffs(eqm) - 1;
-                const int cf = (int)simt::shfl(HCW_FULL, c, f);
+                const int cf = (int)simt::shfl(HCW_FULL, (uint32_t)c, f);
                 uint32_t len = 4u + (uint32_t)hcw_common_warp(w, q + 4, cf + 4, w.matchlimit);
                 if (WIDER) {                                              // :505 backwards, a lane per byte
                     int lim = q - start_limit; if (cf < lim) lim = cf;    // steps allowed: startt > startLimit, reft > base
@@ -307,15 +348,15 @@ SIMT_DEV HcwHit hcw_search(const Hcw<SMEM>& w, int q, int r, int start_limit, in
                 }
                 if (eq) key = len * 512u + (511u - (uint32_t)k);
             } else if (eq) {
-                uint32_t len = 4u + (uint32_t)hcw_common(w, q + 4, (int)c + 4, w.matchlimit);
+                uint32_t len = 4u + (uint32_t)hcw_common(w, q + 4, c + 4, w.matchlimit);
                 if (WIDER) {                                              // :505 backwards, four bytes at a time
-                    int lim = q - start_limit; if ((int)c < lim) lim = (int)c;          // steps allowed: startt > startLimit, reft > base
+                    int lim = q - start_limit; if (c < lim) lim = c;      // steps allowed: startt > startLimit, reft > base
                     bool open = true;
                     while (open && (int)back + 4 <= lim) {
-                        const uint32_t x = w.rd32((uint32_t)q - back - 4u) ^ w.rd32(c - back - 4u);
-                        if (x) { back += (uint32_t)simt::clz(x) >> 3; open = false; } else back += 4u;
+                        const uint32_t d = w.rd32((uint32_t)q - back - 4u) ^ w.rd32((uint32_t)c - back - 4u);
+                        if (d) { back += (uint32_t)simt::clz(d) >> 3; open = false; } else back += 4u;
                     }
-                    while (open && (int)back < lim && w.rd8((uint32_t)q - back - 1u) == w.rd8(c - back - 1u)) back++;
+                    while (open && (int)back < lim && w.rd8((uint32_t)q - back - 1u) == w.rd8((uint32_t)c - back - 1u)) back++;
                     len += back;
                 }
                 key = len * 512u + (511u - (uint32_t)k);                  // longest first, then earliest in the walk
@@ -324,12 +365,12 @@ SIMT_DEV HcwHit hcw_search(const Hcw<SMEM>& w, int q, int r, int start_limit, in
             if (bm > best) {
                 const int holder = (int)((511u - (bm & 511u)) & 31u);
                 best = bm;
-                best_c = simt::shfl(HCW_FULL, c, holder);
+                best_c = simt::shfl(HCW_FULL, (uint32_t)c, holder);
                 if (WIDER) best_back = simt::shfl(HCW_FULL, back, holder);
             }
             if (!WIDER && b0 == 0 && j == 0) {                            // :411-420 repeat detector: candidate 0, <= 4 back, matching
                 const uint32_t key0 = simt::shfl(HCW_FULL, key, 0);
-                const int c_first = (int)simt::shfl(HCW_FULL, c, 0);
+                const int c_first = (int)simt::shfl(HCW_FULL, (uint32_t)c, 0);
                 if (key0 && c_first >= q - 4) { out.repl = (int)(key0 >> 9); out.delta = q - c_first; }
             }
             if (first_out < 32) ended = true;
@@ -345,28 +386,30 @@ SIMT_DEV HcwHit hcw_search(const Hcw<SMEM>& w, int q, int r, int start_limit, in
     return out;
 }
 
-// ---- 3. literal scan: the first position in [ip, ip+64) whose walk holds a match ---------------------------------------
+// ---- 3. literal scan: the first position in [ip, end) (end = x.round_end(ip, mflimit)) whose walk holds a match ---------
 // Every lane walks for its own two positions (ip+lane, ip+32+lane), four candidates per memory round trip.  Returns the
 // offset of the first position with a match (a position has one iff some examined candidate has its four bytes: every
-// such candidate yields >= 4, :428-431) or -1, and that position's rank.
-struct HcwScan { int off, rank; };
+// such candidate yields >= 4, :428-431) or -1, and that position's place in the index.
+template <class At>
+struct HcwScan { int off; At at; };
 
-template <bool SMEM>
-SIMT_DEV HcwScan hcw_scan(const Hcw<SMEM>& w, int ip)
+template <bool SMEM, class X>
+SIMT_DEV HcwScan<typename X::At> hcw_scan(const HcwBlock<SMEM>& w, const X& x, int ip, int end)
 {
+    typedef typename X::At At;
     const int lane = w.lane;
-    int q[2], r[2]; bool act[2];
-    uint32_t cand[2][4];
+    int q[2]; bool act[2]; At at[2];
+    int cand[2][4];
 #pragma unroll
     for (int s = 0; s < 2; s++) {
-        q[s] = ip + 32 * s + lane; act[s] = q[s] < w.mflimit;
-        r[s] = act[s] ? (int)simt::ldg_u16(w.rank + q[s]) : 0;
+        q[s] = ip + 32 * s + lane; act[s] = q[s] < end;
+        at[s] = act[s] ? x.at(w, q[s]) : At{};
     }
 #pragma unroll
     for (int s = 0; s < 2; s++)
 #pragma unroll
-        for (int t = 0; t < 4; t++) { const int idx = r[s] - 1 - t; cand[s][t] = (act[s] && idx >= 0) ? simt::ldg_u16(w.sorted + idx) : 0u; }
-    HcwScan res{-1, 0};
+        for (int t = 0; t < 4; t++) cand[s][t] = act[s] ? x.cand(at[s], q[s], t) : -1;
+    HcwScan<At> res{-1, At{}};
 #pragma unroll
     for (int s = 0; s < 2; s++) {
         const uint32_t vq = act[s] ? w.rd32((uint32_t)q[s]) : 0u, h = hcw_hash(vq);
@@ -376,25 +419,30 @@ SIMT_DEV HcwScan hcw_scan(const Hcw<SMEM>& w, int ip)
 #pragma unroll
             for (int t = 0; t < 4; t++) {
                 if (!done) {
-                    const int idx = r[s] - 1 - k;
-                    uint32_t c = cand[s][t], vc = 0;
+                    int c = cand[s][t];
+                    uint32_t vc = 0;
                     bool inb = false;
-                    if (idx >= 0) { vc = w.rd32(c); inb = hcw_hash(vc) == h; }
-                    if (!inb) { c = 0; vc = w.v0; }
-                    if (k == 0 && (int)c >= q[s] - 4) K = 257;
-                    if (vc == vq) { hit = true; done = true; }
-                    else if (!inb) done = true;
-                    else if (++k >= K) done = true;
+                    if (c >= 0) { vc = w.rd32((uint32_t)c); inb = hcw_hash(vc) == h; }
+                    if (!inb) {
+                        if (x.ends_at_0(q[s])) { c = 0; vc = w.v0; }
+                        else done = true;                                 // the walk is over without a match
+                    }
+                    if (!done) {
+                        if (k == 0 && c >= q[s] - 4) K = 257;
+                        if (vc == vq) { hit = true; done = true; }
+                        else if (!inb) done = true;
+                        else if (++k >= K) done = true;
+                    }
                 }
             }
             const uint32_t hits = simt::ballot(HCW_FULL, hit), und = simt::ballot(HCW_FULL, !done);
             const uint32_t below = hits ? ((1u << (simt::ffs(hits) - 1)) - 1u) : HCW_FULL;
             if (!(und & below)) {
-                if (hits) { const int l = simt::ffs(hits) - 1; res.off = 32 * s + l; res.rank = (int)simt::shfl(HCW_FULL, (uint32_t)r[s], l); }
+                if (hits) { const int l = simt::ffs(hits) - 1; res.off = 32 * s + l; res.at = at[s].shfl(l); }
                 break;
             }
 #pragma unroll
-            for (int t = 0; t < 4; t++) { const int idx = r[s] - 1 - k - t; cand[s][t] = (!done && idx >= 0) ? simt::ldg_u16(w.sorted + idx) : 0u; }
+            for (int t = 0; t < 4; t++) cand[s][t] = !done ? x.cand(at[s], q[s], k + t) : -1;
         }
         if (res.off >= 0) break;
     }
@@ -426,7 +474,7 @@ SIMT_NOINLINE void hcw_copy_long_input(uint8_t* dst, const uint8_t* src, uint32_
     group_copy<32, false>(dst, HcwInputSrc{src}, n, lane, HCW_FULL);
 }
 template <bool SMEM>
-SIMT_DEV void hcw_literals(const Hcw<SMEM>& w, uint8_t* dst, int at, int n)
+SIMT_DEV void hcw_literals(const HcwBlock<SMEM>& w, uint8_t* dst, int at, int n)
 {
     if (n < 64) {
         for (int i = w.lane; i < n; i += 32) simt::stg_u8(dst + i, (uint8_t)w.rd8((uint32_t)(at + i)));
@@ -437,7 +485,7 @@ SIMT_DEV void hcw_literals(const Hcw<SMEM>& w, uint8_t* dst, int at, int n)
 }
 
 template <bool SMEM>
-SIMT_DEV bool hcw_emit(const Hcw<SMEM>& w, HcwOut& o, int ml, int ref)       // :521-550 LZ4_encodeSequence; true = output full
+SIMT_DEV bool hcw_emit(const HcwBlock<SMEM>& w, HcwOut& o, int ml, int ref)       // :521-550 LZ4_encodeSequence; true = output full
 {
     const int L = o.ip - o.anchor, tok = o.op++;
     uint32_t tv;
@@ -454,34 +502,28 @@ SIMT_DEV bool hcw_emit(const Hcw<SMEM>& w, HcwOut& o, int ml, int ref)       // 
     return false;
 }
 
-// One block, all 32 lanes.  `sm` = HCW_SMEM_BYTES of shared memory (SMEM variant), `index` = this warp's HCW_INDEX_BYTES.
-// Returns the bytes written, 0 = did not fit, HCW_FALLBACK = not for this kernel (the same value in every lane).
-template <bool SMEM>
-SIMT_DEV int hcw_encode_block(simt::smem_ref sm, void* index, const uint8_t* src, int n, uint8_t* dst, int cap, int lane)
+// ---- 4. the parse (:581-739) over either index, all 32 lanes ----------------------------------------------------------
+// Returns the bytes written, 0 = did not fit, HCW_FALLBACK = a state the index does not describe (the same value in every
+// lane).  x.prepare(w, q) runs before every scan round at q and every wider search at q.
+template <bool SMEM, class X>
+SIMT_DEV int hcw_parse(const HcwBlock<SMEM>& w, X& x, uint8_t* dst, int cap)
 {
-    if (n < 0 || cap < 0) return 0;
-    if (n > HCW_MAX_BLOCK) return HCW_FALLBACK;
-    Hcw<SMEM> w; w.sm = sm; w.rank = (uint16_t*)index; w.sorted = w.rank + 65536; w.cnt = (uint32_t*)(w.sorted + 65536);
-    w.src = src; w.n = n; w.lane = lane; w.in.init(src);
-    w.mflimit = n - 12; w.matchlimit = n - 5;
-    if (w.mflimit > 1) hcw_build(w);
-    if constexpr (SMEM) hcw_stage(w);
-    w.v0 = n >= 4 ? w.rd32(0) : 0u;
+    const int lane = w.lane, n = w.n, mflimit = w.mflimit;
     HcwOut o{dst, cap, 0, 1, 0, lane};                                 // :581 ip = 1
-    const int mflimit = w.mflimit, matchlimit = w.matchlimit;
-    (void)matchlimit;
     int next = 1;                                                      // nextToUpdate (:334)
     int ml, ml2, ml3, ml0, ref = 0, ref2 = 0, ref3 = 0, ref0, start2 = 0, start3 = 0, start0;
-    bool odd = false;                                                  // a state the static index does not describe
+    bool odd = false;                                                  // a state the index does not describe
 
     while (o.ip < mflimit) {                                           // :584
         if (o.ip < next) return HCW_FALLBACK;
-        const HcwScan sc = hcw_scan(w, o.ip);
-        if (sc.off < 0) { next = o.ip + 63 < mflimit ? o.ip + 63 : mflimit - 1; o.ip += 64; continue; }   // 64 x "if (!ml) { ip++; continue; }"
+        x.prepare(w, o.ip);
+        const int end = x.round_end(o.ip, mflimit);
+        const HcwScan<typename X::At> sc = hcw_scan(w, x, o.ip, end);
+        if (sc.off < 0) { next = end - 1; o.ip = end; continue; }     // (end - ip) x "if (!ml) { ip++; continue; }"
         o.ip += sc.off;
         next = o.ip;
         {
-            const HcwHit b = hcw_search<false, SMEM>(w, o.ip, sc.rank, 0, 0);
+            const HcwHit b = hcw_search<false>(w, x, o.ip, sc.at, 0, 0);
             ml = b.len; ref = b.ref;
             if (b.repl) {                                              // :437-455: chain[ip..end) := delta, nextToUpdate = end
                 if (b.delta >= 2) {                                    // equal to the static chain unless two of the period's strings share a hash
@@ -489,8 +531,8 @@ SIMT_DEV int hcw_encode_block(simt::smem_ref sm, void* index, const uint8_t* src
                     const uint32_t h0 = simt::shfl(HCW_FULL, hj, 0), h1 = simt::shfl(HCW_FULL, hj, 1), h2 = simt::shfl(HCW_FULL, hj, 2), h3 = simt::shfl(HCW_FULL, hj, 3);
                     if (h0 == h1 || h0 == h2 || h0 == h3 || h1 == h2 || h1 == h3 || h2 == h3) odd = true;
                 }
-                const int end = o.ip + b.repl - 3;
-                if (end > next) next = end;
+                const int e = o.ip + b.repl - 3;
+                if (e > next) next = e;
             }
         }
         if (odd || !ml) return HCW_FALLBACK;
@@ -514,7 +556,8 @@ SIMT_DEV int hcw_encode_block(simt::smem_ref sm, void* index, const uint8_t* src
             if (wq + (to_search2 ? 2 : 3) < mflimit) {                 // "ip + ml < mflimit" / "start2 + ml2 < mflimit"
                 if (wq < next) return HCW_FALLBACK;
                 next = wq;
-                const HcwHit h = hcw_search<true, SMEM>(w, wq, (int)simt::ldg_u16(w.rank + wq), wlim, wlong);
+                x.prepare(w, wq);
+                const HcwHit h = hcw_search<true>(w, x, wq, x.at(w, wq), wlim, wlong);
                 wml = h.len; wref = h.ref; wstart = h.start;
             }
             if (to_search2) {                                          // _Search2  :594-622
@@ -569,6 +612,23 @@ SIMT_DEV int hcw_encode_block(simt::smem_ref sm, void* index, const uint8_t* src
         o.op += R;
     }
     return o.op;
+}
+
+// One block of at most 64 KiB, all 32 lanes.  `sm` = HCW_SMEM_BYTES of shared memory (SMEM variant), `index` = this warp's
+// HCW_INDEX_BYTES.  Returns what hcw_parse returns; HCW_FALLBACK also for a block above 64 KiB.
+template <bool SMEM>
+SIMT_DEV int hcw_encode_block(simt::smem_ref sm, void* index, const uint8_t* src, int n, uint8_t* dst, int cap, int lane)
+{
+    if (n < 0 || cap < 0) return 0;
+    if (n > HCW_MAX_BLOCK) return HCW_FALLBACK;
+    HcwBlock<SMEM> w; w.sm = sm;
+    w.src = src; w.n = n; w.lane = lane; w.in.init(src);
+    w.mflimit = n - 12; w.matchlimit = n - 5;
+    HcwIndex x; x.rank = (uint16_t*)index; x.sorted = x.rank + 65536;
+    if (w.mflimit > 1) hcw_build(w, x, HcwCounters<SMEM>{sm, (uint32_t*)(x.sorted + 65536), lane});
+    if constexpr (SMEM) hcw_stage(w);
+    w.v0 = n >= 4 ? w.rd32(0) : 0u;
+    return hcw_parse(w, x, dst, cap);
 }
 
 }  // namespace lz4b200
