@@ -153,6 +153,33 @@ int lz4b200_wrap_batch(lz4b200_ctx* ctx, const void* src, const int64_t* src_off
 int lz4b200_unwrap_batch(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
                          void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n);
 
+/* The same packets in device memory, asynchronous on `stream` (no host synchronisation, except that an HC batch may
+ * synchronise once to grow the context's HC arena, as device HC batches do).  A batch already in HBM never crosses PCIe:
+ * the encoders / decoders run as in lz4b200_{encode,decode}_batch(MEM_DEVICE), and the header, the stored-raw rule and
+ * the stored copies run on the device.  Packets and statuses are byte for byte those of the host calls above, so a packet
+ * made on either side, or by lz4net's LZ4Codec.Wrap / WrapHC, is read by the other's Unwrap.
+ *
+ * wrap_batch_device: packet i = Wrap / WrapHC of src + src_off[i] (src_len[i] bytes), written at dst + dst_off[i];
+ *   dst_cap[i] >= src_len[i] + 8.  out_len[i] = packet size (at most src_len[i] + 8), or LZ4B200_E_ARG for that packet
+ *   (negative length, capacity too small), which then has nothing written.  Bytes behind out_len[i] in the slot may be
+ *   overwritten.  For packets back to back, pass the slots and out_len to lz4b200_compact. */
+int lz4b200_wrap_batch_device(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                              int high_compression, void* dst, const int64_t* dst_off, const int32_t* dst_cap,
+                              int32_t* out_len, int32_t n, void* stream);
+/* unwrap_batch_device: packet i = src + src_off[i], src_len[i] bytes, restored to dst + dst_off[i], capacity dst_cap[i].
+ *   out_len[i] = bytes restored, LZ4B200_E_FORMAT or LZ4B200_E_ARG: what lz4b200_unwrap_batch returns for the same packet
+ *   and capacity.  Nothing is written outside [dst_off[i], dst_off[i] + dst_cap[i]). */
+int lz4b200_unwrap_batch_device(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len,
+                                int32_t n, void* stream);
+/* unwrap_batch_packed: unwrap into PACKED output that the library sizes from the headers, with the contract of
+ * lz4b200_decode_batch_packed: out_off[0..n] (int64, n+1 entries) = exclusive prefix sum of max(size, 0), size = the
+ * header's unwrapped size or the packet's negative status.  If out_off[n] <= dst_total_cap, packet i is restored to
+ * dst + out_off[i] and out_len[i] is as in unwrap_batch_device; otherwise dst is untouched and out_len holds the sizes. */
+int lz4b200_unwrap_batch_packed(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len,
+                                int32_t n, void* stream);
+
 /* ---- host buffers the caller keeps for a while (a pinned byte[] behind a GCHandle, a native arena) --------------------
  * Host-memory batches copy straight from / to the caller's buffers.  From pageable memory the driver stages every copy
  * through its own pinned bounce buffers, synchronously; page-locking a long-lived buffer once (cudaHostRegister) lets the

@@ -61,6 +61,40 @@ def decode_packed(ctx: Context, comp: torch.Tensor, src_off, src_len, out: torch
                  "decode_batch_packed")
 
 
+def wrap(ctx: Context, raw: torch.Tensor, src_off, src_len, packets: torch.Tensor, dst_off, dst_cap, out_len, hc: bool = False):
+    """LZ4Codec.Wrap / WrapHC packets in device memory (lz4b200_wrap_batch_device): packet i of input i lands at
+    packets + dst_off[i] (dst_cap[i] >= src_len[i] + 8); out_len[i] = its size or LZ4B200_E_ARG.  Asynchronous on the
+    current torch stream."""
+    native.check(native.lib().lz4b200_wrap_batch_device(ctx.handle, _p(raw), _p(src_off), _p(src_len), int(hc), _p(packets),
+                                                        _p(dst_off), _p(dst_cap), _p(out_len), src_off.numel(), _stream()),
+                 "wrap_batch_device")
+
+
+def wrap_packed(ctx: Context, raw: torch.Tensor, src_off, src_len, slots: torch.Tensor, slot_off, slot_cap, out_len,
+                packed: torch.Tensor, out_off, hc: bool = False):
+    """wrap() into the slots, then compact(): the packets back to back at packed + out_off[i] (int64[n+1], out_off[n] =
+    the total).  A packet with a negative out_len occupies no bytes.  Asynchronous on the current torch stream."""
+    wrap(ctx, raw, src_off, src_len, slots, slot_off, slot_cap, out_len, hc=hc)
+    compact(ctx, slots, slot_off, out_len, packed, out_off)
+
+
+def unwrap(ctx: Context, packets: torch.Tensor, src_off, src_len, out: torch.Tensor, dst_off, dst_cap, out_len):
+    """Mirror image of wrap() (lz4b200_unwrap_batch_device): out_len[i] = bytes restored, LZ4B200_E_FORMAT or E_ARG.
+    Asynchronous on the current torch stream."""
+    native.check(native.lib().lz4b200_unwrap_batch_device(ctx.handle, _p(packets), _p(src_off), _p(src_len), _p(out),
+                                                          _p(dst_off), _p(dst_cap), _p(out_len), src_off.numel(), _stream()),
+                 "unwrap_batch_device")
+
+
+def unwrap_packed(ctx: Context, packets: torch.Tensor, src_off, src_len, out: torch.Tensor, out_off, out_len):
+    """Unwrap into packed output sized from the headers (lz4b200_unwrap_batch_packed), in the shape of decode_packed:
+    packet i lands at out + out_off[i] when out_off[n] fits out.numel() bytes; otherwise out is untouched and out_len
+    holds the sizes.  Asynchronous on the current torch stream."""
+    native.check(native.lib().lz4b200_unwrap_batch_packed(ctx.handle, _p(packets), _p(src_off), _p(src_len), _p(out), out.numel(),
+                                                          _p(out_off), _p(out_len), src_off.numel(), _stream()),
+                 "unwrap_batch_packed")
+
+
 def compact(ctx: Context, slots: torch.Tensor, slot_off, lens, packed, out_off):
     """out_off: int64[n+1]; packed may be None to compute only the offsets."""
     native.check(native.lib().lz4b200_compact(ctx.handle, _p(slots), _p(slot_off), _p(lens),

@@ -119,6 +119,7 @@ struct lz4b200_ctx {
     int next_counter = 0;
     DevBuf hc_arena, compact_tmp;
     DevBuf packed_caps;                    // lz4b200_decode_batch_packed: per-block capacities + the "fits" flag (serialised like compact_tmp)
+    DevBuf wrap_tmp;                       // the device Wrap / Unwrap calls: the codec's view of the packets (serialised like compact_tmp)
     cudaEvent_t hc_done = nullptr;         // the HC state arena is shared: HC launches are chained through this event
     cudaEvent_t compact_done = nullptr;    // likewise the scan scratch of lz4b200_compact
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
@@ -397,6 +398,35 @@ int single(const char* source, char* dest, int isize, int ocap, int op)
     return out;
 }
 
+// The device Wrap / Unwrap calls: the context's scratch for n packets (with `packed`, also the scan scratch and the
+// capacities + "fits" flag of the packed unwrap), grown like compact_tmp, and `st` ordered behind the previous call that
+// used it (on whatever stream).  The caller holds the lock and records compact_done on `st` when its launches are in.
+int frame_scratch(lz4b200_ctx* c, int32_t n, bool packed, cudaStream_t st, WrapScratch* w)
+{
+    const size_t nn = (size_t)n;
+    const size_t need = nn * sizeof(int64_t) + 3 * nn * sizeof(int32_t);
+    const size_t caps_bytes = sizeof(int32_t) * (nn + 1);
+    if (need > c->wrap_tmp.cap || (packed && (compact_tmp_bytes(n) > c->compact_tmp.cap || caps_bytes > c->packed_caps.cap))) {
+        CU(cudaDeviceSynchronize());               // the scratch may still be in use by an earlier call
+        CU(c->wrap_tmp.reserve(need));
+        if (packed) { CU(c->compact_tmp.reserve(compact_tmp_bytes(n))); CU(c->packed_caps.reserve(caps_bytes)); }
+    }
+    CU(cudaStreamWaitEvent(st, c->compact_done, 0));
+    w->off = (int64_t*)c->wrap_tmp.p;
+    w->len = (int32_t*)(w->off + n);
+    w->cap = w->len + n;
+    w->res = w->cap + n;
+    return LZ4B200_OK;
+}
+
+// argument checks, the lock and the device of the device Wrap / Unwrap calls (n > 0)
+#define FRAME_CALL_PROLOGUE(c, n)                                                                     \
+    if (!(c)) return fail(LZ4B200_E_ARG, "null context");                                             \
+    if ((n) < 0) return fail(LZ4B200_E_ARG, "negative packet count");                                 \
+    std::lock_guard<std::mutex> lock((c)->mu);                                                        \
+    DeviceGuard g((c)->device);                                                                       \
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+
 }  // namespace
 
 extern "C" {
@@ -458,7 +488,7 @@ void lz4b200_destroy(lz4b200_ctx* c)
         if (s.done) cudaEventDestroy(s.done);
         if (s.stream) cudaStreamDestroy(s.stream);
     }
-    c->hc_arena.release(); c->compact_tmp.release(); c->packed_caps.release();
+    c->hc_arena.release(); c->compact_tmp.release(); c->packed_caps.release(); c->wrap_tmp.release();
     if (c->hc_done) cudaEventDestroy(c->hc_done);
     if (c->compact_done) cudaEventDestroy(c->compact_done);
     if (c->counters) cudaFree(c->counters);
@@ -554,6 +584,76 @@ int lz4b200_compact(lz4b200_ctx* c, const void* slots, const int64_t* slot_off, 
     cudaError_t e = launch_compact((const uint8_t*)slots, slot_off, len, (uint8_t*)packed, out_off, n,
                                    c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "compact launch");
+    CU(cudaEventRecord(c->compact_done, st));
+    return LZ4B200_OK;
+}
+
+// ---- Wrap / Unwrap packets in device memory (lz4_wrap.cuh): prep -> the batch codec, unchanged -> finish, on `stream` ----
+int lz4b200_wrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, int high_compression,
+                              void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
+{
+    FRAME_CALL_PROLOGUE(c, n)
+    if (n == 0) return LZ4B200_OK;
+    if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    WrapScratch w;
+    int rc = frame_scratch(c, n, false, st, &w); if (rc) return rc;
+    const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
+    cudaError_t e = launch_wrap_prep(a, w, st, &c->launches);
+    if (e != cudaSuccess) return cuda_fail(e, "wrap prep launch");
+    // every packet's payload, capacity = its input length (LZ4Codec.cs:518-523); the same path as lz4b200_encode_batch(MEM_DEVICE)
+    const BatchArgs enc{(const uint8_t*)src, src_off, w.len, (uint8_t*)dst, w.off, w.cap, w.res, n};
+    rc = run_device(c, enc, high_compression ? 1 : 0, st); if (rc) return rc;
+    e = launch_wrap_finish(a, w, st, &c->launches);
+    if (e != cudaSuccess) return cuda_fail(e, "wrap finish launch");
+    CU(cudaEventRecord(c->compact_done, st));
+    return LZ4B200_OK;
+}
+
+int lz4b200_unwrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                                const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
+{
+    FRAME_CALL_PROLOGUE(c, n)
+    if (n == 0) return LZ4B200_OK;
+    if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    WrapScratch w;
+    int rc = frame_scratch(c, n, false, st, &w); if (rc) return rc;
+    const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
+    cudaError_t e = launch_unwrap_prep(a, w, st, &c->launches);
+    if (e != cudaSuccess) return cuda_fail(e, "unwrap prep launch");
+    // the compressed packets, known size (LZ4Codec.cs:595); stored and rejected ones are neutral entries
+    const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, dst_off, w.cap, w.res, n};
+    rc = run_device(c, dec, 2, st); if (rc) return rc;
+    e = launch_unwrap_finish(a, w, nullptr, st, &c->launches);
+    if (e != cudaSuccess) return cuda_fail(e, "unwrap finish launch");
+    CU(cudaEventRecord(c->compact_done, st));
+    return LZ4B200_OK;
+}
+
+// sizes from the headers -> scan into out_off -> capacities + "fits" -> decode and stored copies, both behind the flag
+int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                                int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n, void* stream)
+{
+    FRAME_CALL_PROLOGUE(c, n)
+    if (!out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
+    if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
+    WrapScratch w;
+    int rc = frame_scratch(c, n, true, st, &w); if (rc) return rc;
+    int32_t* caps = (int32_t*)c->packed_caps.p;
+    int* fits = (int*)(caps + n);
+    const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, nullptr, out_len, n};
+    cudaError_t e = launch_unwrap_prep(a, w, st, &c->launches);
+    if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, out_len, nullptr, out_off, n, c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
+    if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, caps, fits, st, &c->launches);
+    if (e == cudaSuccess) {
+        const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, out_off, caps, w.res, n};
+        e = launch_decode(dec, true, c->decode_lanes_auto ? 0 : c->decode_lanes, c->counter(), c->dev, st, &c->launches, fits);
+    }
+    if (e == cudaSuccess) e = launch_unwrap_finish(a, w, fits, st, &c->launches);
+    if (e != cudaSuccess) return cuda_fail(e, "packed unwrap launch");
     CU(cudaEventRecord(c->compact_done, st));
     return LZ4B200_OK;
 }

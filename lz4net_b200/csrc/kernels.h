@@ -48,6 +48,16 @@ cudaError_t launch_compact(const uint8_t* slots, const int64_t* slot_off, const 
                            int64_t* out_off, int32_t n_blocks, void* scan_tmp, size_t scan_tmp_bytes,
                            const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 size_t      compact_tmp_bytes(int32_t n_blocks);
+// Wrap / Unwrap packets in device memory (wrap.cu, lz4_wrap.cuh).  The scratch holds the codec's view of the batch: payload
+// offsets, lengths and capacities per packet, and the codec's per-packet results.
+struct WrapScratch { int64_t* off; int32_t* len; int32_t* cap; int32_t* res; };
+// a = the caller's batch (src_off / src_len / dst_off / dst_cap / out_len of the packets)
+cudaError_t launch_wrap_prep(const BatchArgs& a, const WrapScratch& w, cudaStream_t stream, int64_t* launches);
+cudaError_t launch_wrap_finish(const BatchArgs& a, const WrapScratch& w, cudaStream_t stream, int64_t* launches);
+// a.dst_cap may be null (no limit: the packed unwrap); out_len[i] = the packet's size or status until the finish step
+cudaError_t launch_unwrap_prep(const BatchArgs& a, const WrapScratch& w, cudaStream_t stream, int64_t* launches);
+// gate (optional): a device int; when it reads 0 the kernel returns at once
+cudaError_t launch_unwrap_finish(const BatchArgs& a, const WrapScratch& w, const int* gate, cudaStream_t stream, int64_t* launches);
 cudaError_t launch_synth(uint8_t* dst, int64_t n_blocks, int32_t block_size, int cls, uint64_t seed, int64_t first_block,
                          const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 
