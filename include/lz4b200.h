@@ -33,6 +33,18 @@ extern "C" {
 /* where the buffers of a batch call live */
 #define LZ4B200_MEM_HOST   0           /* src/dst/offset/length arrays are host memory; copies are inside the call */
 #define LZ4B200_MEM_DEVICE 1           /* everything is device memory on the context's GPU; the call only enqueues */
+/* Mixed memory (encode_batch / decode_batch; not measure_batch, which has no destination).  The offset, length and out_len
+ * arrays are host memory.  Only compressed bytes cross PCIe, in one direction; device scratch stays at the host pipeline's
+ * per-stage size whatever the batch.  Contract of every mixed call:
+ *   - synchronous, like MEM_HOST;
+ *   - its device reads and writes are ordered after all work enqueued on `stream` before the call (a kernel that fills
+ *     src, or one still reading the old contents of dst), and every device access is complete when it returns;
+ *   - out_len[i] and the bytes block i produced equal what MEM_DEVICE and MEM_HOST give for the same block;
+ *   - a host destination receives only the bytes each block produced, as with MEM_HOST; a device destination is written
+ *     only inside [dst_off[i], dst_off[i] + dst_cap[i]), as with MEM_DEVICE;
+ *   - LZ4B200_E_ARG when the device side is not memory of the context's GPU, or the host side is device memory. */
+#define LZ4B200_MEM_DEVICE_TO_HOST 2   /* src: device memory of the context's GPU; dst: host memory, pageable or page-locked */
+#define LZ4B200_MEM_HOST_TO_DEVICE 3   /* src: host memory; dst: device memory of the context's GPU */
 
 /* status codes (batch / context calls).  Per-block results are reported in out_len[], never here. */
 #define LZ4B200_OK            0
@@ -66,7 +78,8 @@ int  lz4b200_compress_bound(int input_size);
  * decode:  known_len != 0 -> LZ4_uncompress (dst_cap[i] is the exact decoded size; out_len[i] = bytes read,
  *                            the caller compares it with src_len[i] like src/LZ4cc/LZ4Codec.64.cpp:88-93);
  *          known_len == 0 -> LZ4_uncompress_unknownOutputSize (dst_cap[i] = capacity; out_len[i] = bytes written).
- * MEM_DEVICE: asynchronous on `stream`; MEM_HOST: synchronous, chunked + overlapped copies inside the call.
+ * MEM_DEVICE: asynchronous on `stream`; MEM_HOST: synchronous, chunked + overlapped copies inside the call;
+ * MEM_DEVICE_TO_HOST / MEM_HOST_TO_DEVICE: synchronous like MEM_HOST, ordered behind `stream` (see above).
  * Returns LZ4B200_OK or a negative status; malformed / too-small blocks are NOT a call failure. */
 int lz4b200_encode_batch(lz4b200_ctx* ctx,
                          const void* src, const int64_t* src_off, const int32_t* src_len,
@@ -86,7 +99,8 @@ int lz4b200_decode_batch(lz4b200_ctx* ctx,
  *
  * measure_batch: out_len[i] = what lz4b200_decode_batch (same arguments) would store; nothing is decoded or written.
  *   Non-negative values are equal, negative ones agree in sign.  dst_cap may be NULL when known_len == 0 (capacity
- *   INT32_MAX per block; LZ4B200_E_ARG otherwise).  MEM_DEVICE: asynchronous on `stream`; MEM_HOST: synchronous. */
+ *   INT32_MAX per block; LZ4B200_E_ARG otherwise).  MEM_DEVICE: asynchronous on `stream`; MEM_HOST: synchronous; the
+ *   mixed values are LZ4B200_E_ARG. */
 int lz4b200_measure_batch(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
                           const int32_t* dst_cap, int32_t* out_len, int32_t n_blocks, int known_len, int mem, void* stream);
 
@@ -111,6 +125,15 @@ int lz4b200_encode_batch_packed(lz4b200_ctx* ctx,
                                 const void* src, const int64_t* src_off, const int32_t* src_len, const int32_t* dst_cap,
                                 void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len,
                                 int32_t n_blocks, int mode);
+
+/* The same with src in device memory of the context's GPU (the offload of data that lives in HBM): the contract of
+ * lz4b200_encode_batch_packed -- out_off[0..n], only the produced bytes land in dst (host memory, pageable or
+ * page-locked), LZ4B200_E_ARG when dst_total_cap is too small -- plus that of every mixed call (MEM_DEVICE_TO_HOST above):
+ * synchronous, ordered behind `stream`, no copy of src. */
+int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* ctx,
+                                            const void* src, const int64_t* src_off, const int32_t* src_len,
+                                            const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                            int32_t* out_len, int32_t n_blocks, int mode, void* stream);
 
 /* Compaction of fixed-stride encoder slots into one contiguous payload (device memory only): the batched form of
  * the Buffer.BlockCopy trim in LZ4Codec.Encode (src/LZ4/LZ4Codec.cs:357-364).  out_off[i] (int64, n_blocks+1

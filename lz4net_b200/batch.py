@@ -6,9 +6,14 @@ one block at a time, src/LZ4/LZ4Stream.cs:239-269).  Layouts:
 * raw blocks      uint8[n_blocks * block_size], block i at i * block_size
 * encoder slots   uint8[n_blocks * slot], slot = MaximumOutputLength(block_size) (or block_size for LZ4Stream/Wrap caps)
 * packed payload  uint8[sum(len)], block i at off[i] (exclusive prefix sum, int64[n_blocks + 1])
+
+The mixed-memory helpers (encode_to_host, encode_to_host_packed, decode_from_host) take the device side as a torch CUDA
+tensor and the host side -- data, offsets, lengths, results -- as numpy arrays.  They are synchronous, ordered behind the
+work already queued on the current torch stream, and move only compressed bytes over PCIe.
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 from . import native
@@ -16,6 +21,19 @@ from .codec import Context
 
 
 def _p(t: torch.Tensor) -> int:
+    return t.data_ptr()
+
+
+def _h(a: np.ndarray, dtype, n: int = 0) -> int:
+    """Address of a host array that the library reads or writes in place: C-contiguous, of this dtype, >= n items."""
+    if not (isinstance(a, np.ndarray) and a.dtype == dtype and a.flags.c_contiguous and a.size >= n):
+        raise TypeError(f"expected a C-contiguous numpy {np.dtype(dtype).name} array of at least {n} items")
+    return a.ctypes.data
+
+
+def _d(t: torch.Tensor) -> int:
+    if not (isinstance(t, torch.Tensor) and t.is_cuda):
+        raise TypeError("expected a torch CUDA tensor")
     return t.data_ptr()
 
 
@@ -93,6 +111,38 @@ def unwrap_packed(ctx: Context, packets: torch.Tensor, src_off, src_len, out: to
     native.check(native.lib().lz4b200_unwrap_batch_packed(ctx.handle, _p(packets), _p(src_off), _p(src_len), _p(out), out.numel(),
                                                           _p(out_off), _p(out_len), src_off.numel(), _stream()),
                  "unwrap_batch_packed")
+
+
+def encode_to_host(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, out_len, hc: bool = False):
+    """Blocks of a device tensor encoded into slots of a host array (lz4b200_encode_batch, MEM_DEVICE_TO_HOST): block i
+    reads raw + src_off[i] and its compressed bytes land at dst + dst_off[i] (only the out_len[i] bytes it produced).
+    src_off / dst_off int64, src_len / dst_cap / out_len int32 numpy arrays."""
+    n = len(src_off)
+    ctx.encode_batch_ptr(_d(raw), _h(src_off, np.int64), _h(src_len, np.int32, n), _h(dst, np.uint8), _h(dst_off, np.int64, n),
+                         _h(dst_cap, np.int32, n), _h(out_len, np.int32, n), n, hc=hc, stream=_stream(),
+                         mem=native.MEM_DEVICE_TO_HOST)
+
+
+def encode_to_host_packed(ctx: Context, raw: torch.Tensor, src_off, src_len, dst_cap, dst: np.ndarray, out_off, out_len,
+                          hc: bool = False) -> int:
+    """The same, packed (lz4b200_encode_batch_packed_from_device): block i's bytes land at dst + out_off[i], back to back in
+    block order, out_off (int64[n+1]) [n] = the total, which is returned.  Raises when the total exceeds dst.nbytes."""
+    n = len(src_off)
+    native.check(native.lib().lz4b200_encode_batch_packed_from_device(
+        ctx.handle, _d(raw), _h(src_off, np.int64), _h(src_len, np.int32, n), _h(dst_cap, np.int32, n), _h(dst, np.uint8),
+        dst.nbytes, _h(out_off, np.int64, n + 1), _h(out_len, np.int32, n), n,
+        native.MODE_HC if hc else native.MODE_FAST, _stream()), "encode_batch_packed_from_device")
+    return int(out_off[n])
+
+
+def decode_from_host(ctx: Context, comp: np.ndarray, src_off, src_len, out: torch.Tensor, dst_off, dst_cap, out_len,
+                     known: bool = True):
+    """Compressed blocks in a host array decoded into a device tensor (lz4b200_decode_batch, MEM_HOST_TO_DEVICE): block i
+    reads comp + src_off[i] and is decoded in place at out + dst_off[i], nothing written outside its dst_cap[i] bytes."""
+    n = len(src_off)
+    ctx.decode_batch_ptr(_h(comp, np.uint8), _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), _h(dst_off, np.int64, n),
+                         _h(dst_cap, np.int32, n), _h(out_len, np.int32, n), n, known=known, stream=_stream(),
+                         mem=native.MEM_HOST_TO_DEVICE)
 
 
 def compact(ctx: Context, slots: torch.Tensor, slot_off, lens, packed, out_off):

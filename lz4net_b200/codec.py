@@ -73,15 +73,19 @@ class Context:
         return int(native.lib().lz4b200_launch_count(self._h))
 
     # ---- batched calls on raw pointers -------------------------------------------------------------------------
-    def encode_batch_ptr(self, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, hc=False, device=True, stream=0):
+    # mem: one of native.MEM_*; when None, device=True means MEM_DEVICE and device=False MEM_HOST
+    @staticmethod
+    def _mem(device, mem):
+        return mem if mem is not None else native.MEM_DEVICE if device else native.MEM_HOST
+
+    def encode_batch_ptr(self, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, hc=False, device=True, stream=0, mem=None):
         native.check(native.lib().lz4b200_encode_batch(self._h, src, src_off, src_len, dst, dst_off, dst_cap, out_len, int(n),
                                                        native.MODE_HC if hc else native.MODE_FAST,
-                                                       native.MEM_DEVICE if device else native.MEM_HOST, stream), "encode_batch")
+                                                       self._mem(device, mem), stream), "encode_batch")
 
-    def decode_batch_ptr(self, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, known=True, device=True, stream=0):
+    def decode_batch_ptr(self, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, known=True, device=True, stream=0, mem=None):
         native.check(native.lib().lz4b200_decode_batch(self._h, src, src_off, src_len, dst, dst_off, dst_cap, out_len, int(n),
-                                                       1 if known else 0,
-                                                       native.MEM_DEVICE if device else native.MEM_HOST, stream), "decode_batch")
+                                                       1 if known else 0, self._mem(device, mem), stream), "decode_batch")
 
     def measure_batch_ptr(self, src, src_off, src_len, dst_cap, out_len, n, known=False, device=True, stream=0):
         native.check(native.lib().lz4b200_measure_batch(self._h, src, src_off, src_len, dst_cap, out_len, int(n), 1 if known else 0,

@@ -3,7 +3,9 @@
 // Every call on host memory (the batches with LZ4B200_MEM_HOST, the packed encode, the measure pass, the single-block entry points and the
 // framing in framing.cpp) goes through one software pipeline, run_host: the block list is cut into chunks, and for each
 // chunk H2D(inputs) -> kernel -> D2H(outputs) is enqueued on one of NSLOT streams, so that the copy engines (both PCIe
-// directions) and the SMs work on different chunks at the same time.  There is no CPU codec in this library: if the
+// directions) and the SMs work on different chunks at the same time.  The mixed-memory batches (MEM_DEVICE_TO_HOST,
+// MEM_HOST_TO_DEVICE and the packed encode from device memory) go through it too, skipping the copy of whichever side is
+// already on the device.  There is no CPU codec in this library: if the
 // device or the kernel image is unusable every entry point reports an error.
 #include "../../include/lz4b200.h"
 #include "kernels.h"
@@ -122,6 +124,7 @@ struct lz4b200_ctx {
     DevBuf wrap_tmp;                       // the device Wrap / Unwrap calls: the codec's view of the packets (serialised like compact_tmp)
     cudaEvent_t hc_done = nullptr;         // the HC state arena is shared: HC launches are chained through this event
     cudaEvent_t compact_done = nullptr;    // likewise the scan scratch of lz4b200_compact
+    cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
     bool decode_lanes_auto = true;         // host-memory batches: chosen per chunk from the compression ratio
     int encode_ctas_per_sm = 0;            // encoder warps (= blocks in flight) per SM: 0 = as many as shared memory holds tables for (14)
@@ -203,20 +206,29 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
 //             into the slot's pinned buffer, scattered to dst + dst_off[i] from there;
 //  APPEND     the packed encode (dst_off == nullptr): compacted likewise and appended at dst + written (straight into dst
 //             when it is page-locked); out_off[i] receives block i's offset there, out_off[n] the total.
+// Mixed memory: src_dev = the source is already device memory (the kernels read the caller's buffer at the caller's
+// offsets; nothing is staged), dst_dev = the destination is device memory (the kernels write the caller's slots in place;
+// nothing is compacted or landed, only out_len comes back: NONE).  A chunk is weighed by what it stages, so the slots'
+// device buffers stay within host_chunk_bytes whatever the batch.  The slots start behind everything enqueued on
+// `caller` before the call: a producer of src, or a reader of dst's old contents.
 int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
              const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op,
-             int64_t* out_off, int64_t dst_total_cap)
+             int64_t* out_off, int64_t dst_total_cap, bool src_dev = false, bool dst_dev = false, cudaStream_t caller = nullptr)
 {
     const bool measure = op >= 4;
     for (int32_t i = 0; i < n; i++)
         if (src_len[i] < 0 || (dst_cap && dst_cap[i] < 0)) return fail(LZ4B200_E_ARG, "negative block length");
-    const bool src_pageable = is_pageable(src), dst_pageable = !measure && is_pageable(dst);
+    const bool src_pageable = !src_dev && is_pageable(src), dst_pageable = !measure && !dst_dev && is_pageable(dst);
     enum Mode { NONE, PER_BLOCK, RUNS, SCATTER, APPEND };
     struct Pending { int32_t b0, b1; Mode mode; };
     Pending pend[NSLOT]; bool busy[NSLOT] = {false, false, false};
     int32_t b0 = 0; int k = 0; int64_t written = 0;
     // whatever happens, nothing of this call is still in flight when it returns (the staging buffers are reused)
     struct Drain { lz4b200_ctx* c; ~Drain() { for (int i = 0; i < NSLOT; i++) cudaStreamSynchronize(c->slot[i].stream); } } drain{c};
+    if (src_dev || dst_dev) {
+        CU(cudaEventRecord(c->entry, caller));
+        for (int i = 0; i < NSLOT; i++) CU(cudaStreamWaitEvent(c->slot[i].stream, c->entry, 0));
+    }
 
     // RUNS: fn(offset in dst, offset in the chunk's dense layout, bytes) for every non-empty maximal run of adjacent slots
     auto for_runs = [&](int32_t c0, int32_t c1, const int64_t* dof, const std::function<int(int64_t, int64_t, size_t)>& fn) -> int {
@@ -281,10 +293,10 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
     };
 
     while (b0 < n) {
-        // ---- pick the chunk [b0, b1): bounded src + dst bytes ----
+        // ---- pick the chunk [b0, b1): bounded staged src + dst bytes ----
         int64_t bytes = 0; int32_t b1 = b0;
         while (b1 < n) {
-            const int64_t w = (int64_t)src_len[b1] + (measure ? 0 : dst_cap[b1]);
+            const int64_t w = (src_dev ? 0 : (int64_t)src_len[b1]) + (measure || dst_dev ? 0 : dst_cap[b1]);
             if (b1 > b0 && bytes + w > (int64_t)c->host_chunk_bytes) break;
             bytes += w; b1++;
         }
@@ -292,24 +304,30 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         int rc = retire(s); if (rc) return rc;
         Slot& sl = c->slot[s];
         const int32_t m = b1 - b0;
-        const Mode mode = measure ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == 2 ? RUNS : SCATTER;
+        const Mode mode = measure || dst_dev ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == 2 ? RUNS : SCATTER;
         CU(sl.meta.reserve((size_t)m * 28)); CU(sl.hmeta.reserve((size_t)m * 28 + sizeof(int64_t) * (size_t)(m + 2)));
         const Meta h(sl.hmeta.p, m), d(sl.meta.p, m);
-        int64_t slo = INT64_MAX, shi = INT64_MIN, dsum = 0;
-        for (int32_t i = b0; i < b1; i++) { slo = std::min(slo, src_off[i]); shi = std::max(shi, src_off[i] + src_len[i]); }
+        int64_t slo = 0, shi = 0, dsum = 0;
+        if (!src_dev) {
+            slo = INT64_MAX; shi = INT64_MIN;
+            for (int32_t i = b0; i < b1; i++) { slo = std::min(slo, src_off[i]); shi = std::max(shi, src_off[i] + src_len[i]); }
+        }
         for (int32_t i = 0; i < m; i++) {
-            h.so[i] = src_off[b0 + i] - slo; h.dof[i] = dsum; dsum += measure ? 0 : dst_cap[b0 + i];
+            h.so[i] = src_off[b0 + i] - slo;
+            if (dst_dev) h.dof[i] = dst_off[b0 + i];
+            else { h.dof[i] = dsum; dsum += measure ? 0 : dst_cap[b0 + i]; }
             h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap ? dst_cap[b0 + i] : INT32_MAX;
         }
         const size_t sbytes = (size_t)(shi - slo);
-        CU(sl.src.reserve(sbytes + 64)); CU(sl.dst.reserve((size_t)dsum + 64));
+        if (!src_dev) CU(sl.src.reserve(sbytes + 64));
+        if (!dst_dev) CU(sl.dst.reserve((size_t)dsum + 64));
         CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, (size_t)m * 24, cudaMemcpyHostToDevice, sl.stream));
         if (sbytes) {
             const uint8_t* from = src + slo;
             if (src_pageable && m > 8) { CU(sl.hsrc.reserve(sbytes)); par_memcpy(sl.hsrc.p, from, sbytes); from = (const uint8_t*)sl.hsrc.p; }
             CU(cudaMemcpyAsync(sl.src.p, from, sbytes, cudaMemcpyHostToDevice, sl.stream));
         }
-        const BatchArgs a{(const uint8_t*)sl.src.p, d.so, d.sl, (uint8_t*)sl.dst.p, d.dof, d.dc, d.out, m};
+        const BatchArgs a{src_dev ? src : (const uint8_t*)sl.src.p, d.so, d.sl, dst_dev ? dst : (uint8_t*)sl.dst.p, d.dof, d.dc, d.out, m};
         int lanes = 0;
         if ((op == 2 || op == 3) && c->decode_lanes_auto) {
             double cs = 0, rs = 0;
@@ -345,8 +363,22 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
     return LZ4B200_OK;
 }
 
+// The side of a mixed-memory call that must be device memory is memory of the context's device (plain or managed); the
+// side that must be host memory is not device memory (pageable, page-locked or managed host memory all copy).
+int check_side(const lz4b200_ctx* c, const void* p, bool device, const char* what)
+{
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+    const bool on_device = a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+    if (device && !(on_device && a.device == c->device))
+        return fail(LZ4B200_E_ARG, std::string(what) + " must be device memory of the context's GPU");
+    if (!device && a.type == cudaMemoryTypeDevice) return fail(LZ4B200_E_ARG, std::string(what) + " must be host memory");
+    return LZ4B200_OK;
+}
+
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
-// packed host encode (lz4b200_encode_batch_packed); the measure pass (op 4 / 5) has no dst, dst_off or out_off.
+// packed encode (lz4b200_encode_batch_packed, or its _from_device form with MEM_DEVICE_TO_HOST); the measure pass
+// (op 4 / 5) has no dst, dst_off or out_off.
 int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
           const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op, int mem, void* stream,
           int64_t* out_off = nullptr, int64_t dst_total_cap = 0)
@@ -364,8 +396,17 @@ int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t
         BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
         return run_device(c, a, op, (cudaStream_t)stream);
     }
-    if (mem != LZ4B200_MEM_HOST) return fail(LZ4B200_E_ARG, "mem must be LZ4B200_MEM_HOST or LZ4B200_MEM_DEVICE");
-    return run_host(c, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, op, out_off, dst_total_cap);
+    const bool src_dev = mem == LZ4B200_MEM_DEVICE_TO_HOST, dst_dev = mem == LZ4B200_MEM_HOST_TO_DEVICE;
+    if (mem != LZ4B200_MEM_HOST && !src_dev && !dst_dev)
+        return fail(LZ4B200_E_ARG, "mem must be LZ4B200_MEM_HOST, _DEVICE, _DEVICE_TO_HOST or _HOST_TO_DEVICE");
+    if (src_dev || dst_dev) {
+        // the measure pass has no destination: MEM_HOST and MEM_DEVICE already cover both places its source can be
+        if (measure) return fail(LZ4B200_E_ARG, "measure_batch takes LZ4B200_MEM_HOST or LZ4B200_MEM_DEVICE");
+        int rc = check_side(c, src, src_dev, "src"); if (rc) return rc;
+        rc = check_side(c, dst, dst_dev, "dst"); if (rc) return rc;
+    }
+    return run_host(c, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, op, out_off, dst_total_cap,
+                    src_dev, dst_dev, (cudaStream_t)stream);
 }
 
 // The single-block entry points are re-entrant like the reference's (SURVEY 8b "Threading"): every calling thread gets
@@ -468,6 +509,7 @@ int lz4b200_create(lz4b200_ctx** out, int device)
     cudaError_t e = cudaMalloc(&c->counters, sizeof(uint32_t) * NCOUNTER);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->hc_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->compact_done, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->entry, cudaEventDisableTiming);
     for (int i = 0; i < NSLOT && e == cudaSuccess; i++) {
         e = cudaStreamCreateWithFlags(&c->slot[i].stream, cudaStreamNonBlocking);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->slot[i].done, cudaEventDisableTiming);
@@ -491,6 +533,7 @@ void lz4b200_destroy(lz4b200_ctx* c)
     c->hc_arena.release(); c->compact_tmp.release(); c->packed_caps.release(); c->wrap_tmp.release();
     if (c->hc_done) cudaEventDestroy(c->hc_done);
     if (c->compact_done) cudaEventDestroy(c->compact_done);
+    if (c->entry) cudaEventDestroy(c->entry);
     if (c->counters) cudaFree(c->counters);
     delete c;
 }
@@ -520,6 +563,18 @@ int lz4b200_encode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
     return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, mode == LZ4B200_MODE_HC ? 1 : 0, LZ4B200_MEM_HOST,
                  nullptr, out_off, dst_total_cap);
+}
+
+int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                            const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                            int32_t* out_len, int32_t n, int mode, void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
+    if (n < 0 || !out_off) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
+    return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, mode == LZ4B200_MODE_HC ? 1 : 0,
+                 LZ4B200_MEM_DEVICE_TO_HOST, stream, out_off, dst_total_cap);
 }
 
 int lz4b200_decode_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,

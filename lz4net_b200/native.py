@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.path.join(_HERE, "liblz4b200.so")
 
 MODE_FAST, MODE_HC = 0, 1
-MEM_HOST, MEM_DEVICE = 0, 1
+MEM_HOST, MEM_DEVICE, MEM_DEVICE_TO_HOST, MEM_HOST_TO_DEVICE = 0, 1, 2, 3
 OK, E_ARG, E_NODEVICE, E_CUDA, E_NOMEM, E_FORMAT = 0, -1, -2, -3, -4, -5
 
 # every symbol include/lz4b200.h declares: (name, restype, argtypes)
@@ -28,6 +28,7 @@ SIGNATURES = {
     "lz4b200_encode_batch": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _I, _I, _P]),
     "lz4b200_decode_batch": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _I, _I, _P]),
     "lz4b200_encode_batch_packed": (_I, [_P, _P, _P, _P, _P, _P, _L, _P, _P, C.c_int32, _I]),
+    "lz4b200_encode_batch_packed_from_device": (_I, [_P, _P, _P, _P, _P, _P, _L, _P, _P, C.c_int32, _I, _P]),
     "lz4b200_compact": (_I, [_P, _P, _P, _P, _P, _P, C.c_int32, _P]),
     "lz4b200_measure_batch": (_I, [_P, _P, _P, _P, _P, _P, C.c_int32, _I, _I, _P]),
     "lz4b200_decode_batch_packed": (_I, [_P, _P, _P, _P, _P, _L, _P, _P, C.c_int32, _P]),
