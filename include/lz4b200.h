@@ -163,6 +163,25 @@ int64_t lz4b200_stream_encode(lz4b200_ctx* ctx, const void* src, int64_t n, int3
 int64_t lz4b200_stream_decoded_size(const void* src, int64_t n);     /* sum of rawLen over all chunks, <0 = malformed */
 int64_t lz4b200_stream_decode(lz4b200_ctx* ctx, const void* src, int64_t n, void* dst, int64_t dst_cap);
 
+/* The same stream between device memory and host memory: the stream bytes stay in host memory (a file, a socket), the
+ * raw bytes in HBM, and only the stream bytes cross PCIe, once, overlapped with the kernels.  The host walks the chunk
+ * headers; the device encodes, decodes, writes the frames and copies stored payloads.  Both follow the contract of every
+ * mixed call (LZ4B200_MEM_DEVICE_TO_HOST above): synchronous, ordered behind the work already queued on `stream`, and
+ * LZ4B200_E_ARG when either side is the wrong kind of memory.  n == 0 returns 0.
+ *
+ * stream_encode_from_device: the wire bytes lz4b200_stream_encode writes for a host copy of src.  src: device memory of
+ *   the context's GPU (n bytes); dst: host memory, pageable or page-locked, dst_cap >= lz4b200_stream_bound(n, block_size).
+ *   block_size >= 1 and at most INT32_MAX - 11 (a chunk's frame fits an int32).  Returns bytes written or a negative status. */
+int64_t lz4b200_stream_encode_from_device(lz4b200_ctx* ctx, const void* src, int64_t n, int32_t block_size,
+                                          int high_compression, void* dst, int64_t dst_cap, void* stream);
+/* stream_decode_to_device: the decoded stream, lz4b200_stream_decoded_size bytes, at dst (device memory of the context's
+ *   GPU).  src: host memory.  Returns the decoded size or a negative status: LZ4B200_E_FORMAT / E_ARG exactly where
+ *   lz4b200_stream_decode returns them.  Nothing is written outside [dst, dst + decoded size); a malformed header is found
+ *   before any device work, so nothing is written at all; after a chunk that does not decode (E_FORMAT) the bytes inside
+ *   the range are unspecified. */
+int64_t lz4b200_stream_decode_to_device(lz4b200_ctx* ctx, const void* src, int64_t n, void* dst, int64_t dst_cap,
+                                        void* stream);
+
 /* LZ4Codec.Wrap / Unwrap packet (src/LZ4/LZ4Codec.cs:510-543,574-599): u32le rawLen, u32le storedLen, payload. */
 int lz4b200_wrap(lz4b200_ctx* ctx, const void* src, int32_t n, int high_compression, void* dst, int32_t dst_cap);
 int lz4b200_unwrap_size(const void* src, int32_t n);

@@ -9,7 +9,8 @@ one block at a time, src/LZ4/LZ4Stream.cs:239-269).  Layouts:
 
 The mixed-memory helpers (encode_to_host, encode_to_host_packed, decode_from_host) take the device side as a torch CUDA
 tensor and the host side -- data, offsets, lengths, results -- as numpy arrays.  They are synchronous, ordered behind the
-work already queued on the current torch stream, and move only compressed bytes over PCIe.
+work already queued on the current torch stream, and move only compressed bytes over PCIe.  stream_encode_to_host and
+stream_decode_to_device do the same for the LZ4Stream format: a device tensor's bytes as a stream in host memory, and back.
 """
 from __future__ import annotations
 
@@ -143,6 +144,47 @@ def decode_from_host(ctx: Context, comp: np.ndarray, src_off, src_len, out: torc
     ctx.decode_batch_ptr(_h(comp, np.uint8), _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), _h(dst_off, np.int64, n),
                          _h(dst_cap, np.int32, n), _h(out_len, np.int32, n), n, known=known, stream=_stream(),
                          mem=native.MEM_HOST_TO_DEVICE)
+
+
+def _flat_bytes(t: torch.Tensor) -> torch.Tensor:
+    """The bytes of a contiguous CUDA tensor, in storage order, as a flat uint8 tensor on the same memory."""
+    _d(t)
+    if not t.is_contiguous():
+        raise TypeError("expected a contiguous torch CUDA tensor")
+    return t.reshape(-1).view(torch.uint8)
+
+
+def stream_encode_to_host(ctx: Context, raw: torch.Tensor, block_size: int = 1 << 20, hc: bool = False,
+                          dst: np.ndarray = None) -> np.ndarray:
+    """The LZ4Stream wire bytes of a device tensor's bytes, written to host memory (lz4b200_stream_encode_from_device):
+    the bytes stream_encode writes for a host copy, with only the stream bytes crossing PCIe.  `dst` (uint8, at least
+    lz4b200_stream_bound bytes; pageable or page-locked) receives them, or a new array does.  Returns the view of it that
+    holds the stream.  Synchronous, ordered behind the work already queued on the current torch stream."""
+    r = _flat_bytes(raw)
+    n = r.numel()
+    cap = int(native.lib().lz4b200_stream_bound(n, block_size))
+    if cap < 0:
+        raise native.Lz4B200Error(f"stream_encode_to_host: bad block_size {block_size}")
+    if dst is None:
+        dst = np.empty(max(cap, 1), np.uint8)
+    w = native.lib().lz4b200_stream_encode_from_device(ctx.handle, r.data_ptr(), n, block_size, int(hc), _h(dst, np.uint8),
+                                                       dst.nbytes, _stream())
+    if w < 0:
+        raise native.Lz4B200Error(f"stream_encode_from_device failed with status {w}: {native.last_error()}")
+    return dst[:w]
+
+
+def stream_decode_to_device(ctx: Context, wire: np.ndarray, out: torch.Tensor) -> int:
+    """An LZ4Stream in host memory (a uint8 numpy array) decoded into a device tensor's bytes, from its first byte
+    (lz4b200_stream_decode_to_device).  Returns the decoded size; nothing is written behind it.  Raises Lz4B200Error with
+    the status (E_FORMAT for a malformed stream, E_ARG when `out` is too small).  Synchronous, ordered behind the work
+    already queued on the current torch stream."""
+    o = _flat_bytes(out)
+    r = native.lib().lz4b200_stream_decode_to_device(ctx.handle, _h(wire, np.uint8), wire.nbytes, o.data_ptr(), o.numel(),
+                                                     _stream())
+    if r < 0:
+        raise native.Lz4B200Error(f"stream_decode_to_device failed with status {r}: {native.last_error()}")
+    return int(r)
 
 
 def compact(ctx: Context, slots: torch.Tensor, slot_off, lens, packed, out_off):

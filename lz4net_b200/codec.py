@@ -14,6 +14,7 @@ torch is used only to own device memory / streams; every call goes through ``lib
 from __future__ import annotations
 
 import ctypes as C
+import sys
 from typing import Optional
 
 import numpy as np
@@ -179,6 +180,40 @@ class Context:
         if r < 0:
             raise native.Lz4B200Error(f"stream_decode failed ({r}): {native.last_error()}")
         return dst[:total].tobytes()
+
+    def stream_encode_from_device(self, raw, block_size: int = 1 << 20, high_compression: bool = False) -> bytes:
+        """stream_encode of a contiguous CUDA tensor's bytes, written straight from device memory
+        (lz4b200_stream_encode_from_device)."""
+        from . import batch
+        return batch.stream_encode_to_host(self, raw, block_size, high_compression).tobytes()
+
+    def stream_decode_to_device(self, data: bytes, out) -> int:
+        """stream_decode into the first bytes of a contiguous CUDA tensor (lz4b200_stream_decode_to_device); returns the
+        decoded size.  Raises like stream_decode, and Lz4B200Error when `out` is too small."""
+        from . import batch
+        src = np.frombuffer(bytes(data) + b"\0", np.uint8)
+        if native.lib().lz4b200_stream_decoded_size(src.ctypes.data, len(data)) < 0:
+            raise EOFError("LZ4Stream: unexpected end of stream / corrupt chunk header")     # EndOfStreamException
+        try:
+            return batch.stream_decode_to_device(self, src[:len(data)], out)
+        except native.Lz4B200Error as e:
+            if f"status {native.E_FORMAT}:" in str(e):
+                raise ValueError("LZ4 block has been corrupted") from e
+            raise
+
+
+def _is_tensor(x) -> bool:
+    """A torch tensor (without importing torch when the caller has not)."""
+    torch = sys.modules.get("torch")
+    return torch is not None and isinstance(x, torch.Tensor)
+
+
+def _tensor_bytes(t):
+    """The bytes of a contiguous tensor in storage order, as a flat uint8 tensor on the same memory."""
+    if not t.is_contiguous():
+        raise TypeError("expected a contiguous tensor")
+    import torch
+    return t.reshape(-1).view(torch.uint8)
 
 
 def default_context() -> Context:
@@ -391,7 +426,12 @@ class LZ4Stream:
     ``Flush``/``Close``, FlushCurrentChunk :239-269); the dispatcher differs: up to ``batchBlocks`` buffered blocks (and at
     most ``maxBufferBytes``) are encoded / decoded by ONE batched GPU call instead of one block per call.  With
     ``InteractiveRead`` the reader decodes every chunk as soon as it has been read, like the reference (:376-401): a
-    socket or pipe that has delivered one chunk is never asked for the next one before the caller has seen the first."""
+    socket or pipe that has delivered one chunk is never asked for the next one before the caller has seen the first.
+
+    ``Write`` also takes a contiguous CUDA tensor (its bytes in storage order) and ``ReadInto`` fills one: whole blocks are
+    encoded straight from device memory and whole chunks decoded straight into it (the context's
+    ``stream_encode_from_device`` / ``stream_decode_to_device``), so the raw bytes never cross PCIe.  The wire bytes and
+    chunk boundaries are those of the same bytes written from host memory."""
 
     def __init__(self, innerStream, compressionMode, compressionFlags=LZ4StreamFlags.Default, blockSize=1024 * 1024,
                  batchBlocks=256, context: Optional[Context] = None, maxBufferBytes=64 * 1024 * 1024):
@@ -424,11 +464,36 @@ class LZ4Stream:
     def Write(self, buffer, offset=0, count=None):
         if not self.CanWrite:
             raise NotImplementedError("Operation 'Write' is not supported")
+        if _is_tensor(buffer):
+            self._write_tensor(buffer, offset, count)
+            return
         count = len(buffer) - offset if count is None else count
         self._pending += bytes(buffer[offset:offset + count])
+        self._drain()
+
+    def _drain(self):
         full = min(self._batch, self._max_bytes // self._block) * self._block
         while len(self._pending) > full:          # a full buffer is flushed only when more data arrives (:463-467)
             self._emit(full)
+
+    def _write_tensor(self, tensor, offset, count):
+        """Bytes [offset, offset + count) of a tensor: the head that completes the pending chunk comes to the host (less
+        than one block), the whole blocks after it are encoded from device memory, the tail (less than one block) stays
+        pending.  The chunks are the ones a host write of the same bytes makes."""
+        t = _tensor_bytes(tensor)
+        count = t.numel() - offset if count is None else count
+        if offset < 0 or count < 0 or offset + count > t.numel():
+            raise ValueError("offset and count are invalid for the given buffer")
+        t = t[offset:offset + count]
+        head = min(count, -len(self._pending) % self._block)
+        self._pending += t[:head].cpu().numpy().tobytes()
+        whole = (count - head) // self._block * self._block
+        if whole:
+            if self._pending:                     # whole blocks only: the same chunks as one host write
+                self._emit(len(self._pending))
+            self._inner.write(self._ctx.stream_encode_from_device(t[head:head + whole], self._block, self._hc))
+        self._pending += t[head + whole:].cpu().numpy().tobytes()
+        self._drain()
 
     def WriteByte(self, value):
         self.Write(bytes([value]))
@@ -469,10 +534,15 @@ class LZ4Stream:
             if not (b[0] & 0x80) or count >= 64:
                 return v
 
-    def _acquire(self):
+    def _acquire(self, out=None, room=0):
+        """Reads the next chunks.  With `out` (a flat uint8 tensor), the leading chunks whose decoded bytes fit in `room`
+        are decoded straight into it; the rest are decoded to the host as without it.  Returns None at the end of the
+        stream, else the number of bytes decoded into `out`."""
         raw = bytearray()
+        direct = b""
         decoded = 0
         for _ in range(1 if self._interactive else self._batch):       # interactive: one chunk, then hand it over
+            start = len(raw)
             flags = self._read_varint(raw, True)
             if flags is None:
                 break
@@ -487,14 +557,17 @@ class LZ4Stream:
                     raise EOFError("Unexpected end of stream")
                 payload += more
             raw += payload
+            if out is not None and start == 0 and decoded + raw_len <= room:
+                direct += raw                                           # every chunk so far fits: it goes to the device
+                del raw[:]
             decoded += raw_len
             if decoded >= self._max_bytes:                              # cap the read-ahead by bytes, not only by chunks
                 break
-        if not raw:
-            return False
-        self._ready = self._ctx.stream_decode(bytes(raw))
+        if not raw and not direct:
+            return None
+        self._ready = self._ctx.stream_decode(bytes(raw)) if raw else b""
         self._rpos = 0
-        return True
+        return self._ctx.stream_decode_to_device(bytes(direct), out) if direct else 0
 
     def Read(self, count):
         """Returns up to `count` bytes (b"" at end of stream); with InteractiveRead returns as soon as it has any."""
@@ -509,9 +582,36 @@ class LZ4Stream:
                 if self._interactive:
                     break
                 count -= chunk
-            elif not self._acquire():
+            elif self._acquire() is None:
                 break
         return bytes(out)
+
+    def ReadInto(self, tensor):
+        """Read into a contiguous CUDA tensor's bytes, up to its size: returns the bytes read (0 at end of stream), with
+        Read's semantics (InteractiveRead included).  Bytes already decoded come first; chunks that fit in what is left are
+        decoded straight into the tensor; the chunk that straddles its end is decoded to the host, like Read."""
+        if not self.CanRead:
+            raise NotImplementedError("Operation 'Read' is not supported")
+        out = _tensor_bytes(tensor)
+        import torch
+        count, pos = out.numel(), 0
+        while pos < count:
+            chunk = min(count - pos, len(self._ready) - self._rpos)
+            if chunk > 0:
+                part = np.frombuffer(self._ready, np.uint8, chunk, self._rpos)
+                out[pos:pos + chunk].copy_(torch.from_numpy(part.copy()))
+                self._rpos += chunk
+                pos += chunk
+                if self._interactive:
+                    break
+                continue
+            got = self._acquire(out[pos:], count - pos)
+            if got is None:
+                break
+            pos += got
+            if got and self._interactive:
+                break
+        return pos
 
     def ReadByte(self):
         b = self.Read(1)

@@ -4,11 +4,13 @@
 // framing in framing.cpp) goes through one software pipeline, run_host: the block list is cut into chunks, and for each
 // chunk H2D(inputs) -> kernel -> D2H(outputs) is enqueued on one of NSLOT streams, so that the copy engines (both PCIe
 // directions) and the SMs work on different chunks at the same time.  The mixed-memory batches (MEM_DEVICE_TO_HOST,
-// MEM_HOST_TO_DEVICE and the packed encode from device memory) go through it too, skipping the copy of whichever side is
-// already on the device.  There is no CPU codec in this library: if the
+// MEM_HOST_TO_DEVICE and the packed encode from device memory) and the LZ4Stream calls on device memory go through it
+// too, skipping the copy of whichever side is already on the device.  There is no CPU codec in this library: if the
 // device or the kernel image is unusable every entry point reports an error.
 #include "../../include/lz4b200.h"
+#include "framing.h"
 #include "kernels.h"
+#include "lz4_stream.cuh"
 
 #include <cuda_runtime.h>
 
@@ -105,12 +107,19 @@ struct Slot {
 };
 
 // One chunk's metadata, laid out the same in the slot's hmeta (host) and meta (device, which has no packed_off):
-// int64 src_off[m] | int64 dst_off[m] | int32 src_len[m] | int32 dst_cap[m] | int32 out_len[m] | int64 packed_off[m+1]
+// int64 src_off[m] | int64 dst_off[m] | int32 src_len[m] | int32 dst_cap[m] | int32 aux[m] | int32 out_len[m] |
+// int64 packed_off[m+1].  aux is used by the LZ4Stream calls only: the frame sizes of an encode (written on the device),
+// the stored payload lengths of a decode (copied up with the first four arrays).
 struct Meta {
-    int64_t *so, *dof; int32_t *sl, *dc, *out; int64_t* off;
-    Meta(void* p, int32_t m) : so((int64_t*)p), dof(so + m), sl((int32_t*)(dof + m)), dc(sl + m), out(dc + m),
+    int64_t *so, *dof; int32_t *sl, *dc, *aux, *out; int64_t* off;
+    Meta(void* p, int32_t m) : so((int64_t*)p), dof(so + m), sl((int32_t*)(dof + m)), dc(sl + m), aux(dc + m), out(aux + m),
                                off((int64_t*)(((uintptr_t)(out + m) + 7) & ~(uintptr_t)7)) {}
 };
+
+// The LZ4Stream calls on device memory (lz4_stream.cuh) inside the pipeline.  Encode (APPEND): the frames of the chunks
+// replace the compaction, hc = the flags' HC bit.  Decode (dst on the device): stored[i] != 0 marks a stored chunk, whose
+// payload is copied by the stored-copy step while the decoder gets the neutral entry (src_len 0, dst_cap 0).
+struct StreamFrames { bool hc; const uint8_t* stored; };
 
 }  // namespace
 
@@ -211,9 +220,12 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
 // nothing is compacted or landed, only out_len comes back: NONE).  A chunk is weighed by what it stages, so the slots'
 // device buffers stay within host_chunk_bytes whatever the batch.  The slots start behind everything enqueued on
 // `caller` before the call: a producer of src, or a reader of dst's old contents.
+// frames (the LZ4Stream calls on device memory, see StreamFrames): an APPEND encode lands the chunks' frames instead of
+// the compacted blocks (out_off[i] = where frame i starts); a decode also copies the stored chunks' payloads.
 int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
              const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op,
-             int64_t* out_off, int64_t dst_total_cap, bool src_dev = false, bool dst_dev = false, cudaStream_t caller = nullptr)
+             int64_t* out_off, int64_t dst_total_cap, bool src_dev = false, bool dst_dev = false, cudaStream_t caller = nullptr,
+             const StreamFrames* frames = nullptr)
 {
     const bool measure = op >= 4;
     for (int32_t i = 0; i < n; i++)
@@ -305,7 +317,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         Slot& sl = c->slot[s];
         const int32_t m = b1 - b0;
         const Mode mode = measure || dst_dev ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == 2 ? RUNS : SCATTER;
-        CU(sl.meta.reserve((size_t)m * 28)); CU(sl.hmeta.reserve((size_t)m * 28 + sizeof(int64_t) * (size_t)(m + 2)));
+        CU(sl.meta.reserve((size_t)m * 32)); CU(sl.hmeta.reserve((size_t)m * 32 + sizeof(int64_t) * (size_t)(m + 2)));
         const Meta h(sl.hmeta.p, m), d(sl.meta.p, m);
         int64_t slo = 0, shi = 0, dsum = 0;
         if (!src_dev) {
@@ -317,11 +329,16 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
             if (dst_dev) h.dof[i] = dst_off[b0 + i];
             else { h.dof[i] = dsum; dsum += measure ? 0 : dst_cap[b0 + i]; }
             h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap ? dst_cap[b0 + i] : INT32_MAX;
+            if (frames && frames->stored) {
+                const bool stored = frames->stored[b0 + i] != 0;
+                h.aux[i] = stored ? h.sl[i] : 0;
+                if (stored) h.sl[i] = h.dc[i] = 0;
+            }
         }
         const size_t sbytes = (size_t)(shi - slo);
         if (!src_dev) CU(sl.src.reserve(sbytes + 64));
         if (!dst_dev) CU(sl.dst.reserve((size_t)dsum + 64));
-        CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, (size_t)m * 24, cudaMemcpyHostToDevice, sl.stream));
+        CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, (size_t)m * (frames && frames->stored ? 28 : 24), cudaMemcpyHostToDevice, sl.stream));
         if (sbytes) {
             const uint8_t* from = src + slo;
             if (src_pageable && m > 8) { CU(sl.hsrc.reserve(sbytes)); par_memcpy(sl.hsrc.p, from, sbytes); from = (const uint8_t*)sl.hsrc.p; }
@@ -337,7 +354,20 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         int32_t hc_large = 0;
         if (op == 1) for (int32_t i = b0; i < b1; i++) hc_large += src_len[i] > 65536;
         rc = run_device(c, a, op, sl.stream, lanes, hc_large); if (rc) return rc;
-        if (mode >= SCATTER) {
+        if (frames && frames->stored) {
+            cudaError_t e = launch_stream_stored(a, d.aux, sl.stream, &c->launches);
+            if (e != cudaSuccess) return cuda_fail(e, "stored copy launch");
+        }
+        if (mode >= SCATTER && frames) {
+            // the frames of the chunks, back to back: sizes -> scan -> headers + payloads
+            CU(sl.packed.reserve((size_t)dsum + (size_t)m * STREAM_HEADER_MAX + 64)); CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1)));
+            CU(sl.scan.reserve(compact_tmp_bytes(m)));
+            cudaError_t e = launch_stream_frame_size(a, d.aux, sl.stream, &c->launches);
+            if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, d.aux, nullptr, (int64_t*)sl.offs.p, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
+            if (e == cudaSuccess) e = launch_stream_frame(a, frames->hc, (uint8_t*)sl.packed.p, (const int64_t*)sl.offs.p, sl.stream, &c->launches);
+            if (e != cudaSuccess) return cuda_fail(e, "stream frame launch");
+            CU(cudaMemcpyAsync(h.off, sl.offs.p, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDeviceToHost, sl.stream));
+        } else if (mode >= SCATTER) {
             CU(sl.packed.reserve((size_t)dsum + 64)); CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
             cudaError_t e = launch_compact(a.dst, a.dst_off, a.out_len, (uint8_t*)sl.packed.p, (int64_t*)sl.offs.p, m,
                                            sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
@@ -468,6 +498,10 @@ int frame_scratch(lz4b200_ctx* c, int32_t n, bool packed, cudaStream_t st, WrapS
     DeviceGuard g((c)->device);                                                                       \
     if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
 
+// The LZ4Stream calls on device memory run the pipeline over at most this many chunks at a time: it bounds the host
+// metadata by chunk count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.
+constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
+
 }  // namespace
 
 extern "C" {
@@ -575,6 +609,75 @@ int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* c, const void* src, con
     if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
     return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, mode == LZ4B200_MODE_HC ? 1 : 0,
                  LZ4B200_MEM_DEVICE_TO_HOST, stream, out_off, dst_total_cap);
+}
+
+// ---- LZ4Stream between device and host memory (lz4_stream.cuh): the host pipeline, the frames written on the device ----
+int64_t lz4b200_stream_encode_from_device(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_size, int high_compression,
+                                          void* dst, int64_t dst_cap, void* stream)
+{
+    if (!c || n < 0 || block_size < 1 || (n > 0 && (!src || !dst))) return fail(LZ4B200_E_ARG, "bad argument");
+    if (block_size > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "block_size: a chunk's frame must fit an int32");
+    if (dst_cap < lz4b200_stream_bound(n, block_size)) return fail(LZ4B200_E_ARG, "dst_cap < lz4b200_stream_bound(n, block_size)");
+    if (n == 0) return 0;
+    std::lock_guard<std::mutex> lock(c->mu);
+    DeviceGuard g(c->device);
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    int rc = check_side(c, src, true, "src"); if (rc) return rc;
+    rc = check_side(c, dst, false, "dst"); if (rc) return rc;
+    const int64_t chunks = (n + block_size - 1) / block_size;
+    const StreamFrames f{high_compression != 0, nullptr};
+    std::vector<int64_t> so, at; std::vector<int32_t> len, res;
+    int64_t w = 0;
+    for (int64_t c0 = 0; c0 < chunks; c0 += STREAM_RUN_CHUNKS) {
+        const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, chunks - c0);
+        so.resize(m); len.resize(m); res.assign(m, 0); at.assign((size_t)m + 1, 0);
+        for (int32_t i = 0; i < m; i++) {
+            so[i] = (c0 + i) * block_size;
+            len[i] = (int32_t)std::min<int64_t>(block_size, n - so[i]);      // capacity = the chunk's length (LZ4Stream.cs:243-246)
+        }
+        rc = run_host(c, (const uint8_t*)src, so.data(), len.data(), (uint8_t*)dst + w, nullptr, len.data(), res.data(), m,
+                      high_compression ? 1 : 0, at.data(), dst_cap - w, true, false, (cudaStream_t)stream, &f);
+        if (rc) return rc;
+        w += at[m];
+    }
+    return w;
+}
+
+int64_t lz4b200_stream_decode_to_device(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int64_t dst_cap, void* stream)
+{
+    if (!c || n < 0 || (n > 0 && !src)) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n == 0) return 0;
+    std::lock_guard<std::mutex> lock(c->mu);
+    DeviceGuard g(c->device);
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    int rc = check_side(c, src, false, "src"); if (rc) return rc;
+    // the whole header walk before any device work: a malformed stream writes nothing
+    std::vector<StreamChunk> chunks;
+    const int64_t total = stream_walk((const uint8_t*)src, n, &chunks);
+    if (total < 0) return fail((int)total, "malformed LZ4Stream");
+    if (total > dst_cap || (total > 0 && !dst)) return fail(LZ4B200_E_ARG, "dst_cap < the decoded size");
+    if (total == 0) return 0;
+    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
+    // one entry per non-empty chunk; the flag is the header's (a compressed chunk may have compLen == rawLen, LZ4Stream.cs:288)
+    std::vector<int64_t> so, dof; std::vector<int32_t> len, raw, res; std::vector<uint8_t> stored;
+    int64_t pos = 0;
+    for (const StreamChunk& k : chunks) {
+        if (k.raw > 0) { so.push_back(k.payload); len.push_back(k.stored); dof.push_back(pos); raw.push_back(k.raw); stored.push_back(!k.compressed); }
+        pos += k.raw;
+    }
+    const int64_t entries = (int64_t)so.size();
+    for (int64_t e0 = 0; e0 < entries; e0 += STREAM_RUN_CHUNKS) {
+        const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, entries - e0);
+        res.assign(m, -1);
+        const StreamFrames f{false, stored.data() + e0};
+        rc = run_host(c, (const uint8_t*)src, so.data() + e0, len.data() + e0, (uint8_t*)dst, dof.data() + e0, raw.data() + e0,
+                      res.data(), m, 2, nullptr, 0, false, true, (cudaStream_t)stream, &f);
+        if (rc) return rc;
+        // a compressed chunk decodes from exactly its compLen bytes (framing.cpp, LZ4Codec.Safe.cs:539-542)
+        for (int32_t i = 0; i < m; i++)
+            if (!stored[e0 + i] && res[i] != len[e0 + i]) return fail(LZ4B200_E_FORMAT, "a chunk does not decode to its compressed length");
+    }
+    return total;
 }
 
 int lz4b200_decode_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,

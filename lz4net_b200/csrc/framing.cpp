@@ -6,6 +6,7 @@
 // Here the same byte stream is produced / consumed with ONE batched GPU call for all chunks of a buffer.
 // Pure host code: no kernels, no codec arithmetic -- that all lives behind lz4b200_{encode,decode}_batch.
 #include "../../include/lz4b200.h"
+#include "framing.h"
 
 #include <algorithm>
 #include <cstdint>
@@ -56,10 +57,9 @@ int read_header(const uint8_t* s, int32_t n, int32_t* raw, int32_t* stored)
     return *stored >= *raw ? *stored : *raw;                                             // :587-596
 }
 
-struct Chunk { int64_t payload; int32_t raw; int32_t stored; bool compressed; };
+}  // namespace
 
-// walk the chunk headers of a whole stream; returns total raw size or a negative status
-int64_t walk(const uint8_t* s, int64_t n, std::vector<Chunk>* out)
+int64_t lz4b200::stream_walk(const uint8_t* s, int64_t n, std::vector<StreamChunk>* out)
 {
     int64_t pos = 0, total = 0;
     for (;;) {
@@ -75,12 +75,10 @@ int64_t walk(const uint8_t* s, int64_t n, std::vector<Chunk>* out)
         if (rawi < 0 || cleni < 0 || cleni > rawi) return LZ4B200_E_FORMAT;   // :288 corrupted
         if (pos + cleni > n) return LZ4B200_E_FORMAT;                         // :293 short read
         if (comp && (flags >> 2) != 0) return LZ4B200_E_FORMAT;               // :301-303 multi-pass chunks unsupported
-        if (out) out->push_back(Chunk{pos, rawi, cleni, comp});
+        if (out) out->push_back(StreamChunk{pos, rawi, cleni, comp});
         pos += cleni; total += rawi;
     }
 }
-
-}  // namespace
 
 extern "C" {
 
@@ -132,20 +130,20 @@ int64_t lz4b200_stream_encode(lz4b200_ctx* ctx, const void* src, int64_t n, int3
 int64_t lz4b200_stream_decoded_size(const void* src, int64_t n)
 {
     if (n < 0 || (n > 0 && !src)) return LZ4B200_E_ARG;
-    return walk((const uint8_t*)src, n, nullptr);
+    return lz4b200::stream_walk((const uint8_t*)src, n, nullptr);
 }
 
 int64_t lz4b200_stream_decode(lz4b200_ctx* ctx, const void* src, int64_t n, void* dst, int64_t dst_cap)
 {
     if (!ctx || n < 0 || (n > 0 && !src)) return LZ4B200_E_ARG;
-    std::vector<Chunk> chunks;
-    const int64_t total = walk((const uint8_t*)src, n, &chunks);
+    std::vector<lz4b200::StreamChunk> chunks;
+    const int64_t total = lz4b200::stream_walk((const uint8_t*)src, n, &chunks);
     if (total < 0) return total;
     if (total > dst_cap || (total > 0 && !dst)) return LZ4B200_E_ARG;
     const uint8_t* s = (const uint8_t*)src; uint8_t* d = (uint8_t*)dst;
     std::vector<int64_t> so, dof; std::vector<int32_t> sl, dc, out;
     int64_t pos = 0;
-    for (const Chunk& c : chunks) {
+    for (const lz4b200::StreamChunk& c : chunks) {
         if (!c.compressed) std::memcpy(d + pos, s + c.payload, (size_t)c.raw);           // stored chunk (:295-299)
         else if (c.raw > 0) { so.push_back(c.payload); sl.push_back(c.stored); dof.push_back(pos); dc.push_back(c.raw); }
         pos += c.raw;

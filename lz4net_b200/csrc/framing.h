@@ -1,0 +1,18 @@
+// framing.h -- internal interface of framing.cpp: the LZ4Stream header walk, shared by the host stream decode and the
+// decode into device memory (capi.cu lz4b200_stream_decode_to_device), so that both read a stream by the same rules.
+#pragma once
+#include <stdint.h>
+
+#include <vector>
+
+namespace lz4b200 {
+
+// One chunk of an LZ4Stream: payload at byte `payload` of the stream, `stored` bytes of it (compLen, or rawLen for a
+// stored chunk), `raw` bytes decoded.
+struct StreamChunk { int64_t payload; int32_t raw; int32_t stored; bool compressed; };
+
+// Walks the chunk headers of a whole stream of n bytes (LZ4Stream.cs:274-312); appends every chunk to *out when out is
+// not null.  Returns the total decoded size or LZ4B200_E_FORMAT.
+int64_t stream_walk(const uint8_t* s, int64_t n, std::vector<StreamChunk>* out);
+
+}  // namespace lz4b200

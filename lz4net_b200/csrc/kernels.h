@@ -58,6 +58,15 @@ cudaError_t launch_wrap_finish(const BatchArgs& a, const WrapScratch& w, cudaStr
 cudaError_t launch_unwrap_prep(const BatchArgs& a, const WrapScratch& w, cudaStream_t stream, int64_t* launches);
 // gate (optional): a device int; when it reads 0 the kernel returns at once
 cudaError_t launch_unwrap_finish(const BatchArgs& a, const WrapScratch& w, const int* gate, cudaStream_t stream, int64_t* launches);
+// LZ4Stream frames in device memory (stream.cu, lz4_stream.cuh).  a = the encoded batch: src / src_off / src_len = the
+// chunks' raw bytes, dst / dst_off = the encoder's slots, out_len = its results.  frame_len[i] = the size of chunk i's
+// frame; launch_stream_frame writes frame i at frames + frame_off[i].
+cudaError_t launch_stream_frame_size(const BatchArgs& a, int32_t* frame_len, cudaStream_t stream, int64_t* launches);
+cudaError_t launch_stream_frame(const BatchArgs& a, bool hc, uint8_t* frames, const int64_t* frame_off, cudaStream_t stream,
+                                int64_t* launches);
+// a = the decoded batch (src / src_off = the staged stream and the payload offsets, dst / dst_off = the output): copies
+// stored_len[i] bytes of payload i to its output; entries with stored_len[i] == 0 do nothing
+cudaError_t launch_stream_stored(const BatchArgs& a, const int32_t* stored_len, cudaStream_t stream, int64_t* launches);
 cudaError_t launch_synth(uint8_t* dst, int64_t n_blocks, int32_t block_size, int cls, uint64_t seed, int64_t first_block,
                          const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 
