@@ -222,6 +222,40 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* ctx, const void* src, const int64_t
                                 void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len,
                                 int32_t n, void* stream);
 
+/* The same packets between device memory and host memory: the packets stay in host memory (a socket buffer, an RPC
+ * payload), the raw bytes in HBM, and only the packets cross PCIe, once, overlapped with the kernels.  The host reads the
+ * unwrap headers; the device encodes, decodes, writes the headers and copies stored payloads.  Offsets, lengths, out_off
+ * and out_len are host arrays.  All four follow the contract of every mixed call (LZ4B200_MEM_DEVICE_TO_HOST above):
+ * synchronous, ordered behind the work already queued on `stream`, and LZ4B200_E_ARG when either side is the wrong kind
+ * of memory.  n == 0 is LZ4B200_OK (the packed forms set out_off[0] = 0).
+ *
+ * wrap_batch_from_device: src in device memory of the context's GPU, dst in host memory, pageable or page-locked.  Packet
+ *   i is byte for byte what lz4b200_wrap_batch makes of a host copy of input i; it lands at dst + dst_off[i], and only
+ *   its out_len[i] bytes are written there.  As in lz4b200_wrap_batch, a negative length or dst_cap[i] < src_len[i] + 8
+ *   makes the whole call LZ4B200_E_ARG before any device work. */
+int lz4b200_wrap_batch_from_device(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                   int high_compression, void* dst, const int64_t* dst_off, const int32_t* dst_cap,
+                                   int32_t* out_len, int32_t n, void* stream);
+/* wrap_batch_packed_from_device: the same packets back to back in host memory, in packet order (what a sender writes to
+ *   a socket): packet i at dst + out_off[i], out_off[0..n] (n+1 entries), out_off[n] the total.  sum(src_len[i] + 8) is
+ *   always enough; a smaller dst_total_cap that the packets do not fit is LZ4B200_E_ARG, as in
+ *   lz4b200_encode_batch_packed_from_device.  A packet above INT32_MAX bytes (src_len[i] > INT32_MAX - 8) is E_ARG. */
+int lz4b200_wrap_batch_packed_from_device(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                          int high_compression, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                          int32_t* out_len, int32_t n, void* stream);
+/* unwrap_batch_to_device: packets in host memory, outputs in device memory of the context's GPU.  out_len[i] is what
+ *   lz4b200_unwrap_batch returns for the same packet and capacity: bytes restored, LZ4B200_E_FORMAT or E_ARG (a bad packet
+ *   is that packet's status, never the call's).  Nothing is written outside [dst_off[i], dst_off[i] + dst_cap[i]). */
+int lz4b200_unwrap_batch_to_device(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                   void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len,
+                                   int32_t n, void* stream);
+/* unwrap_batch_packed_to_device: the contract of lz4b200_unwrap_batch_packed with out_off and out_len on the host.  The
+ *   sizes come from the headers before any device work; if out_off[n] > dst_total_cap, dst is untouched and out_len holds
+ *   the sizes, otherwise it is unwrap_batch_to_device with dst_off = out_off and dst_cap = the sizes. */
+int lz4b200_unwrap_batch_packed_to_device(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                          void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len,
+                                          int32_t n, void* stream);
+
 /* ---- host buffers the caller keeps for a while (a pinned byte[] behind a GCHandle, a native arena) --------------------
  * Host-memory batches copy straight from / to the caller's buffers.  From pageable memory the driver stages every copy
  * through its own pinned bounce buffers, synchronously; page-locking a long-lived buffer once (cudaHostRegister) lets the

@@ -11,6 +11,8 @@ The mixed-memory helpers (encode_to_host, encode_to_host_packed, decode_from_hos
 tensor and the host side -- data, offsets, lengths, results -- as numpy arrays.  They are synchronous, ordered behind the
 work already queued on the current torch stream, and move only compressed bytes over PCIe.  stream_encode_to_host and
 stream_decode_to_device do the same for the LZ4Stream format: a device tensor's bytes as a stream in host memory, and back.
+wrap_to_host, wrap_to_host_packed, unwrap_to_device and unwrap_to_device_packed do it for Wrap packets: inputs in a device
+tensor, packets in a host array, and back.
 """
 from __future__ import annotations
 
@@ -144,6 +146,49 @@ def decode_from_host(ctx: Context, comp: np.ndarray, src_off, src_len, out: torc
     ctx.decode_batch_ptr(_h(comp, np.uint8), _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), _h(dst_off, np.int64, n),
                          _h(dst_cap, np.int32, n), _h(out_len, np.int32, n), n, known=known, stream=_stream(),
                          mem=native.MEM_HOST_TO_DEVICE)
+
+
+def wrap_to_host(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, out_len, hc: bool = False):
+    """Wrap / WrapHC packets of a device tensor's inputs written into slots of a host array (lz4b200_wrap_batch_from_device):
+    packet i of raw + src_off[i] lands at dst + dst_off[i] (dst_cap[i] >= src_len[i] + 8), only its out_len[i] bytes.
+    src_off / dst_off int64, src_len / dst_cap / out_len int32 numpy arrays."""
+    n = len(src_off)
+    native.check(native.lib().lz4b200_wrap_batch_from_device(
+        ctx.handle, _d(raw), _h(src_off, np.int64), _h(src_len, np.int32, n), int(hc), _h(dst, np.uint8), _h(dst_off, np.int64, n),
+        _h(dst_cap, np.int32, n), _h(out_len, np.int32, n), n, _stream()), "wrap_batch_from_device")
+
+
+def wrap_to_host_packed(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: np.ndarray, out_off, out_len,
+                        hc: bool = False) -> int:
+    """The same packets back to back in a host array (lz4b200_wrap_batch_packed_from_device): packet i at dst + out_off[i],
+    out_off (int64[n+1]) [n] = the total, which is returned.  sum(src_len + 8) bytes of dst are always enough; raises when
+    the packets do not fit dst.nbytes."""
+    n = len(src_off)
+    native.check(native.lib().lz4b200_wrap_batch_packed_from_device(
+        ctx.handle, _d(raw), _h(src_off, np.int64), _h(src_len, np.int32, n), int(hc), _h(dst, np.uint8), dst.nbytes,
+        _h(out_off, np.int64, n + 1), _h(out_len, np.int32, n), n, _stream()), "wrap_batch_packed_from_device")
+    return int(out_off[n])
+
+
+def unwrap_to_device(ctx: Context, packets: np.ndarray, src_off, src_len, out: torch.Tensor, dst_off, dst_cap, out_len):
+    """Packets in a host array unwrapped into a device tensor (lz4b200_unwrap_batch_to_device): packet i of
+    packets + src_off[i] is restored at out + dst_off[i], nothing written outside its dst_cap[i] bytes; out_len[i] = bytes
+    restored, LZ4B200_E_FORMAT or E_ARG, as lz4b200_unwrap_batch returns."""
+    n = len(src_off)
+    native.check(native.lib().lz4b200_unwrap_batch_to_device(
+        ctx.handle, _h(packets, np.uint8), _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), _h(dst_off, np.int64, n),
+        _h(dst_cap, np.int32, n), _h(out_len, np.int32, n), n, _stream()), "unwrap_batch_to_device")
+
+
+def unwrap_to_device_packed(ctx: Context, packets: np.ndarray, src_off, src_len, out: torch.Tensor, out_off, out_len) -> int:
+    """Unwrap into packed output sized from the headers (lz4b200_unwrap_batch_packed_to_device): packet i lands at
+    out + out_off[i] (int64[n+1]) when out_off[n] fits out.nbytes; otherwise out is untouched and out_len holds the sizes.
+    Returns out_off[n]."""
+    n = len(src_off)
+    native.check(native.lib().lz4b200_unwrap_batch_packed_to_device(
+        ctx.handle, _h(packets, np.uint8), _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), out.nbytes,
+        _h(out_off, np.int64, n + 1), _h(out_len, np.int32, n), n, _stream()), "unwrap_batch_packed_to_device")
+    return int(out_off[n])
 
 
 def _flat_bytes(t: torch.Tensor) -> torch.Tensor:

@@ -338,8 +338,19 @@ class LZ4Codec:
         return cls._service.Decode(input, inputOffset, inputLength, output, outputOffset, outputLength, knownOutputLength)
 
     # ---- Wrap / Unwrap (:510-599) ------------------------------------------------------------------------------
+    # Wrap / WrapHC also take a contiguous CUDA tensor (its bytes in storage order; offset and length count bytes): the
+    # packet is written straight from device memory (lz4b200_wrap_batch_packed_from_device), the same bytes as for the
+    # tensor's host copy.
     @staticmethod
     def _wrap(data, hc):
+        if _is_tensor(data) and data.numel():                        # (an empty input has no device address to read)
+            from . import batch
+            n = data.numel()
+            dst = np.empty(n + 8, np.uint8)
+            off, out = np.zeros(2, np.int64), np.zeros(1, np.int32)
+            w = batch.wrap_to_host_packed(default_context(), data, np.zeros(1, np.int64), np.array([n], np.int32), dst, off, out,
+                                          hc=hc)
+            return dst[:w].tobytes()
         l = native.lib()
         src = np.frombuffer(bytes(data) + b"\0", np.uint8)
         dst = np.zeros(len(data) + 8 + 16, np.uint8)
@@ -348,19 +359,25 @@ class LZ4Codec:
             raise native.Lz4B200Error(f"wrap failed ({r}): {native.last_error()}")
         return dst[:r].tobytes()
 
-    @classmethod
-    def Wrap(cls, inputBuffer, inputOffset=0, inputLength=2 ** 31 - 1):
+    @staticmethod
+    def _wrap_input(inputBuffer, inputOffset, inputLength):
+        """The input of Wrap / WrapHC: bytes, or the flat uint8 view of a CUDA tensor's bytes."""
+        cuda = _is_tensor(inputBuffer) and inputBuffer.is_cuda
+        if cuda:
+            inputBuffer = _tensor_bytes(inputBuffer)
         inputLength = min(len(inputBuffer) - inputOffset, inputLength)
         if inputLength < 0:
             raise ValueError("inputBuffer size of inputLength is invalid")
-        return cls._wrap(bytes(inputBuffer[inputOffset:inputOffset + inputLength]), False)
+        part = inputBuffer[inputOffset:inputOffset + inputLength]
+        return part if cuda else bytes(part)
+
+    @classmethod
+    def Wrap(cls, inputBuffer, inputOffset=0, inputLength=2 ** 31 - 1):
+        return cls._wrap(cls._wrap_input(inputBuffer, inputOffset, inputLength), False)
 
     @classmethod
     def WrapHC(cls, inputBuffer, inputOffset=0, inputLength=2 ** 31 - 1):
-        inputLength = min(len(inputBuffer) - inputOffset, inputLength)
-        if inputLength < 0:
-            raise ValueError("inputBuffer size of inputLength is invalid")
-        return cls._wrap(bytes(inputBuffer[inputOffset:inputOffset + inputLength]), True)
+        return cls._wrap(cls._wrap_input(inputBuffer, inputOffset, inputLength), True)
 
     @staticmethod
     def Unwrap(inputBuffer, inputOffset=0):

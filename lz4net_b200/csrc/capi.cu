@@ -4,13 +4,14 @@
 // framing in framing.cpp) goes through one software pipeline, run_host: the block list is cut into chunks, and for each
 // chunk H2D(inputs) -> kernel -> D2H(outputs) is enqueued on one of NSLOT streams, so that the copy engines (both PCIe
 // directions) and the SMs work on different chunks at the same time.  The mixed-memory batches (MEM_DEVICE_TO_HOST,
-// MEM_HOST_TO_DEVICE and the packed encode from device memory) and the LZ4Stream calls on device memory go through it
-// too, skipping the copy of whichever side is already on the device.  There is no CPU codec in this library: if the
-// device or the kernel image is unusable every entry point reports an error.
+// MEM_HOST_TO_DEVICE and the packed encode from device memory) and the LZ4Stream and Wrap / Unwrap calls between device
+// and host memory go through it too, skipping the copy of whichever side is already on the device.  There is no CPU codec
+// in this library: if the device or the kernel image is unusable every entry point reports an error.
 #include "../../include/lz4b200.h"
 #include "framing.h"
 #include "kernels.h"
 #include "lz4_stream.cuh"
+#include "lz4_wrap.cuh"
 
 #include <cuda_runtime.h>
 
@@ -108,18 +109,25 @@ struct Slot {
 
 // One chunk's metadata, laid out the same in the slot's hmeta (host) and meta (device, which has no packed_off):
 // int64 src_off[m] | int64 dst_off[m] | int32 src_len[m] | int32 dst_cap[m] | int32 aux[m] | int32 out_len[m] |
-// int64 packed_off[m+1].  aux is used by the LZ4Stream calls only: the frame sizes of an encode (written on the device),
-// the stored payload lengths of a decode (copied up with the first four arrays).
+// int64 packed_off[m+1].  aux is used by the LZ4Stream and Unwrap calls only: the frame sizes of an encode (written on the
+// device), the stored payload lengths of a decode (copied up with the first four arrays).  A Wrap encode from device
+// memory keeps the codec's view of its packets (WrapScratch: int64 off[m] | int32 len[m] | int32 cap[m] | int32 res[m])
+// in the device block behind out, at WRAP_META_OFFSET * m bytes: the slots are in flight at once, so it is theirs.
 struct Meta {
     int64_t *so, *dof; int32_t *sl, *dc, *aux, *out; int64_t* off;
     Meta(void* p, int32_t m) : so((int64_t*)p), dof(so + m), sl((int32_t*)(dof + m)), dc(sl + m), aux(dc + m), out(aux + m),
                                off((int64_t*)(((uintptr_t)(out + m) + 7) & ~(uintptr_t)7)) {}
 };
+constexpr size_t META_BYTES = 32, WRAP_META_OFFSET = 32, WRAP_META_BYTES = WRAP_META_OFFSET + 20;
 
-// The LZ4Stream calls on device memory (lz4_stream.cuh) inside the pipeline.  Encode (APPEND): the frames of the chunks
-// replace the compaction, hc = the flags' HC bit.  Decode (dst on the device): stored[i] != 0 marks a stored chunk, whose
-// payload is copied by the stored-copy step while the decoder gets the neutral entry (src_len 0, dst_cap 0).
-struct StreamFrames { bool hc; const uint8_t* stored; };
+// The framing calls between device and host memory inside the pipeline.
+//  LZ4Stream encode (APPEND, lz4_stream.cuh): the frames of the chunks replace the compaction, hc = the flags' HC bit.
+//  Wrap encode (wrap, lz4_wrap.cuh): dst_cap[i] = the packet's capacity, src_len[i] + 8.  The encoder writes each payload
+//    behind its header's place in the slot; the finish step writes the headers and the stored inputs and sets out_len to
+//    the packet sizes.  The slot then holds whole packets, which land like the blocks of an encode.
+//  Decode (dst on the device; LZ4Stream chunks, Unwrap packets): stored[i] != 0 marks a stored chunk or packet, whose
+//    payload is copied by the stored-copy step while the decoder gets the neutral entry (src_len 0, dst_cap 0).
+struct Framing { bool hc; const uint8_t* stored; bool wrap; };
 
 }  // namespace
 
@@ -220,14 +228,15 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
 // nothing is compacted or landed, only out_len comes back: NONE).  A chunk is weighed by what it stages, so the slots'
 // device buffers stay within host_chunk_bytes whatever the batch.  The slots start behind everything enqueued on
 // `caller` before the call: a producer of src, or a reader of dst's old contents.
-// frames (the LZ4Stream calls on device memory, see StreamFrames): an APPEND encode lands the chunks' frames instead of
-// the compacted blocks (out_off[i] = where frame i starts); a decode also copies the stored chunks' payloads.
+// frames (the framing calls between device and host memory, see Framing): an APPEND LZ4Stream encode lands the chunks'
+// frames instead of the compacted blocks (out_off[i] = where frame i starts); a Wrap encode lands whole packets in any
+// mode; a decode also copies the stored chunks' or packets' payloads.
 int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
              const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op,
              int64_t* out_off, int64_t dst_total_cap, bool src_dev = false, bool dst_dev = false, cudaStream_t caller = nullptr,
-             const StreamFrames* frames = nullptr)
+             const Framing* frames = nullptr)
 {
-    const bool measure = op >= 4;
+    const bool measure = op >= 4, wrap = frames && frames->wrap;
     for (int32_t i = 0; i < n; i++)
         if (src_len[i] < 0 || (dst_cap && dst_cap[i] < 0)) return fail(LZ4B200_E_ARG, "negative block length");
     const bool src_pageable = !src_dev && is_pageable(src), dst_pageable = !measure && !dst_dev && is_pageable(dst);
@@ -317,7 +326,8 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         Slot& sl = c->slot[s];
         const int32_t m = b1 - b0;
         const Mode mode = measure || dst_dev ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == 2 ? RUNS : SCATTER;
-        CU(sl.meta.reserve((size_t)m * 32)); CU(sl.hmeta.reserve((size_t)m * 32 + sizeof(int64_t) * (size_t)(m + 2)));
+        CU(sl.meta.reserve((size_t)m * (wrap ? WRAP_META_BYTES : META_BYTES)));
+        CU(sl.hmeta.reserve((size_t)m * META_BYTES + sizeof(int64_t) * (size_t)(m + 2)));
         const Meta h(sl.hmeta.p, m), d(sl.meta.p, m);
         int64_t slo = 0, shi = 0, dsum = 0;
         if (!src_dev) {
@@ -353,12 +363,25 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         }
         int32_t hc_large = 0;
         if (op == 1) for (int32_t i = b0; i < b1; i++) hc_large += src_len[i] > 65536;
-        rc = run_device(c, a, op, sl.stream, lanes, hc_large); if (rc) return rc;
+        if (wrap) {
+            // prep (payload at dof + 8, capacity = the input length) -> encode -> finish: whole packets in the slot
+            WrapScratch w;
+            w.off = (int64_t*)((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m);
+            w.len = (int32_t*)(w.off + m); w.cap = w.len + m; w.res = w.cap + m;
+            cudaError_t e = launch_wrap_prep(a, w, sl.stream, &c->launches);
+            if (e != cudaSuccess) return cuda_fail(e, "wrap prep launch");
+            const BatchArgs enc{a.src, a.src_off, w.len, a.dst, w.off, w.cap, w.res, m};
+            rc = run_device(c, enc, op, sl.stream, lanes, hc_large); if (rc) return rc;
+            e = launch_wrap_finish(a, w, sl.stream, &c->launches);
+            if (e != cudaSuccess) return cuda_fail(e, "wrap finish launch");
+        } else {
+            rc = run_device(c, a, op, sl.stream, lanes, hc_large); if (rc) return rc;
+        }
         if (frames && frames->stored) {
             cudaError_t e = launch_stream_stored(a, d.aux, sl.stream, &c->launches);
             if (e != cudaSuccess) return cuda_fail(e, "stored copy launch");
         }
-        if (mode >= SCATTER && frames) {
+        if (mode >= SCATTER && frames && !wrap) {
             // the frames of the chunks, back to back: sizes -> scan -> headers + payloads
             CU(sl.packed.reserve((size_t)dsum + (size_t)m * STREAM_HEADER_MAX + 64)); CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1)));
             CU(sl.scan.reserve(compact_tmp_bytes(m)));
@@ -502,6 +525,73 @@ int frame_scratch(lz4b200_ctx* c, int32_t n, bool packed, cudaStream_t st, WrapS
 // metadata by chunk count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.
 constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
 
+// The Wrap packets of device inputs, landed in host memory: in the caller's slots, or packed (dst_off == nullptr, out_off
+// as in the packed encode).  Every argument is checked before any device work, as lz4b200_wrap_batch does.
+int wrap_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, int high_compression,
+                     void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n,
+                     int64_t* out_off, int64_t dst_total_cap, void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
+    if (n == 0) { if (out_off) out_off[0] = 0; return LZ4B200_OK; }
+    if (!src || !src_off || !src_len || !dst || !out_len || (dst_off ? !dst_cap : !out_off)) return fail(LZ4B200_E_ARG, "null argument");
+    // the slots' dense layout holds packets, whatever room the caller's slots have
+    std::vector<int32_t> pcap((size_t)n);
+    for (int32_t i = 0; i < n; i++) {
+        if (src_len[i] < 0 || src_len[i] > INT32_MAX - WRAP_HEADER) return fail(LZ4B200_E_ARG, "input length: negative, or a packet above INT32_MAX bytes");
+        if (dst_off && (int64_t)dst_cap[i] < (int64_t)src_len[i] + WRAP_HEADER) return fail(LZ4B200_E_ARG, "dst_cap[i] < src_len[i] + 8");
+        pcap[i] = src_len[i] + WRAP_HEADER;
+    }
+    std::lock_guard<std::mutex> lock(c->mu);
+    DeviceGuard g(c->device);
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    int rc = check_side(c, src, true, "src"); if (rc) return rc;
+    rc = check_side(c, dst, false, "dst"); if (rc) return rc;
+    const Framing f{false, nullptr, true};
+    return run_host(c, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, pcap.data(), out_len, n,
+                    high_compression ? 1 : 0, out_off, dst_total_cap, true, false, (cudaStream_t)stream, &f);
+}
+
+// The headers of n packets in host memory (framing.h read_header), read by several threads: small packets far apart in a
+// large batch cost a cache and TLB miss each, and one thread would then take longer than the link.
+struct WrapHeader { int32_t raw, stored, size; };
+std::vector<WrapHeader> read_headers(const uint8_t* src, const int64_t* src_off, const int32_t* src_len, int32_t n)
+{
+    std::vector<WrapHeader> h((size_t)n);
+    par_ranges((size_t)n, 4096, [&](size_t lo, size_t hi) {
+        for (size_t i = lo; i < hi; i++) h[i].size = read_header(src + src_off[i], src_len[i], &h[i].raw, &h[i].stored);
+    });
+    return h;
+}
+
+// Unwrap from host memory into device memory, the caller holding the lock with both sides checked and the headers read.
+// A rejected packet gets its status before any device work (E_FORMAT, or E_ARG above its capacity), an empty one 0.
+// Every other packet is one entry of a known-size decode: a compressed one decodes its stored bytes into raw bytes, a
+// stored one is copied (Framing::stored).
+int unwrap_to_device(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const WrapHeader* hdr, uint8_t* dst,
+                     const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, cudaStream_t stream)
+{
+    std::vector<int64_t> so, dof; std::vector<int32_t> len, cap, res, idx; std::vector<uint8_t> stored;
+    for (int32_t i = 0; i < n; i++) {
+        const WrapHeader& h = hdr[i];
+        out_len[i] = h.size >= 0 && h.size > dst_cap[i] ? LZ4B200_E_ARG : h.size;
+        if (out_len[i] <= 0) continue;
+        so.push_back(src_off[i] + WRAP_HEADER); len.push_back(h.stored); dof.push_back(dst_off[i]); cap.push_back(h.size);
+        stored.push_back(h.stored >= h.raw); idx.push_back(i);
+    }
+    if (so.empty()) return LZ4B200_OK;
+    const int32_t m = (int32_t)so.size();
+    res.assign((size_t)m, -1);
+    const Framing f{false, stored.data(), false};
+    int rc = run_host(c, src, so.data(), len.data(), dst, dof.data(), cap.data(), res.data(), m, 2, nullptr, 0, false, true, stream, &f);
+    if (rc) return rc;
+    // a compressed packet decodes from exactly its stored bytes (framing.cpp lz4b200_unwrap_batch); one that does not is
+    // that packet's E_FORMAT, not the call's
+    for (int32_t j = 0; j < m; j++)
+        if (!stored[j]) out_len[idx[j]] = res[j] == len[j] ? cap[j] : LZ4B200_E_FORMAT;
+    return LZ4B200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -625,7 +715,7 @@ int64_t lz4b200_stream_encode_from_device(lz4b200_ctx* c, const void* src, int64
     int rc = check_side(c, src, true, "src"); if (rc) return rc;
     rc = check_side(c, dst, false, "dst"); if (rc) return rc;
     const int64_t chunks = (n + block_size - 1) / block_size;
-    const StreamFrames f{high_compression != 0, nullptr};
+    const Framing f{high_compression != 0, nullptr, false};
     std::vector<int64_t> so, at; std::vector<int32_t> len, res;
     int64_t w = 0;
     for (int64_t c0 = 0; c0 < chunks; c0 += STREAM_RUN_CHUNKS) {
@@ -669,7 +759,7 @@ int64_t lz4b200_stream_decode_to_device(lz4b200_ctx* c, const void* src, int64_t
     for (int64_t e0 = 0; e0 < entries; e0 += STREAM_RUN_CHUNKS) {
         const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, entries - e0);
         res.assign(m, -1);
-        const StreamFrames f{false, stored.data() + e0};
+        const Framing f{false, stored.data() + e0, false};
         rc = run_host(c, (const uint8_t*)src, so.data() + e0, len.data() + e0, (uint8_t*)dst, dof.data() + e0, raw.data() + e0,
                       res.data(), m, 2, nullptr, 0, false, true, (cudaStream_t)stream, &f);
         if (rc) return rc;
@@ -814,6 +904,63 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (e != cudaSuccess) return cuda_fail(e, "packed unwrap launch");
     CU(cudaEventRecord(c->compact_done, st));
     return LZ4B200_OK;
+}
+
+// ---- Wrap / Unwrap packets between device and host memory: the host pipeline (run_host, Framing) ----
+int lz4b200_wrap_batch_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                   int high_compression, void* dst, const int64_t* dst_off, const int32_t* dst_cap,
+                                   int32_t* out_len, int32_t n, void* stream)
+{
+    if (!dst_off && n > 0) return fail(LZ4B200_E_ARG, "null argument");        // (a null dst_off means packed inside)
+    return wrap_from_device(c, src, src_off, src_len, high_compression, dst, dst_off, dst_cap, out_len, n, nullptr, 0, stream);
+}
+
+int lz4b200_wrap_batch_packed_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                          int high_compression, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                          int32_t* out_len, int32_t n, void* stream)
+{
+    if (!out_off) return fail(LZ4B200_E_ARG, "bad argument");
+    return wrap_from_device(c, src, src_off, src_len, high_compression, dst, nullptr, nullptr, out_len, n, out_off,
+                            dst_total_cap, stream);
+}
+
+int lz4b200_unwrap_batch_to_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                                   const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
+{
+    FRAME_CALL_PROLOGUE(c, n)
+    if (n == 0) return LZ4B200_OK;
+    if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
+    int rc = check_side(c, src, false, "src"); if (rc) return rc;
+    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
+    const std::vector<WrapHeader> hdr = read_headers((const uint8_t*)src, src_off, src_len, n);
+    return unwrap_to_device(c, (const uint8_t*)src, src_off, hdr.data(), (uint8_t*)dst, dst_off, dst_cap, out_len, n,
+                            (cudaStream_t)stream);
+}
+
+// the sizes from the headers, on the host, then the unwrap into slots at their prefix sums
+int lz4b200_unwrap_batch_packed_to_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                          void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
+                                          void* stream)
+{
+    FRAME_CALL_PROLOGUE(c, n)
+    if (!out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
+    if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
+    int rc = check_side(c, src, false, "src"); if (rc) return rc;
+    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
+    const std::vector<WrapHeader> hdr = read_headers((const uint8_t*)src, src_off, src_len, n);
+    std::vector<int32_t> cap((size_t)n);
+    int64_t total = 0;
+    for (int32_t i = 0; i < n; i++) {
+        out_len[i] = hdr[i].size;
+        cap[i] = std::max(hdr[i].size, 0);
+        out_off[i] = total;
+        total += cap[i];
+    }
+    out_off[n] = total;
+    if (total > dst_total_cap) return LZ4B200_OK;
+    return unwrap_to_device(c, (const uint8_t*)src, src_off, hdr.data(), (uint8_t*)dst, out_off, cap.data(), out_len, n,
+                            (cudaStream_t)stream);
 }
 
 int lz4b200_synth_fill(lz4b200_ctx* c, void* dst, int64_t n_blocks, int32_t block_size, int cls, uint64_t seed,

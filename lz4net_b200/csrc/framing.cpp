@@ -47,17 +47,15 @@ inline int get_varint(const uint8_t* s, int64_t n, int64_t* pos, uint64_t* out)
 inline uint32_t get_u32le(const uint8_t* p) { return p[0] | p[1] << 8 | p[2] << 16 | (uint32_t)p[3] << 24; }
 inline void put_u32le(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
 
-// The Wrap packet header (src/LZ4/LZ4Codec.cs:574-599): u32le raw length, u32le stored length.  Returns the unwrapped
-// size, or LZ4B200_E_FORMAT for a malformed packet.
-int read_header(const uint8_t* s, int32_t n, int32_t* raw, int32_t* stored)
+}  // namespace
+
+int lz4b200::read_header(const uint8_t* s, int32_t n, int32_t* raw, int32_t* stored)
 {
     if (!s || n < 8) return LZ4B200_E_FORMAT;                                            // :577-578
     *raw = (int32_t)get_u32le(s); *stored = (int32_t)get_u32le(s + 4);
     if (*stored > n - 8 || *stored < 0 || *raw < 0) return LZ4B200_E_FORMAT;             // :582-583
     return *stored >= *raw ? *stored : *raw;                                             // :587-596
 }
-
-}  // namespace
 
 int64_t lz4b200::stream_walk(const uint8_t* s, int64_t n, std::vector<StreamChunk>* out)
 {
@@ -174,7 +172,7 @@ int lz4b200_wrap(lz4b200_ctx* ctx, const void* src, int32_t n, int hc, void* dst
 int lz4b200_unwrap_size(const void* src, int32_t n)
 {
     int32_t raw, stored;
-    return read_header((const uint8_t*)src, n, &raw, &stored);
+    return lz4b200::read_header((const uint8_t*)src, n, &raw, &stored);
 }
 
 int lz4b200_unwrap(lz4b200_ctx* ctx, const void* src, int32_t n, void* dst, int32_t dst_cap)
@@ -236,7 +234,7 @@ int lz4b200_unwrap_batch(lz4b200_ctx* ctx, const void* src, const int64_t* src_o
     for (int32_t i = 0; i < n; i++) {
         const uint8_t* p = s + src_off[i];
         int32_t raw, stored;
-        const int size = read_header(p, src_len[i], &raw, &stored);
+        const int size = lz4b200::read_header(p, src_len[i], &raw, &stored);
         if (size < 0) { out_len[i] = size; continue; }
         if (size > dst_cap[i]) { out_len[i] = LZ4B200_E_ARG; continue; }
         if (stored >= raw) { std::memcpy(d + dst_off[i], p + 8, (size_t)stored); out_len[i] = stored; continue; }

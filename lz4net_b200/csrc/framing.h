@@ -1,5 +1,6 @@
-// framing.h -- internal interface of framing.cpp: the LZ4Stream header walk, shared by the host stream decode and the
-// decode into device memory (capi.cu lz4b200_stream_decode_to_device), so that both read a stream by the same rules.
+// framing.h -- internal interface of framing.cpp: the LZ4Stream header walk and the Wrap packet header, shared by the host
+// calls and the decodes into device memory (capi.cu lz4b200_stream_decode_to_device, lz4b200_unwrap_batch_to_device), so
+// that both read a stream or a packet by the same rules.
 #pragma once
 #include <stdint.h>
 
@@ -14,5 +15,9 @@ struct StreamChunk { int64_t payload; int32_t raw; int32_t stored; bool compress
 // Walks the chunk headers of a whole stream of n bytes (LZ4Stream.cs:274-312); appends every chunk to *out when out is
 // not null.  Returns the total decoded size or LZ4B200_E_FORMAT.
 int64_t stream_walk(const uint8_t* s, int64_t n, std::vector<StreamChunk>* out);
+
+// The Wrap packet header (src/LZ4/LZ4Codec.cs:574-599) of a packet of n bytes at s: u32le raw length, u32le stored
+// length.  Returns the unwrapped size, or LZ4B200_E_FORMAT for a malformed packet.
+int read_header(const uint8_t* s, int32_t n, int32_t* raw, int32_t* stored);
 
 }  // namespace lz4b200

@@ -50,6 +50,10 @@ SIGNATURES = {
     "lz4b200_wrap_batch_device": (_I, [_P, _P, _P, _P, _I, _P, _P, _P, _P, C.c_int32, _P]),
     "lz4b200_unwrap_batch_device": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P]),
     "lz4b200_unwrap_batch_packed": (_I, [_P, _P, _P, _P, _P, _L, _P, _P, C.c_int32, _P]),
+    "lz4b200_wrap_batch_from_device": (_I, [_P, _P, _P, _P, _I, _P, _P, _P, _P, C.c_int32, _P]),
+    "lz4b200_wrap_batch_packed_from_device": (_I, [_P, _P, _P, _P, _I, _P, _L, _P, _P, C.c_int32, _P]),
+    "lz4b200_unwrap_batch_to_device": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, _P]),
+    "lz4b200_unwrap_batch_packed_to_device": (_I, [_P, _P, _P, _P, _P, _L, _P, _P, C.c_int32, _P]),
     "lz4b200_host_register": (_I, [_P, _L]),
     "lz4b200_peer_copy": (_I, [_P, _P, _L, _P]),
     "lz4b200_host_unregister": (_I, [_P]),
