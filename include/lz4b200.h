@@ -156,7 +156,9 @@ int lz4b200_uncompress_unknownOutputSize(const char* source, char* dest, int isi
  * LZ4Stream chunk format (src/LZ4/LZ4Stream.cs:239-312): varint(flags) varint(rawLen) [varint(compLen)] payload.
  * stream_encode cuts `src` into block_size chunks, encodes all of them in one batch and writes the exact byte
  * stream an LZ4Stream(..., Compress, highCompression, block_size) would have produced for one Write + Close.
- * Returns bytes written, or a negative status (LZ4B200_E_ARG if dst_cap is too small / the stream is malformed). */
+ * Returns bytes written, or a negative status (LZ4B200_E_ARG if dst_cap is too small / the stream is malformed).
+ * The frames are written on the device, where a chunk's frame must fit an int32: a stream that holds a chunk above
+ * INT32_MAX - 11 bytes (min(block_size, n) > INT32_MAX - 11) is LZ4B200_E_ARG.  Any block_size works below that. */
 int64_t lz4b200_stream_bound(int64_t n, int32_t block_size);
 int64_t lz4b200_stream_encode(lz4b200_ctx* ctx, const void* src, int64_t n, int32_t block_size, int high_compression,
                               void* dst, int64_t dst_cap);

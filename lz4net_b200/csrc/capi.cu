@@ -1,12 +1,14 @@
 // capi.cu -- the C ABI of liblz4b200.so (include/lz4b200.h): context, batched entry points, single-block entry points.
 //
-// Every call on host memory (the batches with LZ4B200_MEM_HOST, the packed encode, the measure pass, the single-block entry points and the
-// framing in framing.cpp) goes through one software pipeline, run_host: the block list is cut into chunks, and for each
-// chunk H2D(inputs) -> kernel -> D2H(outputs) is enqueued on one of NSLOT streams, so that the copy engines (both PCIe
-// directions) and the SMs work on different chunks at the same time.  The mixed-memory batches (MEM_DEVICE_TO_HOST,
-// MEM_HOST_TO_DEVICE and the packed encode from device memory) and the LZ4Stream and Wrap / Unwrap calls between device
-// and host memory go through it too, skipping the copy of whichever side is already on the device.  There is no CPU codec
-// in this library: if the device or the kernel image is unusable every entry point reports an error.
+// Every call on host memory (the batches with LZ4B200_MEM_HOST, the packed encode, the measure pass, the single-block entry
+// points, and the LZ4Stream and Wrap / Unwrap calls) goes through one software pipeline, run_host: the block list is cut
+// into chunks, and for each chunk H2D(inputs) -> kernel -> D2H(outputs) is enqueued on one of NSLOT streams, so that the
+// copy engines (both PCIe directions) and the SMs work on different chunks at the same time.  The mixed-memory batches
+// (MEM_DEVICE_TO_HOST, MEM_HOST_TO_DEVICE and the packed encode from device memory) and the LZ4Stream and Wrap / Unwrap
+// calls between device and host memory go through it too, skipping the copy of whichever side is already on the device.
+// The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
+// caller's bytes are on; the host only reads headers (framing.cpp).  There is no CPU codec in this library: if the device
+// or the kernel image is unusable every entry point reports an error.
 #include "../../include/lz4b200.h"
 #include "framing.h"
 #include "kernels.h"
@@ -120,13 +122,14 @@ struct Meta {
 };
 constexpr size_t META_BYTES = 32, WRAP_META_OFFSET = 32, WRAP_META_BYTES = WRAP_META_OFFSET + 20;
 
-// The framing calls between device and host memory inside the pipeline.
+// The framing calls inside the pipeline.
 //  LZ4Stream encode (APPEND, lz4_stream.cuh): the frames of the chunks replace the compaction, hc = the flags' HC bit.
 //  Wrap encode (wrap, lz4_wrap.cuh): dst_cap[i] = the packet's capacity, src_len[i] + 8.  The encoder writes each payload
 //    behind its header's place in the slot; the finish step writes the headers and the stored inputs and sets out_len to
 //    the packet sizes.  The slot then holds whole packets, which land like the blocks of an encode.
-//  Decode (dst on the device; LZ4Stream chunks, Unwrap packets): stored[i] != 0 marks a stored chunk or packet, whose
-//    payload is copied by the stored-copy step while the decoder gets the neutral entry (src_len 0, dst_cap 0).
+//  Decode (LZ4Stream chunks, Unwrap packets; dst in host or device memory): stored[i] != 0 marks a stored chunk or packet,
+//    whose payload is copied by the stored-copy step while the decoder gets the neutral entry (src_len 0, dst_cap 0).  In
+//    host memory it lands like a decoded block of dst_cap[i] bytes.
 struct Framing { bool hc; const uint8_t* stored; bool wrap; };
 
 }  // namespace
@@ -228,15 +231,15 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
 // nothing is compacted or landed, only out_len comes back: NONE).  A chunk is weighed by what it stages, so the slots'
 // device buffers stay within host_chunk_bytes whatever the batch.  The slots start behind everything enqueued on
 // `caller` before the call: a producer of src, or a reader of dst's old contents.
-// frames (the framing calls between device and host memory, see Framing): an APPEND LZ4Stream encode lands the chunks'
-// frames instead of the compacted blocks (out_off[i] = where frame i starts); a Wrap encode lands whole packets in any
-// mode; a decode also copies the stored chunks' or packets' payloads.
+// frames (the LZ4Stream and Wrap / Unwrap calls, see Framing): an APPEND LZ4Stream encode lands the chunks' frames instead
+// of the compacted blocks (out_off[i] = where frame i starts); a Wrap encode lands whole packets in any mode; a decode
+// also copies the stored chunks' or packets' payloads.
 int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
              const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op,
              int64_t* out_off, int64_t dst_total_cap, bool src_dev = false, bool dst_dev = false, cudaStream_t caller = nullptr,
              const Framing* frames = nullptr)
 {
-    const bool measure = op >= 4, wrap = frames && frames->wrap;
+    const bool measure = op >= 4, wrap = frames && frames->wrap, stored_copy = frames && frames->stored;
     for (int32_t i = 0; i < n; i++)
         if (src_len[i] < 0 || (dst_cap && dst_cap[i] < 0)) return fail(LZ4B200_E_ARG, "negative block length");
     const bool src_pageable = !src_dev && is_pageable(src), dst_pageable = !measure && !dst_dev && is_pageable(dst);
@@ -276,8 +279,10 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         std::memcpy(out_len + p.b0, h.out, sizeof(int32_t) * (size_t)m);
         if (p.mode == PER_BLOCK) {
             for (int32_t i = 0; i < m; i++) {
+                // a known-size decode produced dst_cap bytes when it succeeded, a stored copy (aux > 0: the decoder saw
+                // the neutral entry and failed it) always
                 const int32_t b = p.b0 + i, r = h.out[i];
-                const int64_t nbytes = op == 2 ? (r >= 0 ? dst_cap[b] : 0) : std::max(r, 0);
+                const int64_t nbytes = op == 2 ? (r >= 0 || (stored_copy && h.aux[i] > 0) ? dst_cap[b] : 0) : std::max(r, 0);
                 if (nbytes > 0)
                     CU(cudaMemcpyAsync(dst + dst_off[b], (uint8_t*)sl.dst.p + h.dof[i], (size_t)nbytes, cudaMemcpyDeviceToHost, sl.stream));
             }
@@ -339,7 +344,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
             if (dst_dev) h.dof[i] = dst_off[b0 + i];
             else { h.dof[i] = dsum; dsum += measure ? 0 : dst_cap[b0 + i]; }
             h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap ? dst_cap[b0 + i] : INT32_MAX;
-            if (frames && frames->stored) {
+            if (stored_copy) {
                 const bool stored = frames->stored[b0 + i] != 0;
                 h.aux[i] = stored ? h.sl[i] : 0;
                 if (stored) h.sl[i] = h.dc[i] = 0;
@@ -348,7 +353,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         const size_t sbytes = (size_t)(shi - slo);
         if (!src_dev) CU(sl.src.reserve(sbytes + 64));
         if (!dst_dev) CU(sl.dst.reserve((size_t)dsum + 64));
-        CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, (size_t)m * (frames && frames->stored ? 28 : 24), cudaMemcpyHostToDevice, sl.stream));
+        CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, (size_t)m * (stored_copy ? 28 : 24), cudaMemcpyHostToDevice, sl.stream));
         if (sbytes) {
             const uint8_t* from = src + slo;
             if (src_pageable && m > 8) { CU(sl.hsrc.reserve(sbytes)); par_memcpy(sl.hsrc.p, from, sbytes); from = (const uint8_t*)sl.hsrc.p; }
@@ -377,7 +382,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         } else {
             rc = run_device(c, a, op, sl.stream, lanes, hc_large); if (rc) return rc;
         }
-        if (frames && frames->stored) {
+        if (stored_copy) {
             cudaError_t e = launch_stream_stored(a, d.aux, sl.stream, &c->launches);
             if (e != cudaSuccess) return cuda_fail(e, "stored copy launch");
         }
@@ -521,15 +526,89 @@ int frame_scratch(lz4b200_ctx* c, int32_t n, bool packed, cudaStream_t st, WrapS
     DeviceGuard g((c)->device);                                                                       \
     if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
 
-// The LZ4Stream calls on device memory run the pipeline over at most this many chunks at a time: it bounds the host
-// metadata by chunk count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.
+// The LZ4Stream calls run the pipeline over at most this many chunks at a time: it bounds the host metadata by chunk
+// count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.
 constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
 
-// The Wrap packets of device inputs, landed in host memory: in the caller's slots, or packed (dst_off == nullptr, out_off
-// as in the packed encode).  Every argument is checked before any device work, as lz4b200_wrap_batch does.
-int wrap_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, int high_compression,
-                     void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n,
-                     int64_t* out_off, int64_t dst_total_cap, void* stream)
+// The LZ4Stream of n bytes in host or device memory (src_dev), written into host memory: each run of chunks is encoded
+// (capacity = the chunk's length, LZ4Stream.cs:243-246) and its frames land back to back (Framing, APPEND).  Returns the
+// stream's size.  Only a chunk whose frame does not fit an int32 is refused for its size.
+int64_t stream_encode(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_size, int high_compression, void* dst,
+                      int64_t dst_cap, bool src_dev, void* stream)
+{
+    if (!c || n < 0 || block_size < 1 || (n > 0 && (!src || !dst))) return fail(LZ4B200_E_ARG, "bad argument");
+    if (std::min<int64_t>(block_size, n) > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "a chunk's frame must fit an int32");
+    if (dst_cap < lz4b200_stream_bound(n, block_size)) return fail(LZ4B200_E_ARG, "dst_cap < lz4b200_stream_bound(n, block_size)");
+    if (n == 0) return 0;
+    std::lock_guard<std::mutex> lock(c->mu);
+    DeviceGuard g(c->device);
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    if (src_dev) {
+        int rc = check_side(c, src, true, "src"); if (rc) return rc;
+        rc = check_side(c, dst, false, "dst"); if (rc) return rc;
+    }
+    const int64_t chunks = (n + block_size - 1) / block_size;
+    const Framing f{high_compression != 0, nullptr, false};
+    std::vector<int64_t> so, at; std::vector<int32_t> len, res;
+    int64_t w = 0;
+    for (int64_t c0 = 0; c0 < chunks; c0 += STREAM_RUN_CHUNKS) {
+        const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, chunks - c0);
+        so.resize(m); len.resize(m); res.assign(m, 0); at.assign((size_t)m + 1, 0);
+        for (int32_t i = 0; i < m; i++) {
+            so[i] = (c0 + i) * block_size;
+            len[i] = (int32_t)std::min<int64_t>(block_size, n - so[i]);
+        }
+        int rc = run_host(c, (const uint8_t*)src, so.data(), len.data(), (uint8_t*)dst + w, nullptr, len.data(), res.data(), m,
+                          high_compression ? 1 : 0, at.data(), dst_cap - w, src_dev, false, (cudaStream_t)stream, &f);
+        if (rc) return rc;
+        w += at[m];
+    }
+    return w;
+}
+
+// The LZ4Stream of n bytes in host memory, decoded into host or device memory (dst_dev).  The whole header walk comes
+// before any device work, so a malformed stream writes nothing.  Returns the decoded size.
+int64_t stream_decode(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int64_t dst_cap, bool dst_dev, void* stream)
+{
+    if (!c || n < 0 || (n > 0 && !src)) return fail(LZ4B200_E_ARG, "bad argument");
+    std::lock_guard<std::mutex> lock(c->mu);
+    DeviceGuard g(c->device);
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    if (dst_dev) { int rc = check_side(c, src, false, "src"); if (rc) return rc; }
+    std::vector<StreamChunk> chunks;
+    const int64_t total = stream_walk((const uint8_t*)src, n, &chunks);
+    if (total < 0) return fail((int)total, "malformed LZ4Stream");
+    if (total > dst_cap || (total > 0 && !dst)) return fail(LZ4B200_E_ARG, "dst_cap < the decoded size");
+    if (total == 0) return 0;
+    if (dst_dev) { int rc = check_side(c, dst, true, "dst"); if (rc) return rc; }
+    // one entry per non-empty chunk; the flag is the header's (a compressed chunk may have compLen == rawLen, LZ4Stream.cs:288)
+    std::vector<int64_t> so, dof; std::vector<int32_t> len, raw, res; std::vector<uint8_t> stored;
+    int64_t pos = 0;
+    for (const StreamChunk& k : chunks) {
+        if (k.raw > 0) { so.push_back(k.payload); len.push_back(k.stored); dof.push_back(pos); raw.push_back(k.raw); stored.push_back(!k.compressed); }
+        pos += k.raw;
+    }
+    const int64_t entries = (int64_t)so.size();
+    for (int64_t e0 = 0; e0 < entries; e0 += STREAM_RUN_CHUNKS) {
+        const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, entries - e0);
+        res.assign(m, -1);
+        const Framing f{false, stored.data() + e0, false};
+        int rc = run_host(c, (const uint8_t*)src, so.data() + e0, len.data() + e0, (uint8_t*)dst, dof.data() + e0, raw.data() + e0,
+                          res.data(), m, 2, nullptr, 0, false, dst_dev, (cudaStream_t)stream, &f);
+        if (rc) return rc;
+        // a compressed chunk decodes from exactly its compLen bytes (LZ4Codec.Safe.cs:539-542)
+        for (int32_t i = 0; i < m; i++)
+            if (!stored[e0 + i] && res[i] != len[e0 + i]) return fail(LZ4B200_E_FORMAT, "a chunk does not decode to its compressed length");
+    }
+    return total;
+}
+
+// The Wrap packets of inputs in host or device memory (src_dev), landed in host memory: in the caller's slots, or packed
+// (dst_off == nullptr, out_off as in the packed encode).  Every argument is checked before any device work: a negative
+// length or a slot too small for its packet fails the whole call.
+int wrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, int high_compression,
+                 void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n,
+                 int64_t* out_off, int64_t dst_total_cap, bool src_dev, void* stream)
 {
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
@@ -545,35 +624,60 @@ int wrap_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, co
     std::lock_guard<std::mutex> lock(c->mu);
     DeviceGuard g(c->device);
     if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
-    int rc = check_side(c, src, true, "src"); if (rc) return rc;
-    rc = check_side(c, dst, false, "dst"); if (rc) return rc;
+    if (src_dev) {
+        int rc = check_side(c, src, true, "src"); if (rc) return rc;
+        rc = check_side(c, dst, false, "dst"); if (rc) return rc;
+    }
     const Framing f{false, nullptr, true};
     return run_host(c, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, pcap.data(), out_len, n,
-                    high_compression ? 1 : 0, out_off, dst_total_cap, true, false, (cudaStream_t)stream, &f);
+                    high_compression ? 1 : 0, out_off, dst_total_cap, src_dev, false, (cudaStream_t)stream, &f);
 }
 
-// The headers of n packets in host memory (framing.h read_header), read by several threads: small packets far apart in a
-// large batch cost a cache and TLB miss each, and one thread would then take longer than the link.
-struct WrapHeader { int32_t raw, stored, size; };
-std::vector<WrapHeader> read_headers(const uint8_t* src, const int64_t* src_off, const int32_t* src_len, int32_t n)
+// Unwrap n packets in host memory into host or device memory (dst_dev): into the caller's slots, or packed (dst_off ==
+// nullptr: packet i at out_off[i], the prefix sum of the sizes, out_off[n] the total; nothing is restored and out_len holds
+// the sizes when the total exceeds dst_total_cap).  The headers are read first, by several threads: small packets far
+// apart in a large batch cost a cache and TLB miss each, and one thread would then take longer than the link.  A rejected
+// packet gets its status before any device work (E_FORMAT, or E_ARG above its capacity), an empty one 0.  Every other
+// packet is one entry of a known-size decode: a compressed one decodes its stored bytes into raw bytes, a stored one is
+// copied (Framing::stored).
+int unwrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                   const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
+                   int64_t dst_total_cap, bool dst_dev, void* stream)
 {
-    std::vector<WrapHeader> h((size_t)n);
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
+    if (n == 0) { if (out_off) out_off[0] = 0; return LZ4B200_OK; }
+    if (!src || !src_off || !src_len || !dst || !out_len || (dst_off ? !dst_cap : !out_off)) return fail(LZ4B200_E_ARG, "null argument");
+    std::lock_guard<std::mutex> lock(c->mu);
+    DeviceGuard g(c->device);
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    if (dst_dev) {
+        int rc = check_side(c, src, false, "src"); if (rc) return rc;
+        rc = check_side(c, dst, true, "dst"); if (rc) return rc;
+    }
+    const uint8_t* s = (const uint8_t*)src;
+    struct Header { int32_t raw, stored, size; };
+    std::vector<Header> hdr((size_t)n);
     par_ranges((size_t)n, 4096, [&](size_t lo, size_t hi) {
-        for (size_t i = lo; i < hi; i++) h[i].size = read_header(src + src_off[i], src_len[i], &h[i].raw, &h[i].stored);
+        for (size_t i = lo; i < hi; i++) hdr[i].size = read_header(s + src_off[i], src_len[i], &hdr[i].raw, &hdr[i].stored);
     });
-    return h;
-}
-
-// Unwrap from host memory into device memory, the caller holding the lock with both sides checked and the headers read.
-// A rejected packet gets its status before any device work (E_FORMAT, or E_ARG above its capacity), an empty one 0.
-// Every other packet is one entry of a known-size decode: a compressed one decodes its stored bytes into raw bytes, a
-// stored one is copied (Framing::stored).
-int unwrap_to_device(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const WrapHeader* hdr, uint8_t* dst,
-                     const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, cudaStream_t stream)
-{
+    std::vector<int32_t> sizes;
+    if (!dst_off) {
+        sizes.resize((size_t)n);
+        int64_t total = 0;
+        for (int32_t i = 0; i < n; i++) {
+            out_len[i] = hdr[i].size;
+            sizes[i] = std::max(hdr[i].size, 0);
+            out_off[i] = total;
+            total += sizes[i];
+        }
+        out_off[n] = total;
+        if (total > dst_total_cap) return LZ4B200_OK;
+        dst_off = out_off; dst_cap = sizes.data();
+    }
     std::vector<int64_t> so, dof; std::vector<int32_t> len, cap, res, idx; std::vector<uint8_t> stored;
     for (int32_t i = 0; i < n; i++) {
-        const WrapHeader& h = hdr[i];
+        const Header& h = hdr[i];
         out_len[i] = h.size >= 0 && h.size > dst_cap[i] ? LZ4B200_E_ARG : h.size;
         if (out_len[i] <= 0) continue;
         so.push_back(src_off[i] + WRAP_HEADER); len.push_back(h.stored); dof.push_back(dst_off[i]); cap.push_back(h.size);
@@ -583,10 +687,11 @@ int unwrap_to_device(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off,
     const int32_t m = (int32_t)so.size();
     res.assign((size_t)m, -1);
     const Framing f{false, stored.data(), false};
-    int rc = run_host(c, src, so.data(), len.data(), dst, dof.data(), cap.data(), res.data(), m, 2, nullptr, 0, false, true, stream, &f);
+    int rc = run_host(c, s, so.data(), len.data(), (uint8_t*)dst, dof.data(), cap.data(), res.data(), m, 2, nullptr, 0, false,
+                      dst_dev, (cudaStream_t)stream, &f);
     if (rc) return rc;
-    // a compressed packet decodes from exactly its stored bytes (framing.cpp lz4b200_unwrap_batch); one that does not is
-    // that packet's E_FORMAT, not the call's
+    // a compressed packet decodes from exactly its stored bytes (LZ4Codec.cs:595); one that does not is that packet's
+    // E_FORMAT, not the call's
     for (int32_t j = 0; j < m; j++)
         if (!stored[j]) out_len[idx[j]] = res[j] == len[j] ? cap[j] : LZ4B200_E_FORMAT;
     return LZ4B200_OK;
@@ -701,73 +806,29 @@ int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* c, const void* src, con
                  LZ4B200_MEM_DEVICE_TO_HOST, stream, out_off, dst_total_cap);
 }
 
-// ---- LZ4Stream between device and host memory (lz4_stream.cuh): the host pipeline, the frames written on the device ----
+// ---- LZ4Stream (lz4_stream.cuh): the host pipeline, the frames written on the device ----------------------------------
+int64_t lz4b200_stream_encode(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_size, int high_compression, void* dst,
+                              int64_t dst_cap)
+{
+    return stream_encode(c, src, n, block_size, high_compression, dst, dst_cap, false, nullptr);
+}
+
+int64_t lz4b200_stream_decode(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int64_t dst_cap)
+{
+    return stream_decode(c, src, n, dst, dst_cap, false, nullptr);
+}
+
 int64_t lz4b200_stream_encode_from_device(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_size, int high_compression,
                                           void* dst, int64_t dst_cap, void* stream)
 {
-    if (!c || n < 0 || block_size < 1 || (n > 0 && (!src || !dst))) return fail(LZ4B200_E_ARG, "bad argument");
     if (block_size > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "block_size: a chunk's frame must fit an int32");
-    if (dst_cap < lz4b200_stream_bound(n, block_size)) return fail(LZ4B200_E_ARG, "dst_cap < lz4b200_stream_bound(n, block_size)");
-    if (n == 0) return 0;
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
-    int rc = check_side(c, src, true, "src"); if (rc) return rc;
-    rc = check_side(c, dst, false, "dst"); if (rc) return rc;
-    const int64_t chunks = (n + block_size - 1) / block_size;
-    const Framing f{high_compression != 0, nullptr, false};
-    std::vector<int64_t> so, at; std::vector<int32_t> len, res;
-    int64_t w = 0;
-    for (int64_t c0 = 0; c0 < chunks; c0 += STREAM_RUN_CHUNKS) {
-        const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, chunks - c0);
-        so.resize(m); len.resize(m); res.assign(m, 0); at.assign((size_t)m + 1, 0);
-        for (int32_t i = 0; i < m; i++) {
-            so[i] = (c0 + i) * block_size;
-            len[i] = (int32_t)std::min<int64_t>(block_size, n - so[i]);      // capacity = the chunk's length (LZ4Stream.cs:243-246)
-        }
-        rc = run_host(c, (const uint8_t*)src, so.data(), len.data(), (uint8_t*)dst + w, nullptr, len.data(), res.data(), m,
-                      high_compression ? 1 : 0, at.data(), dst_cap - w, true, false, (cudaStream_t)stream, &f);
-        if (rc) return rc;
-        w += at[m];
-    }
-    return w;
+    return stream_encode(c, src, n, block_size, high_compression, dst, dst_cap, true, stream);
 }
 
 int64_t lz4b200_stream_decode_to_device(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int64_t dst_cap, void* stream)
 {
-    if (!c || n < 0 || (n > 0 && !src)) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n == 0) return 0;
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
-    int rc = check_side(c, src, false, "src"); if (rc) return rc;
-    // the whole header walk before any device work: a malformed stream writes nothing
-    std::vector<StreamChunk> chunks;
-    const int64_t total = stream_walk((const uint8_t*)src, n, &chunks);
-    if (total < 0) return fail((int)total, "malformed LZ4Stream");
-    if (total > dst_cap || (total > 0 && !dst)) return fail(LZ4B200_E_ARG, "dst_cap < the decoded size");
-    if (total == 0) return 0;
-    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
-    // one entry per non-empty chunk; the flag is the header's (a compressed chunk may have compLen == rawLen, LZ4Stream.cs:288)
-    std::vector<int64_t> so, dof; std::vector<int32_t> len, raw, res; std::vector<uint8_t> stored;
-    int64_t pos = 0;
-    for (const StreamChunk& k : chunks) {
-        if (k.raw > 0) { so.push_back(k.payload); len.push_back(k.stored); dof.push_back(pos); raw.push_back(k.raw); stored.push_back(!k.compressed); }
-        pos += k.raw;
-    }
-    const int64_t entries = (int64_t)so.size();
-    for (int64_t e0 = 0; e0 < entries; e0 += STREAM_RUN_CHUNKS) {
-        const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, entries - e0);
-        res.assign(m, -1);
-        const Framing f{false, stored.data() + e0, false};
-        rc = run_host(c, (const uint8_t*)src, so.data() + e0, len.data() + e0, (uint8_t*)dst, dof.data() + e0, raw.data() + e0,
-                      res.data(), m, 2, nullptr, 0, false, true, (cudaStream_t)stream, &f);
-        if (rc) return rc;
-        // a compressed chunk decodes from exactly its compLen bytes (framing.cpp, LZ4Codec.Safe.cs:539-542)
-        for (int32_t i = 0; i < m; i++)
-            if (!stored[e0 + i] && res[i] != len[e0 + i]) return fail(LZ4B200_E_FORMAT, "a chunk does not decode to its compressed length");
-    }
-    return total;
+    if (c && n == 0) return 0;
+    return stream_decode(c, src, n, dst, dst_cap, true, stream);
 }
 
 int lz4b200_decode_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
@@ -906,13 +967,24 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     return LZ4B200_OK;
 }
 
-// ---- Wrap / Unwrap packets between device and host memory: the host pipeline (run_host, Framing) ----
+// ---- Wrap / Unwrap packets with a side in host memory: the host pipeline (run_host, Framing) ----
+int lz4b200_wrap_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, int high_compression,
+                       void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n)
+{
+    return wrap_packets(c, src, src_off, src_len, high_compression, dst, dst_off, dst_cap, out_len, n, nullptr, 0, false, nullptr);
+}
+
+int lz4b200_unwrap_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                         const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n)
+{
+    return unwrap_packets(c, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, nullptr, 0, false, nullptr);
+}
+
 int lz4b200_wrap_batch_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
                                    int high_compression, void* dst, const int64_t* dst_off, const int32_t* dst_cap,
                                    int32_t* out_len, int32_t n, void* stream)
 {
-    if (!dst_off && n > 0) return fail(LZ4B200_E_ARG, "null argument");        // (a null dst_off means packed inside)
-    return wrap_from_device(c, src, src_off, src_len, high_compression, dst, dst_off, dst_cap, out_len, n, nullptr, 0, stream);
+    return wrap_packets(c, src, src_off, src_len, high_compression, dst, dst_off, dst_cap, out_len, n, nullptr, 0, true, stream);
 }
 
 int lz4b200_wrap_batch_packed_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
@@ -920,47 +992,22 @@ int lz4b200_wrap_batch_packed_from_device(lz4b200_ctx* c, const void* src, const
                                           int32_t* out_len, int32_t n, void* stream)
 {
     if (!out_off) return fail(LZ4B200_E_ARG, "bad argument");
-    return wrap_from_device(c, src, src_off, src_len, high_compression, dst, nullptr, nullptr, out_len, n, out_off,
-                            dst_total_cap, stream);
+    return wrap_packets(c, src, src_off, src_len, high_compression, dst, nullptr, nullptr, out_len, n, out_off, dst_total_cap,
+                        true, stream);
 }
 
 int lz4b200_unwrap_batch_to_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
                                    const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
 {
-    FRAME_CALL_PROLOGUE(c, n)
-    if (n == 0) return LZ4B200_OK;
-    if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    int rc = check_side(c, src, false, "src"); if (rc) return rc;
-    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
-    const std::vector<WrapHeader> hdr = read_headers((const uint8_t*)src, src_off, src_len, n);
-    return unwrap_to_device(c, (const uint8_t*)src, src_off, hdr.data(), (uint8_t*)dst, dst_off, dst_cap, out_len, n,
-                            (cudaStream_t)stream);
+    return unwrap_packets(c, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, nullptr, 0, true, stream);
 }
 
-// the sizes from the headers, on the host, then the unwrap into slots at their prefix sums
 int lz4b200_unwrap_batch_packed_to_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
                                           void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
                                           void* stream)
 {
-    FRAME_CALL_PROLOGUE(c, n)
     if (!out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
-    if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    int rc = check_side(c, src, false, "src"); if (rc) return rc;
-    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
-    const std::vector<WrapHeader> hdr = read_headers((const uint8_t*)src, src_off, src_len, n);
-    std::vector<int32_t> cap((size_t)n);
-    int64_t total = 0;
-    for (int32_t i = 0; i < n; i++) {
-        out_len[i] = hdr[i].size;
-        cap[i] = std::max(hdr[i].size, 0);
-        out_off[i] = total;
-        total += cap[i];
-    }
-    out_off[n] = total;
-    if (total > dst_total_cap) return LZ4B200_OK;
-    return unwrap_to_device(c, (const uint8_t*)src, src_off, hdr.data(), (uint8_t*)dst, out_off, cap.data(), out_len, n,
-                            (cudaStream_t)stream);
+    return unwrap_packets(c, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off, dst_total_cap, true, stream);
 }
 
 int lz4b200_synth_fill(lz4b200_ctx* c, void* dst, int64_t n_blocks, int32_t block_size, int cls, uint64_t seed,

@@ -1,6 +1,7 @@
-// framing.h -- internal interface of framing.cpp: the LZ4Stream header walk and the Wrap packet header, shared by the host
-// calls and the decodes into device memory (capi.cu lz4b200_stream_decode_to_device, lz4b200_unwrap_batch_to_device), so
-// that both read a stream or a packet by the same rules.
+// framing.h -- internal interface of framing.cpp, the host-side reader of the framing formats: the LZ4Stream header walk
+// and the Wrap packet header, read before any device work by the LZ4Stream decode and the Unwrap calls (capi.cu
+// stream_decode, unwrap_packets) and by the size queries of the C ABI.  The writers are on the device (lz4_stream.cuh,
+// lz4_wrap.cuh).
 #pragma once
 #include <stdint.h>
 

@@ -1,17 +1,17 @@
-// lz4_stream.cuh -- the LZ4Stream chunk frame (src/LZ4/LZ4Stream.cs:239-269) written and read on the device, for the
-// mixed-memory stream calls (capi.cu lz4b200_stream_encode_from_device / stream_decode_to_device).
+// lz4_stream.cuh -- the LZ4Stream chunk frame (src/LZ4/LZ4Stream.cs:239-269) written and read on the device, for every
+// stream call (capi.cu stream_encode / stream_decode: host or device raw bytes, stream bytes in host memory).
 //
 // A chunk is  varint(flags) varint(rawLen) [varint(compLen)] payload : the compressed bytes, or the raw bytes when the
 // encoder's result r (at capacity = rawLen) does not satisfy 0 < r < rawLen (:248-255).  flags = compressed (1) | HC (2);
 // the HC bit is set on stored chunks too (:257-264).  The stream bytes live in host memory and the host walks their
-// headers (framing.cpp stream_walk); the device only writes the frames of an encode and copies the stored payloads of a
+// headers (framing.cpp stream_walk); the device writes the frames of an encode and copies the stored payloads of a
 // decode:
 //   encode:  encode (capacity = chunk length) -> frame sizes (a thread per chunk) -> scan (launch_compact without a
 //            payload) -> frame write (a warp per chunk: header bytes, then the payload from the encoder's slot or, for a
-//            stored chunk, from the caller's device source)
+//            stored chunk, from the source: the caller's device memory, or the pipeline's staged copy of host bytes)
 //   decode:  known-size decode of the compressed chunks (stored ones get the neutral entry, see lz4_wrap.cuh) -> stored
 //            copy (a warp per chunk: a stored chunk's payload to its place in the output; compressed chunks do nothing)
-// The rules restate framing.cpp (lz4b200_stream_encode), so the frames are the same whichever side wrote them.
+// This is the library's only writer of the format.
 #pragma once
 #include "lz4_copy.cuh"
 
@@ -22,7 +22,7 @@ constexpr int32_t STREAM_HEADER_MAX = 11;                             // flags (
 
 SIMT_DEV int stream_varint_size(uint32_t v) { return v < (1u << 7) ? 1 : v < (1u << 14) ? 2 : v < (1u << 21) ? 3 : v < (1u << 28) ? 4 : 5; }
 
-// the chunk is compressed when the encoder's result shrinks it (LZ4Stream.cs:248-255, framing.cpp:120)
+// the chunk is compressed when the encoder's result shrinks it (LZ4Stream.cs:248-255)
 SIMT_DEV bool stream_compressed(int32_t raw, int32_t r) { return r > 0 && r < raw; }
 
 SIMT_DEV int32_t stream_header_size(int32_t raw, int32_t r)

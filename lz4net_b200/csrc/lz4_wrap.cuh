@@ -1,4 +1,4 @@
-// lz4_wrap.cuh -- the Wrap / Unwrap packet (src/LZ4/LZ4Codec.cs:510-543, 574-599) around the batch codec, in device memory.
+// lz4_wrap.cuh -- the Wrap / Unwrap packet (src/LZ4/LZ4Codec.cs:510-543, 574-599) around the batch codec, on the device.
 //
 // A packet is  u32le rawLen, u32le storedLen, payload : the compressed bytes, or the input itself when compression does not
 // shrink it (storedLen == rawLen).  The device entry points (capi.cu lz4b200_wrap_batch_device / unwrap_batch_device /
@@ -10,8 +10,9 @@
 // A neutral decode entry (src_len 0, dst_cap 0) reads and writes nothing in every decoder: they all reject an empty stream
 // before touching it (decode_block / decode_block_staged / lpb_decode_warp: isize <= 0), and only their result, which
 // the finish step ignores, is stored.
-// The rules restate framing.cpp (read_header, the stored-raw rule of lz4b200_wrap_batch, the status of
-// lz4b200_unwrap_batch), so a packet and a status are the same whichever side made them.
+// The wrap side is the library's only writer of the packet: the calls with a side in host memory (capi.cu wrap_packets)
+// run the same prep and finish inside the host pipeline.  Those unwraps read the headers on the host (framing.cpp
+// read_header, the same rules as unwrap_header) and reuse the stored copy of lz4_stream.cuh.
 #pragma once
 #include "lz4_copy.cuh"
 
@@ -21,7 +22,7 @@ constexpr int32_t WRAP_HEADER = 8;
 constexpr int32_t WRAP_E_ARG = -1, WRAP_E_FORMAT = -5;           // LZ4B200_E_ARG / LZ4B200_E_FORMAT
 
 // ---- wrap -----------------------------------------------------------------------------------------------------------
-// The packet is valid when its input length is not negative and its capacity holds input + header (framing.cpp:208).
+// The packet is valid when its input length is not negative (LZ4Codec.cs:513-514) and its capacity holds input + header.
 SIMT_DEV bool wrap_valid(int32_t len, int32_t cap) { return len >= 0 && (int64_t)cap >= (int64_t)len + WRAP_HEADER; }
 
 // Prep: what the encoder sees of packet i.  An invalid packet, or an empty input, is given nothing to read and capacity 0,
@@ -34,7 +35,7 @@ SIMT_DEV void wrap_prep_one(int64_t dst_off, int32_t len, int32_t cap, int64_t* 
     *enc_cap = go ? len : 0;
 }
 
-// Stored unless compression shrinks the input (LZ4Codec.cs:527-540, framing.cpp:220).  r = the encoder's result.
+// Stored unless compression shrinks the input (LZ4Codec.cs:527-540).  r = the encoder's result.
 SIMT_DEV int32_t wrap_stored(int32_t len, int32_t r) { return r >= len || r <= 0 ? len : r; }
 
 // Finish, called by all 32 lanes of a warp with the same arguments: writes the header (and, for a stored packet, the input
@@ -55,7 +56,7 @@ SIMT_DEV int32_t wrap_finish_one(const uint8_t* in, int32_t len, int32_t cap, in
 }
 
 // ---- unwrap ---------------------------------------------------------------------------------------------------------
-// read_header (framing.cpp:49-57): the unwrapped size, or LZ4B200_E_FORMAT.  The header is read only when the packet holds
+// The packet header (LZ4Codec.cs:574-599): the unwrapped size, or LZ4B200_E_FORMAT.  The header is read only when the packet holds
 // it, byte by byte: a packet shorter than 8 bytes, or one at any alignment, never reads a byte outside itself.
 SIMT_DEV int32_t unwrap_header(const uint8_t* p, int32_t n, int32_t* raw, int32_t* stored)
 {
@@ -74,7 +75,7 @@ SIMT_DEV int32_t unwrap_prep_one(const uint8_t* p, int32_t n, int32_t cap, int32
 {
     int32_t raw = 0, stored = 0;
     int32_t size = unwrap_header(p, n, &raw, &stored);
-    if (size >= 0 && size > cap) size = WRAP_E_ARG;                                     // framing.cpp:243
+    if (size >= 0 && size > cap) size = WRAP_E_ARG;                                     // a slot too small
     const bool comp = size >= 0 && stored < raw;
     *dec_len = comp ? stored : 0;
     *dec_cap = comp ? raw : 0;
@@ -83,7 +84,7 @@ SIMT_DEV int32_t unwrap_prep_one(const uint8_t* p, int32_t n, int32_t cap, int32
 
 // Finish, called by all 32 lanes of a warp with the same arguments: size = what the prep returned, (dec_len, dec_cap) its
 // decode entry, read = the decoder's result for it.  Copies a stored payload to dst and returns out_len: the stored
-// length, bytes restored when the decoder read exactly the stored bytes (framing.cpp:252), else LZ4B200_E_FORMAT; a
+// length, bytes restored when the decoder read exactly the stored bytes (LZ4Codec.cs:595), else LZ4B200_E_FORMAT; a
 // rejected packet keeps its status.
 SIMT_DEV int32_t unwrap_finish_one(const uint8_t* p, int32_t size, int32_t dec_len, int32_t dec_cap, int32_t read, uint8_t* dst, int lane)
 {

@@ -382,24 +382,51 @@ def test_wrap_unwrap(ctx):
         LZ4Codec.Unwrap(b"\x01\x02\x03")
 
 
+def _wrap_batch_pinned(ctx, inputs, hc):
+    """lz4b200_wrap_batch into page-locked slots 5 bytes larger than the packets' capacity, filled with guard bytes: the
+    packets; nothing behind a packet in its slot is written."""
+    import torch
+    from lz4net_b200 import codec, native
+    src, lens, so = codec._pack(inputs)
+    caps = lens + 8 + 5
+    do = codec._offsets(caps)
+    dst = torch.full((int(caps.sum()) + 16,), 0xEE, dtype=torch.uint8).pin_memory().numpy()
+    out = np.zeros(len(inputs), np.int32)
+    native.check(native.lib().lz4b200_wrap_batch(ctx.handle, src.ctypes.data, so.ctypes.data, lens.ctypes.data, int(hc),
+                                                 dst.ctypes.data, do.ctypes.data, caps.ctypes.data, out.ctypes.data,
+                                                 len(inputs)), "wrap_batch")
+    for o, r, c in zip(do, out, caps):
+        assert (dst[o + r:o + c] == 0xEE).all(), "a byte behind a packet changed"
+    return [dst[int(o):int(o) + int(r)].tobytes() for o, r in zip(do, out)]
+
+
 @pytest.mark.parametrize("hc", [False, True])
 def test_wrap_unwrap_batch(ctx, hc):
     """n packets through ONE batch (lz4b200_wrap_batch / unwrap_batch): every packet is byte for byte what the per-packet
-    call and the reference rule (src/LZ4/LZ4Codec.cs:510-543: stored when compression does not shrink it) produce."""
+    call and the reference rule (src/LZ4/LZ4Codec.cs:510-543: stored when compression does not shrink it) produce.  With
+    the default and with 1 MiB pipeline stages (a batch over several stages), into pageable and page-locked slots."""
     from lz4net_b200 import LZ4Codec, codec
     inputs = [cases.LOREM, cases.content("E0", 2048, 0).tobytes(), b"a", b"", cases.AUTOTEST, cases.content("ETEXT", 70000, 1).tobytes()]
     inputs += [cases.content(m, n, seed=3 + i).tobytes() for i, m in enumerate(cases.MODELS) for n in (1, 100, 5000, 65536)]
-    packets = codec.wrap_batch(inputs, hc=hc)
-    single = LZ4Codec.WrapHC if hc else LZ4Codec.Wrap
-    for d, p in zip(inputs, packets):
+    wants = []
+    for d in inputs:
         r, o = (oracle.encode_hc if hc else oracle.encode)(d, cap=len(d)) if d else (0, b"")
-        want = bytes(8) if not d else (len(d).to_bytes(4, "little") * 2 + d if (r >= len(d) or r <= 0) else len(d).to_bytes(4, "little") + r.to_bytes(4, "little") + o)
-        assert p == want, len(d)
-    assert packets[:6] == [single(d) for d in inputs[:6]]
-    assert codec.unwrap_batch(packets) == inputs
-    bad = list(packets); bad[3] = b"\x01\x02\x03"
-    with pytest.raises(ValueError):
-        codec.unwrap_batch(bad)
+        wants.append(bytes(8) if not d else (len(d).to_bytes(4, "little") * 2 + d if (r >= len(d) or r <= 0) else len(d).to_bytes(4, "little") + r.to_bytes(4, "little") + o))
+    single = LZ4Codec.WrapHC if hc else LZ4Codec.Wrap
+    for chunk_mb in (128, 1):
+        ctx.set_option("host_chunk_mb", chunk_mb)
+        try:
+            packets = codec.wrap_batch(inputs, hc=hc)
+            for d, p, want in zip(inputs, packets, wants):
+                assert p == want, (chunk_mb, len(d))
+            assert _wrap_batch_pinned(ctx, inputs, hc) == wants, chunk_mb
+            assert packets[:6] == [single(d) for d in inputs[:6]]
+            assert codec.unwrap_batch(packets) == inputs
+            bad = list(packets); bad[3] = b"\x01\x02\x03"
+            with pytest.raises(ValueError):
+                codec.unwrap_batch(bad)
+        finally:
+            ctx.set_option("host_chunk_mb", 128)
 
 
 def _ref_stream(data, block_size, hc):
@@ -423,16 +450,38 @@ def _ref_stream(data, block_size, hc):
     return bytes(out)
 
 
+def _stream_encode_pinned(ctx, data, block_size, hc):
+    """lz4b200_stream_encode into page-locked memory with guard bytes behind the bound: the stream; nothing behind it is
+    written."""
+    import torch
+    from lz4net_b200 import native
+    l = native.lib()
+    src = np.frombuffer(bytes(data) + b"\0", np.uint8)
+    cap = int(l.lz4b200_stream_bound(len(data), block_size))
+    dst = torch.full((cap + 64,), 0xEE, dtype=torch.uint8).pin_memory().numpy()
+    w = l.lz4b200_stream_encode(ctx.handle, src.ctypes.data, len(data), block_size, int(hc), dst.ctypes.data, cap)
+    assert w >= 0 and (dst[w:] == 0xEE).all(), w
+    return dst[:w].tobytes()
+
+
 @pytest.mark.parametrize("hc", [False, True])
 def test_lz4stream_wire_format(ctx, hc):
-    """StreamTests.cs:22-63 shape: write, read back; plus byte equality of the chunk stream with the reference format."""
+    """StreamTests.cs:22-63 shape: write, read back; plus byte equality of the chunk stream with the reference format.
+    With the default and with 1 MiB pipeline stages (then three times the data: a stream over several stages), into
+    pageable and page-locked memory."""
     data = b"".join(cases.content(m, n, seed=9).tobytes() for m, n in
                     (("ETEXT", 200000), ("E0", 70000), ("E100", 130000), ("mixed", 65536), ("lowent", 12345)))
-    for bs in (65536, 1 << 20, 1000, 16):
-        d = data if bs >= 1000 else data[:3000]
-        s = ctx.stream_encode(d, bs, hc)
-        assert s == _ref_stream(d, bs, hc), bs
-        assert ctx.stream_decode(s) == d
+    for chunk_mb in (128, 1):
+        ctx.set_option("host_chunk_mb", chunk_mb)
+        try:
+            for bs in (65536, 1 << 20, 1000, 16):
+                d = (data if chunk_mb == 128 else data * 3) if bs >= 1000 else data[:3000]
+                s = ctx.stream_encode(d, bs, hc)
+                assert s == _ref_stream(d, bs, hc), (chunk_mb, bs)
+                assert _stream_encode_pinned(ctx, d, bs, hc) == s, (chunk_mb, bs)
+                assert ctx.stream_decode(s) == d
+        finally:
+            ctx.set_option("host_chunk_mb", 128)
     assert ctx.stream_encode(b"", 65536, hc) == b"" and ctx.stream_decode(b"") == b""
     s = ctx.stream_encode(data[:100000], 65536, hc)
     with pytest.raises((EOFError, ValueError)):

@@ -14,7 +14,7 @@ import pytest
 
 from tests import cases
 from tests.test_mixed_memory_gpu import _busy, _host, _Options, CHUNK_MB_DEFAULT
-from tests.test_wrap_device_gpu import _corrupt, _host_unwrap, _host_unwrap_sized, _host_wrap, _sizes, _src, ref_wrap
+from tests.test_wrap_device_gpu import _corrupt, _device_unwrap, _host_unwrap, _host_unwrap_sized, _host_wrap, _sizes, _src, ref_wrap
 
 pytestmark = pytest.mark.gpu
 
@@ -181,10 +181,16 @@ def _status_cases(ctx):
 @pytest.mark.parametrize("chunk_mb", [1, CHUNK_MB_DEFAULT], ids=["many-stages", "default-stages"])
 def test_gpu_unwrap_to_device_statuses_equal_host(ctx, chunk_mb):
     """Packets of 0-7 bytes, storedLen > n - 8, lengths of 2^31 or more, size-0 packets, payloads cut short, trailing
-    bytes, bit flips, a capacity one byte short: statuses and restored bytes equal lz4b200_unwrap_batch's."""
+    bytes, bit flips, a capacity one byte short: statuses and restored bytes equal lz4b200_unwrap_batch's, and both equal
+    those of lz4b200_unwrap_batch_device, which reads the headers on the device instead of the host."""
     pairs = _status_cases(ctx)
     packets, caps = [p for p, _ in pairs], [c for _, c in pairs]
     want, wout = _host_unwrap(ctx, packets, caps)
+    dev, dout = _device_unwrap(ctx, packets, caps)
+    assert dev == want
+    for i, w in enumerate(want):
+        if w >= 0:
+            assert dout[i] == wout[i], i
     with _Options(ctx, host_chunk_mb=chunk_mb):
         got, gout = _unwrap_slots(ctx, packets, caps)
         want_nolimit, wout_nl = _host_unwrap_sized(ctx, packets)
