@@ -110,11 +110,34 @@ int lz4b200_measure_batch(lz4b200_ctx* ctx, const void* src, const int64_t* src_
  * dst + out_off[i] with capacity = its measured size and out_len[i] is the decoder's result (a malformed block reports a
  * negative value and occupies no bytes).  Otherwise dst is not touched and out_len[i] holds the measured sizes: allocate
  * out_off[n] bytes and call again.
- * There is no host-memory form: the host pipeline sizes its chunks by decoded bytes, which this call learns only on the
- * device.  Host callers use lz4b200_measure_batch, then lz4b200_decode_batch. */
+ * Blocks in host memory wanted in device memory: lz4b200_decode_batch_packed_to_device below.  There is no form with a
+ * host DESTINATION: the host pipeline sizes the device output buffer of a chunk by decoded bytes, which this call learns
+ * only on the device.  Callers who want the output in host memory use lz4b200_measure_batch, then lz4b200_decode_batch. */
 int lz4b200_decode_batch_packed(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
                                 void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n_blocks,
                                 void* stream);
+
+/* decode_batch_packed_to_device: the same for blocks in host memory (a file, a key-value store, a socket: compressed
+ * lengths only) wanted decoded in device memory.  src: host memory, pageable or page-locked; dst: device memory of the
+ * context's GPU; src_off, src_len, out_off (n_blocks+1 entries) and out_len are host arrays.  The contract of every mixed
+ * call (LZ4B200_MEM_HOST_TO_DEVICE above): synchronous, ordered behind the work already queued on `stream`, LZ4B200_E_ARG
+ * when src is device memory or dst is not memory of the context's GPU; only the compressed bytes cross PCIe, ONCE (not
+ * once to be measured and once to be decoded), and device scratch stays at the per-stage size whatever n_blocks is.
+ *   - out_off[0..n] = exclusive prefix sum of max(size_i, 0), size_i = what lz4b200_measure_batch(known_len = 0, dst_cap =
+ *     NULL) reports for block i; out_off[n] = the total.  They are filled whether the total fits or not.
+ *   - out_off[n] <= dst_total_cap: block i is decoded to dst + out_off[i] with capacity size_i; out_off, out_len and the
+ *     bytes dst[0, out_off[n]) equal what lz4b200_decode_batch_packed gives for a device copy of the batch.  A malformed
+ *     block reports a negative out_len[i] and occupies no bytes: that block's status, not the call's.
+ *   - out_off[n] > dst_total_cap: still LZ4B200_OK.  Nothing outside [dst, dst + dst_total_cap) is written, the bytes
+ *     inside it are unspecified, and out_len[i] is non-negative exactly for the well-formed blocks, where it equals size_i.
+ *     Allocate out_off[n] bytes and call again.  This is weaker than lz4b200_decode_batch_packed's "dst is not touched", on
+ *     purpose: the batch is decoded a pipeline stage at a time, the total is known only when the last stage has been
+ *     uploaded, and holding the decoded output back until then would take the second pass over the compressed bytes that
+ *     this call exists to avoid.  (A stage is decoded when everything up to its end fits.)
+ *   - n_blocks == 0 is LZ4B200_OK with out_off[0] = 0; a negative src_len[i] is LZ4B200_E_ARG before any device work. */
+int lz4b200_decode_batch_packed_to_device(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                          void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len,
+                                          int32_t n_blocks, void* stream);
 
 /* Host-memory encode with PACKED output: block i's compressed bytes land at dst + out_off[i] (out_off has n_blocks+1
  * entries; out_off[n_blocks] = total bytes written <= dst_total_cap), back to back in block order -- the layout the

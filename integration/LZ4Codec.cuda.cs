@@ -56,6 +56,9 @@ namespace LZ4
         private static extern unsafe int lz4b200_decode_batch_packed(IntPtr ctx, byte* src, long* srcOff, int* srcLen, byte* dst,
                                                                      long dstTotalCap, long* outOff, int* outLen, int nBlocks, IntPtr stream);
         [DllImport(Library, CallingConvention = CallingConvention.Cdecl)]
+        private static extern unsafe int lz4b200_decode_batch_packed_to_device(IntPtr ctx, byte* src, long* srcOff, int* srcLen, IntPtr dst,
+                                                                               long dstTotalCap, long* outOff, int* outLen, int nBlocks, IntPtr stream);
+        [DllImport(Library, CallingConvention = CallingConvention.Cdecl)]
         private static extern unsafe int lz4b200_wrap_batch(IntPtr ctx, byte* src, long* srcOff, int* srcLen, int highCompression,
                                                             byte* dst, long* dstOff, int* dstCap, int* outLen, int n);
 
@@ -121,6 +124,27 @@ namespace LZ4
                 var rc = lz4b200_measure_batch(CudaContext(), src, so, sl, null, ol, n, 0, 0, IntPtr.Zero);
                 if (rc != 0) throw new InvalidOperationException("lz4b200_measure_batch failed: " + rc);
             }
+        }
+
+        /// <summary>Decodes n raw LZ4 blocks whose decoded sizes nobody stored (input[inputOffsets[i], +inputLengths[i])) back to
+        /// back into device memory of the context's GPU, in one pass over the compressed bytes.  offsets (n + 1 entries)
+        /// receives where each block lies in <paramref name="deviceOutput"/> and, last, the total, which is returned;
+        /// lengths[i] is what <see cref="Decode(byte[],int,int,byte[],int,int,bool)"/> with knownOutputLength = false would
+        /// return, or a negative value for a corrupt block, which occupies no bytes.  When the total exceeds
+        /// <paramref name="deviceCapacity"/> nothing of the output is valid (nothing is written outside it): allocate the
+        /// returned total and call again.  Ordered behind the work already queued on <paramref name="stream"/>.</summary>
+        public static unsafe long DecodeBlocksToDevice(byte[] input, long[] inputOffsets, int[] inputLengths, IntPtr deviceOutput,
+                                                       long deviceCapacity, long[] offsets, int[] lengths, IntPtr stream = default(IntPtr))
+        {
+            var n = inputOffsets.Length;
+            if (inputLengths.Length < n || lengths.Length < n || offsets.Length < n + 1) throw new ArgumentException("arrays too small");
+            fixed (byte* src = input) fixed (long* so = inputOffsets) fixed (int* sl = inputLengths) fixed (long* oo = offsets)
+            fixed (int* ol = lengths)
+            {
+                var rc = lz4b200_decode_batch_packed_to_device(CudaContext(), src, so, sl, deviceOutput, deviceCapacity, oo, ol, n, stream);
+                if (rc != 0) throw new InvalidOperationException("lz4b200_decode_batch_packed_to_device failed: " + rc);
+            }
+            return offsets[n];
         }
 
         #endregion

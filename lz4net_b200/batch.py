@@ -7,7 +7,7 @@ one block at a time, src/LZ4/LZ4Stream.cs:239-269).  Layouts:
 * encoder slots   uint8[n_blocks * slot], slot = MaximumOutputLength(block_size) (or block_size for LZ4Stream/Wrap caps)
 * packed payload  uint8[sum(len)], block i at off[i] (exclusive prefix sum, int64[n_blocks + 1])
 
-The mixed-memory helpers (encode_to_host, encode_to_host_packed, decode_from_host) take the device side as a torch CUDA
+The mixed-memory helpers (encode_to_host, encode_to_host_packed, decode_from_host, decode_from_host_packed) take the device side as a torch CUDA
 tensor and the host side -- data, offsets, lengths, results -- as numpy arrays.  They are synchronous, ordered behind the
 work already queued on the current torch stream, and move only compressed bytes over PCIe.  stream_encode_to_host and
 stream_decode_to_device do the same for the LZ4Stream format: a device tensor's bytes as a stream in host memory, and back.
@@ -146,6 +146,20 @@ def decode_from_host(ctx: Context, comp: np.ndarray, src_off, src_len, out: torc
     ctx.decode_batch_ptr(_h(comp, np.uint8), _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), _h(dst_off, np.int64, n),
                          _h(dst_cap, np.int32, n), _h(out_len, np.int32, n), n, known=known, stream=_stream(),
                          mem=native.MEM_HOST_TO_DEVICE)
+
+
+def decode_from_host_packed(ctx: Context, comp: np.ndarray, src_off, src_len, out: torch.Tensor, out_off, out_len) -> int:
+    """Compressed blocks in a host array whose decoded sizes nobody stored, decoded into a device tensor, packed
+    (lz4b200_decode_batch_packed_to_device): block i lands at out + out_off[i] (int64[n+1], out_off[n] = the total, which is
+    returned) when the total fits out.nbytes.  Otherwise nothing is written outside `out`, its bytes are unspecified, and
+    out_len holds the sizes (negative for malformed blocks): allocate the returned total and call again.  The compressed
+    bytes cross PCIe once."""
+    n = len(src_off)
+    off, res = _h(out_off, np.int64, n + 1), _h(out_len, np.int32, n)
+    native.check(native.lib().lz4b200_decode_batch_packed_to_device(
+        ctx.handle, _h(comp, np.uint8), _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), out.nbytes, off, res, n,
+        _stream()), "decode_batch_packed_to_device")
+    return int(out_off[n])
 
 
 def wrap_to_host(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, out_len, hc: bool = False):

@@ -141,6 +141,19 @@ class Context:
             outs.append(dst[int(o):int(o) + m].tobytes())
         return res, outs
 
+    def decode_blocks_to_device(self, blocks, out):
+        """Raw LZ4 blocks (bytes-like) whose decoded sizes nobody stored, decoded back to back into the bytes of a contiguous
+        CUDA tensor: one lz4b200_decode_batch_packed_to_device call, the compressed bytes cross PCIe once.  Returns
+        (out_len list, out_off list[n+1]): block i lies at out_off[i], out_off[n] is the total.  When the total exceeds the
+        tensor's size its bytes are unspecified and out_len holds the sizes: allocate out_off[n] bytes and call again.  A
+        malformed block has a negative out_len and occupies no bytes."""
+        from . import batch
+        n = len(blocks)
+        src, lens, src_off = _pack(blocks)
+        out_len, out_off = np.zeros(n, np.int32), np.zeros(n + 1, np.int64)
+        batch.decode_from_host_packed(self, src, src_off, lens, batch._flat_bytes(out), out_off, out_len)
+        return out_len.tolist(), out_off.tolist()
+
     def measure_blocks(self, blocks, caps=None, known=False):
         """What decode_blocks(blocks, caps, known) would return as out_len, without decoding: one host-memory batch call.
         caps=None (unknown size only): no limit on the decoded size (INT32_MAX per block)."""
@@ -331,10 +344,21 @@ class LZ4Codec:
             if n != want:
                 raise ValueError("outputLength is not valid")
             return bytes(out)
+        cuda = _is_tensor(output) and output.is_cuda                 # its bytes in storage order; offset and length count bytes
+        if cuda:
+            if knownOutputLength:
+                raise TypeError("a CUDA tensor output takes knownOutputLength=False")
+            output = _tensor_bytes(output)
         inputLength = cls._check(input, inputOffset, inputLength, "input")
         outputLength = cls._check(output, outputOffset, outputLength, "output")
         if inputLength == 0 or outputLength == 0:                    # CheckArguments :156-160 + `if (outputLength == 0) return 0` (Safe.cs:470)
             return 0
+        if cuda:                                                     # decoded straight into device memory
+            block = bytes(input[inputOffset:inputOffset + inputLength])
+            res, off = default_context().decode_blocks_to_device([block], output[outputOffset:outputOffset + outputLength])
+            if res[0] < 0 or off[1] > outputLength:                  # src/LZ4ps/LZ4Codec.Safe.cs:546-549
+                raise ValueError("LZ4 block is corrupted, or invalid length has been given.")
+            return res[0]
         return cls._service.Decode(input, inputOffset, inputLength, output, outputOffset, outputLength, knownOutputLength)
 
     # ---- Wrap / Unwrap (:510-599) ------------------------------------------------------------------------------

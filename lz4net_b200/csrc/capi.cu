@@ -5,7 +5,9 @@
 // into chunks, and for each chunk H2D(inputs) -> kernel -> D2H(outputs) is enqueued on one of NSLOT streams, so that the
 // copy engines (both PCIe directions) and the SMs work on different chunks at the same time.  The mixed-memory batches
 // (MEM_DEVICE_TO_HOST, MEM_HOST_TO_DEVICE and the packed encode from device memory) and the LZ4Stream and Wrap / Unwrap
-// calls between device and host memory go through it too, skipping the copy of whichever side is already on the device.
+// calls between device and host memory go through it too, skipping the copy of whichever side is already on the device;
+// so does the packed unknown-size decode from host into device memory, whose output offset is carried across the stages
+// on the device (lz4_packed.cuh).
 // The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
 // caller's bytes are on; the host only reads headers (framing.cpp).  There is no CPU codec in this library: if the device
 // or the kernel image is unusable every entry point reports an error.
@@ -105,6 +107,7 @@ bool is_pageable(const void* p)
 struct Slot {
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
+    cudaEvent_t carried = nullptr;         // the packed decode into device memory: the stage's placement step is enqueued
     DevBuf src, dst, meta, packed, offs, scan;
     PinBuf hmeta, hsrc, hout;              // pinned: chunk metadata, staged pageable sources, staged outputs
 };
@@ -114,7 +117,8 @@ struct Slot {
 // int64 packed_off[m+1].  aux is used by the LZ4Stream and Unwrap calls only: the frame sizes of an encode (written on the
 // device), the stored payload lengths of a decode (copied up with the first four arrays).  A Wrap encode from device
 // memory keeps the codec's view of its packets (WrapScratch: int64 off[m] | int32 len[m] | int32 cap[m] | int32 res[m])
-// in the device block behind out, at WRAP_META_OFFSET * m bytes: the slots are in flight at once, so it is theirs.
+// in the device block behind out, at WRAP_META_OFFSET * m bytes: the slots are in flight at once, so it is theirs.  The
+// packed decode into device memory keeps its stage's "fits" flag (an int) in the same place, for the same reason.
 struct Meta {
     int64_t *so, *dof; int32_t *sl, *dc, *aux, *out; int64_t* off;
     Meta(void* p, int32_t m) : so((int64_t*)p), dof(so + m), sl((int32_t*)(dof + m)), dc(sl + m), aux(dc + m), out(aux + m),
@@ -145,6 +149,7 @@ struct lz4b200_ctx {
     cudaEvent_t hc_done = nullptr;         // the HC state arena is shared: HC launches are chained through this event
     cudaEvent_t compact_done = nullptr;    // likewise the scan scratch of lz4b200_compact
     cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
+    int64_t* carry = nullptr;              // the packed decode into device memory: NSLOT cells, the running output offset behind each slot's stage
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
     bool decode_lanes_auto = true;         // host-memory batches: chosen per chunk from the compression ratio
     int encode_ctas_per_sm = 0;            // encoder warps (= blocks in flight) per SM: 0 = as many as shared memory holds tables for (14)
@@ -234,12 +239,19 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
 // frames (the LZ4Stream and Wrap / Unwrap calls, see Framing): an APPEND LZ4Stream encode lands the chunks' frames instead
 // of the compacted blocks (out_off[i] = where frame i starts); a Wrap encode lands whole packets in any mode; a decode
 // also copies the stored chunks' or packets' payloads.
+// The packed decode into device memory (dst_dev, op 3, dst_off == nullptr, out_off set; lz4_packed.cuh): nobody stored the
+// decoded sizes, so a stage measures its blocks, scans the sizes and places its blocks behind the earlier stages' -- the
+// running total is carried from stage to stage in the context's `carry` cells, the slot's is the one its stage leaves --
+// then decodes them in place behind the stage's "fits" flag.  Only the placement steps are chained (the slot's `carried`
+// event, waited on by the next stage's stream); everything else of neighbouring stages overlaps as in any other call.
+// out_off[i] receives block i's offset, out_off[n] the total, whether it fits dst_total_cap or not.
 int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
              const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op,
              int64_t* out_off, int64_t dst_total_cap, bool src_dev = false, bool dst_dev = false, cudaStream_t caller = nullptr,
              const Framing* frames = nullptr)
 {
     const bool measure = op >= 4, wrap = frames && frames->wrap, stored_copy = frames && frames->stored;
+    const bool carry = dst_dev && !dst_off;
     for (int32_t i = 0; i < n; i++)
         if (src_len[i] < 0 || (dst_cap && dst_cap[i] < 0)) return fail(LZ4B200_E_ARG, "negative block length");
     const bool src_pageable = !src_dev && is_pageable(src), dst_pageable = !measure && !dst_dev && is_pageable(dst);
@@ -311,6 +323,10 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
                 par_memcpy(dst + written, staged, (size_t)total);
             }
         }
+        if (carry) {
+            std::memcpy(out_off + p.b0, h.dof, sizeof(int64_t) * (size_t)m);
+            written = h.off[0];
+        }
         if (p.mode == APPEND) {
             for (int32_t i = 0; i < m; i++) out_off[p.b0 + i] = written + h.off[i];
             written += total;
@@ -331,7 +347,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         Slot& sl = c->slot[s];
         const int32_t m = b1 - b0;
         const Mode mode = measure || dst_dev ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == 2 ? RUNS : SCATTER;
-        CU(sl.meta.reserve((size_t)m * (wrap ? WRAP_META_BYTES : META_BYTES)));
+        CU(sl.meta.reserve((size_t)m * (wrap ? WRAP_META_BYTES : META_BYTES) + (carry ? sizeof(int64_t) : 0)));
         CU(sl.hmeta.reserve((size_t)m * META_BYTES + sizeof(int64_t) * (size_t)(m + 2)));
         const Meta h(sl.hmeta.p, m), d(sl.meta.p, m);
         int64_t slo = 0, shi = 0, dsum = 0;
@@ -341,7 +357,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         }
         for (int32_t i = 0; i < m; i++) {
             h.so[i] = src_off[b0 + i] - slo;
-            if (dst_dev) h.dof[i] = dst_off[b0 + i];
+            if (dst_dev) h.dof[i] = carry ? 0 : dst_off[b0 + i];
             else { h.dof[i] = dsum; dsum += measure ? 0 : dst_cap[b0 + i]; }
             h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap ? dst_cap[b0 + i] : INT32_MAX;
             if (stored_copy) {
@@ -361,7 +377,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         }
         const BatchArgs a{src_dev ? src : (const uint8_t*)sl.src.p, d.so, d.sl, dst_dev ? dst : (uint8_t*)sl.dst.p, d.dof, d.dc, d.out, m};
         int lanes = 0;
-        if ((op == 2 || op == 3) && c->decode_lanes_auto) {
+        if ((op == 2 || op == 3) && c->decode_lanes_auto && !carry) {      // (a packed stage's decoded size is known on the device only)
             double cs = 0, rs = 0;
             for (int32_t i = b0; i < b1; i++) { cs += src_len[i]; rs += dst_cap[i]; }
             lanes = lanes_for_ratio(rs > 0 ? cs / rs : 1.0, m, c->dev);
@@ -379,6 +395,24 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
             rc = run_device(c, enc, op, sl.stream, lanes, hc_large); if (rc) return rc;
             e = launch_wrap_finish(a, w, sl.stream, &c->launches);
             if (e != cudaSuccess) return cuda_fail(e, "wrap finish launch");
+        } else if (carry) {
+            // measure -> scan -> placement, behind the previous stage's -> decode behind the stage's flag
+            CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
+            const int prev = (s + NSLOT - 1) % NSLOT;
+            int* fits = (int*)d.off;
+            BatchArgs sizes = a; sizes.dst_cap = nullptr;
+            cudaError_t e = launch_measure(sizes, false, c->dev, sl.stream, &c->launches);
+            if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, d.out, nullptr, (int64_t*)sl.offs.p, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
+            if (e != cudaSuccess) return cuda_fail(e, "packed measure launch");
+            if (b0 > 0) CU(cudaStreamWaitEvent(sl.stream, c->slot[prev].carried, 0));
+            e = launch_packed_prep(d.out, (const int64_t*)sl.offs.p, m, dst_total_cap, d.dc, fits, sl.stream, &c->launches,
+                                   b0 > 0 ? c->carry + prev : nullptr, d.dof, c->carry + s);
+            if (e != cudaSuccess) return cuda_fail(e, "packed placement launch");
+            CU(cudaEventRecord(sl.carried, sl.stream));
+            e = launch_decode(a, false, c->decode_lanes_auto ? 0 : c->decode_lanes, c->counter(), c->dev, sl.stream, &c->launches, fits);
+            if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
+            CU(cudaMemcpyAsync(h.dof, d.dof, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, sl.stream));
+            CU(cudaMemcpyAsync(h.off, c->carry + s, sizeof(int64_t), cudaMemcpyDeviceToHost, sl.stream));
         } else {
             rc = run_device(c, a, op, sl.stream, lanes, hc_large); if (rc) return rc;
         }
@@ -736,12 +770,14 @@ int lz4b200_create(lz4b200_ctx** out, int device)
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device); c->dev.smem_per_sm = v;
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device); c->dev.smem_optin = v;
     cudaError_t e = cudaMalloc(&c->counters, sizeof(uint32_t) * NCOUNTER);
+    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * NSLOT);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->hc_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->compact_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->entry, cudaEventDisableTiming);
     for (int i = 0; i < NSLOT && e == cudaSuccess; i++) {
         e = cudaStreamCreateWithFlags(&c->slot[i].stream, cudaStreamNonBlocking);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->slot[i].done, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->slot[i].carried, cudaEventDisableTiming);
     }
     if (e != cudaSuccess) { int rc = cuda_fail(e, "context creation"); lz4b200_destroy(c); return rc; }
     *out = c;
@@ -757,6 +793,7 @@ void lz4b200_destroy(lz4b200_ctx* c)
         Slot& s = c->slot[i];
         s.src.release(); s.dst.release(); s.meta.release(); s.hmeta.release(); s.packed.release(); s.offs.release(); s.scan.release(); s.hsrc.release(); s.hout.release();
         if (s.done) cudaEventDestroy(s.done);
+        if (s.carried) cudaEventDestroy(s.carried);
         if (s.stream) cudaStreamDestroy(s.stream);
     }
     c->hc_arena.release(); c->compact_tmp.release(); c->packed_caps.release(); c->wrap_tmp.release();
@@ -764,6 +801,7 @@ void lz4b200_destroy(lz4b200_ctx* c)
     if (c->compact_done) cudaEventDestroy(c->compact_done);
     if (c->entry) cudaEventDestroy(c->entry);
     if (c->counters) cudaFree(c->counters);
+    if (c->carry) cudaFree(c->carry);
     delete c;
 }
 
@@ -877,6 +915,24 @@ int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
     CU(cudaEventRecord(c->compact_done, st));
     return LZ4B200_OK;
+}
+
+// The same from host memory, through the pipeline (run_host): the sizes stay on the device, a stage at a time.
+int lz4b200_decode_batch_packed_to_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                          void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
+                                          void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
+    if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
+    std::lock_guard<std::mutex> lock(c->mu);
+    DeviceGuard g(c->device);
+    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    int rc = check_side(c, src, false, "src"); if (rc) return rc;
+    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
+    return run_host(c, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, nullptr, nullptr, out_len, n, 3, out_off, dst_total_cap,
+                    false, true, (cudaStream_t)stream);
 }
 
 int lz4b200_compact(lz4b200_ctx* c, const void* slots, const int64_t* slot_off, const int32_t* len, void* packed,

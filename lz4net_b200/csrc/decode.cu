@@ -3,6 +3,7 @@
 #include "lz4_decode.cuh"
 #include "lz4_decode_lpb.cuh"
 #include "lz4_measure.cuh"
+#include "lz4_packed.cuh"
 
 namespace lz4b200 {
 
@@ -236,21 +237,23 @@ cudaError_t launch_measure(const BatchArgs& a, bool known_len, const DeviceInfo&
     return cudaGetLastError();
 }
 
-// Between the scan and the decode of lz4b200_decode_batch_packed: block i's capacity is its measured size (0 for a
-// malformed block: the decoder rejects it without writing a byte), and *fits = whether the total fits the destination.
+// Between the scan and the decode of the packed decodes (lz4_packed.cuh): capacities, the "fits" gate and, for a stage of
+// the host pipeline, the blocks' absolute offsets behind the running total of the earlier stages.  base_in and total_out
+// are different cells: every thread reads the one, thread 0 writes the other.
 __global__ void __launch_bounds__(256) lz4_packed_prep_kernel(const int32_t* size, const int64_t* out_off, int32_t n,
-                                                              int64_t total_cap, int32_t* cap, int* fits)
+                                                              int64_t total_cap, int32_t* cap, int* fits,
+                                                              const int64_t* base_in, int64_t* abs_off, int64_t* total_out)
 {
-    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    if (i < n) cap[i] = size[i] > 0 ? size[i] : 0;
-    if (i == 0) *fits = out_off[n] <= total_cap;
+    packed_place((int64_t)blockIdx.x * 256 + threadIdx.x, size, out_off, n, base_in ? *base_in : 0, total_cap, cap, abs_off, fits,
+                 total_out);
 }
 
 cudaError_t launch_packed_prep(const int32_t* size, const int64_t* out_off, int32_t n, int64_t total_cap, int32_t* cap, int* fits,
-                               cudaStream_t stream, int64_t* launches)
+                               cudaStream_t stream, int64_t* launches, const int64_t* base_in, int64_t* abs_off, int64_t* total_out)
 {
     if (n <= 0) return cudaSuccess;
-    lz4_packed_prep_kernel<<<(unsigned)(((int64_t)n + 255) / 256), 256, 0, stream>>>(size, out_off, n, total_cap, cap, fits);
+    lz4_packed_prep_kernel<<<(unsigned)(((int64_t)n + 255) / 256), 256, 0, stream>>>(size, out_off, n, total_cap, cap, fits,
+                                                                                     base_in, abs_off, total_out);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

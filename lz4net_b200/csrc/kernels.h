@@ -24,9 +24,12 @@ cudaError_t launch_decode(const BatchArgs& a, bool known_len, int lanes_per_bloc
 // out_len[i] = what launch_decode would store for block i, nothing else is written (a.dst / a.dst_off unused; a.dst_cap
 // may be null when !known_len: INT32_MAX for every block).
 cudaError_t launch_measure(const BatchArgs& a, bool known_len, const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
-// cap[i] = max(size[i], 0); *fits = out_off[n] <= total_cap
+// cap[i] = max(size[i], 0); *fits = out_off[n] <= total_cap.  A stage of the host pipeline (lz4_packed.cuh) also passes
+// base_in (the running total of the earlier stages; null = 0), abs_off (abs_off[i] = base + out_off[i]) and total_out
+// (receives base + out_off[n]; a cell other than base_in); *fits is then base + out_off[n] <= total_cap.
 cudaError_t launch_packed_prep(const int32_t* size, const int64_t* out_off, int32_t n, int64_t total_cap, int32_t* cap, int* fits,
-                               cudaStream_t stream, int64_t* launches);
+                               cudaStream_t stream, int64_t* launches, const int64_t* base_in = nullptr,
+                               int64_t* abs_off = nullptr, int64_t* total_out = nullptr);
 cudaError_t launch_encode_fast(const BatchArgs& a, uint32_t* counter, int warps_per_sm, const int* tune4 /* prefetch, lane_copy_max, probe_max, wide_min */, int variant,
                                const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 size_t      hc_scratch_bytes(int concurrency);

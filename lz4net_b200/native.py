@@ -32,6 +32,7 @@ SIGNATURES = {
     "lz4b200_compact": (_I, [_P, _P, _P, _P, _P, _P, C.c_int32, _P]),
     "lz4b200_measure_batch": (_I, [_P, _P, _P, _P, _P, _P, C.c_int32, _I, _I, _P]),
     "lz4b200_decode_batch_packed": (_I, [_P, _P, _P, _P, _P, _L, _P, _P, C.c_int32, _P]),
+    "lz4b200_decode_batch_packed_to_device": (_I, [_P, _P, _P, _P, _P, _L, _P, _P, C.c_int32, _P]),
     "lz4b200_compress_limitedOutput": (_I, [_P, _P, _I, _I]),
     "lz4b200_compressHC_limitedOutput": (_I, [_P, _P, _I, _I]),
     "lz4b200_uncompress": (_I, [_P, _P, _I, _I]),
