@@ -7,7 +7,7 @@
 // (MEM_DEVICE_TO_HOST, MEM_HOST_TO_DEVICE and the packed encode from device memory) and the LZ4Stream and Wrap / Unwrap
 // calls between device and host memory go through it too, skipping the copy of whichever side is already on the device;
 // so does the packed unknown-size decode from host into device memory, whose output offset is carried across the stages
-// on the device (lz4_packed.cuh).
+// on the device (lz4_packed.cuh).  What a stage runs is named by its caller (Stage); the codec operation by Op.
 // The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
 // caller's bytes are on; the host only reads headers (framing.cpp).  There is no CPU codec in this library: if the device
 // or the kernel image is unusable every entry point reports an error.
@@ -46,33 +46,28 @@ constexpr int NSLOT = 3;                       // pipeline depth of host-memory 
 constexpr int NCOUNTER = 256;
 constexpr size_t HOST_CHUNK_BYTES_DEFAULT = 128u << 20; // src + dst bytes per pipeline stage (on H100 the best of 32..512 MiB: profiles/README.md)
 
-struct DevBuf {
+// Grow-only buffers that free themselves (the context's device is current when a context is destroyed): device memory,
+// grown with an eighth to spare, or page-locked host memory.
+template <bool PINNED>
+struct Buf {
     void* p = nullptr; size_t cap = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    ~Buf() { release(); }
     cudaError_t reserve(size_t n)
     {
         if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
-        size_t want = n + (n >> 3) + 4096;
-        cudaError_t e = cudaMalloc(&p, want);
+        release();
+        const size_t want = PINNED ? n + 4096 : n + (n >> 3) + 4096;
+        cudaError_t e = PINNED ? cudaMallocHost(&p, want) : cudaMalloc(&p, want);
         if (e == cudaSuccess) cap = want;
         return e;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    void release() { if (p) (PINNED ? cudaFreeHost(p) : cudaFree(p)); p = nullptr; cap = 0; }
 };
-struct PinBuf {
-    void* p = nullptr; size_t cap = 0;
-    cudaError_t reserve(size_t n)
-    {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFreeHost(p);
-        p = nullptr; cap = 0;
-        cudaError_t e = cudaMallocHost(&p, n + 4096);
-        if (e == cudaSuccess) cap = n + 4096;
-        return e;
-    }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
-};
+using DevBuf = Buf<false>;
+using PinBuf = Buf<true>;
 
 // Pageable host memory (a managed caller's `fixed` byte[]): cudaMemcpyAsync from / to it is staged by the driver through
 // its own small pinned buffers, synchronously (several times slower than from pinned memory).  The library
@@ -115,26 +110,43 @@ struct Slot {
 // One chunk's metadata, laid out the same in the slot's hmeta (host) and meta (device, which has no packed_off):
 // int64 src_off[m] | int64 dst_off[m] | int32 src_len[m] | int32 dst_cap[m] | int32 aux[m] | int32 out_len[m] |
 // int64 packed_off[m+1].  aux is used by the LZ4Stream and Unwrap calls only: the frame sizes of an encode (written on the
-// device), the stored payload lengths of a decode (copied up with the first four arrays).  A Wrap encode from device
-// memory keeps the codec's view of its packets (WrapScratch: int64 off[m] | int32 len[m] | int32 cap[m] | int32 res[m])
-// in the device block behind out, at WRAP_META_OFFSET * m bytes: the slots are in flight at once, so it is theirs.  The
-// packed decode into device memory keeps its stage's "fits" flag (an int) in the same place, for the same reason.
+// device), the stored payload lengths of a decode (copied up with the first four arrays).  A Wrap encode keeps the codec's
+// view of its packets (WrapScratch) in the device block behind out, at WRAP_META_OFFSET * m bytes: the slots are in flight
+// at once, so it is theirs.  The packed decode into device memory keeps its stage's "fits" flag (an int) in the same
+// place, for the same reason.
 struct Meta {
     int64_t *so, *dof; int32_t *sl, *dc, *aux, *out; int64_t* off;
     Meta(void* p, int32_t m) : so((int64_t*)p), dof(so + m), sl((int32_t*)(dof + m)), dc(sl + m), aux(dc + m), out(aux + m),
                                off((int64_t*)(((uintptr_t)(out + m) + 7) & ~(uintptr_t)7)) {}
 };
-constexpr size_t META_BYTES = 32, WRAP_META_OFFSET = 32, WRAP_META_BYTES = WRAP_META_OFFSET + 20;
+// The codec's view of n packets (int64 off[n] | int32 len[n] | int32 cap[n] | int32 res[n]) at p.
+constexpr size_t WRAP_SCRATCH_BYTES = sizeof(int64_t) + 3 * sizeof(int32_t);
+WrapScratch wrap_scratch_at(void* p, int32_t n)
+{
+    int32_t* len = (int32_t*)((int64_t*)p + n);
+    return WrapScratch{(int64_t*)p, len, len + n, len + 2 * n};
+}
+constexpr size_t META_BYTES = 32, WRAP_META_OFFSET = 32, WRAP_META_BYTES = WRAP_META_OFFSET + WRAP_SCRATCH_BYTES;
 
-// The framing calls inside the pipeline.
-//  LZ4Stream encode (APPEND, lz4_stream.cuh): the frames of the chunks replace the compaction, hc = the flags' HC bit.
-//  Wrap encode (wrap, lz4_wrap.cuh): dst_cap[i] = the packet's capacity, src_len[i] + 8.  The encoder writes each payload
-//    behind its header's place in the slot; the finish step writes the headers and the stored inputs and sets out_len to
-//    the packet sizes.  The slot then holds whole packets, which land like the blocks of an encode.
-//  Decode (LZ4Stream chunks, Unwrap packets; dst in host or device memory): stored[i] != 0 marks a stored chunk or packet,
-//    whose payload is copied by the stored-copy step while the decoder gets the neutral entry (src_len 0, dst_cap 0).  In
-//    host memory it lands like a decoded block of dst_cap[i] bytes.
-struct Framing { bool hc; const uint8_t* stored; bool wrap; };
+// The operations of the batch codec.
+enum class Op { ENCODE_FAST, ENCODE_HC, DECODE_KNOWN, DECODE_UNKNOWN, MEASURE_KNOWN, MEASURE_UNKNOWN };
+constexpr Op encode_op(bool hc) { return hc ? Op::ENCODE_HC : Op::ENCODE_FAST; }
+constexpr bool is_encode(Op op) { return op == Op::ENCODE_FAST || op == Op::ENCODE_HC; }
+constexpr bool is_decode(Op op) { return op == Op::DECODE_KNOWN || op == Op::DECODE_UNKNOWN; }
+constexpr bool is_measure(Op op) { return op == Op::MEASURE_KNOWN || op == Op::MEASURE_UNKNOWN; }
+
+// What a stage of the host pipeline (run_host) runs on its chunk.
+enum class Stage {
+    CODEC,            // the operation (run_device)
+    STREAM_ENCODE,    // the encode, then the chunks' LZ4Stream frames (lz4_stream.cuh) in place of the compaction: APPEND
+                      // lands the frames, out_off[i] = where frame i starts
+    WRAP_ENCODE,      // prep -> the encode -> finish (run_wrap, lz4_wrap.cuh): dst_cap[i] = the packet's capacity,
+                      // src_len[i] + 8; the slot then holds whole packets, which land like the blocks of an encode
+    FRAMED_DECODE,    // the known-size decode of LZ4Stream chunks or Unwrap packets: stored[i] != 0 marks a stored one, whose
+                      // payload the stored-copy step copies while the decoder gets the neutral entry (src_len 0, dst_cap 0);
+                      // in host memory it lands like a decoded block of dst_cap[i] bytes
+    PLACED_DECODE,    // the packed unknown-size decode into device memory, its output offset carried across the stages
+};
 
 }  // namespace
 
@@ -147,7 +159,7 @@ struct lz4b200_ctx {
     DevBuf packed_caps;                    // lz4b200_decode_batch_packed: per-block capacities + the "fits" flag (serialised like compact_tmp)
     DevBuf wrap_tmp;                       // the device Wrap / Unwrap calls: the codec's view of the packets (serialised like compact_tmp)
     cudaEvent_t hc_done = nullptr;         // the HC state arena is shared: HC launches are chained through this event
-    cudaEvent_t compact_done = nullptr;    // likewise the scan scratch of lz4b200_compact
+    cudaEvent_t compact_done = nullptr;    // likewise compact_tmp, packed_caps and wrap_tmp (call_scratch)
     cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
     int64_t* carry = nullptr;              // the packed decode into device memory: NSLOT cells, the running output offset behind each slot's stage
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
@@ -164,6 +176,7 @@ struct lz4b200_ctx {
     std::mutex mu;
 
     uint32_t* counter() { uint32_t* c = counters + next_counter; next_counter = (next_counter + 4) % NCOUNTER; return c; }   // fours: [block counter, decoder pick, two more counters]
+    int pinned_lanes() const { return decode_lanes_auto ? 0 : decode_lanes; }   // 0: the decoder is picked on the device
 };
 
 namespace {
@@ -173,6 +186,31 @@ struct DeviceGuard {
     explicit DeviceGuard(int dev) { ok = cudaGetDevice(&prev) == cudaSuccess && cudaSetDevice(dev) == cudaSuccess; }
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
+
+// The context's lock and its device for the rest of a call; rc = LZ4B200_E_CUDA when the device could not be made current.
+struct CallGuard {
+    std::lock_guard<std::mutex> lock;
+    DeviceGuard dev;
+    int rc;
+    explicit CallGuard(lz4b200_ctx* c)
+        : lock(c->mu), dev(c->device), rc(dev.ok ? LZ4B200_OK : fail(LZ4B200_E_CUDA, "cudaSetDevice failed")) {}
+};
+
+// The context's call scratch (compact_tmp, packed_caps, wrap_tmp) is shared by the device calls on every stream.  A call
+// grows the buffers it needs to at least these sizes -- behind one cudaDeviceSynchronize, since an earlier call may still
+// be using them -- and orders `st` behind the last call that used them.  The caller records compact_done on `st` once its
+// launches are in.
+int call_scratch(lz4b200_ctx* c, cudaStream_t st, size_t compact_bytes, size_t caps_bytes = 0, size_t wrap_bytes = 0)
+{
+    if (compact_bytes > c->compact_tmp.cap || caps_bytes > c->packed_caps.cap || wrap_bytes > c->wrap_tmp.cap) {
+        CU(cudaDeviceSynchronize());
+        CU(c->compact_tmp.reserve(compact_bytes)); CU(c->packed_caps.reserve(caps_bytes)); CU(c->wrap_tmp.reserve(wrap_bytes));
+    }
+    CU(cudaStreamWaitEvent(st, c->compact_done, 0));
+    return LZ4B200_OK;
+}
+
+int launched(cudaError_t e, const char* what) { return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, what); }
 
 // Decode group size from the ratio compressed/raw of a batch (tools/sweep.py): incompressible data is long literal runs
 // (whole warps, 128-bit copies), nearly-empty streams are long matches, everything between is sequence-dense (the
@@ -186,14 +224,13 @@ int lanes_for_ratio(double ratio, int64_t n_blocks, const DeviceInfo& dev)
 }
 
 // hc_large: blocks above 64 KiB in an HC batch (-1 = not known: a device-memory batch)
-int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc, 2 dec known, 3 dec unknown, 4 / 5 measure known / unknown*/,
-               cudaStream_t st, int lanes = 0, int32_t hc_large = -1)
+int run_device(lz4b200_ctx* c, const BatchArgs& a, Op op, cudaStream_t st, int lanes = 0, int32_t hc_large = -1)
 {
-    if (!lanes && !c->decode_lanes_auto) lanes = c->decode_lanes;       // (0 = auto: the decoder is picked on the device)
+    if (!lanes) lanes = c->pinned_lanes();
     cudaError_t e = cudaSuccess;
     switch (op) {
-    case 0: e = launch_encode_fast(a, c->counter(), c->encode_ctas_per_sm, c->encode_tune, c->encode_variant, c->dev, st, &c->launches); break;
-    case 1: {
+    case Op::ENCODE_FAST: e = launch_encode_fast(a, c->counter(), c->encode_ctas_per_sm, c->encode_tune, c->encode_variant, c->dev, st, &c->launches); break;
+    case Op::ENCODE_HC: {
         const int conc = (int)std::min<int64_t>(c->hc_concurrency, std::max(a.n_blocks, 1));
         const size_t need = c->hc_kernel < 0 ? hc_auto_scratch_bytes(a.n_blocks, hc_large, c->dev)
                           : (c->hc_kernel ? hcw_scratch_bytes(a.n_blocks, hc_large, c->hc_kernel, c->hc_warps_per_sm, c->dev) : hc_scratch_bytes(conc));
@@ -209,19 +246,30 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
         if (e == cudaSuccess) e = cudaEventRecord(c->hc_done, st);
         break;
     }
-    case 2: e = launch_decode(a, true, lanes, c->counter(), c->dev, st, &c->launches); break;
-    case 3: e = launch_decode(a, false, lanes, c->counter(), c->dev, st, &c->launches); break;
-    default: e = launch_measure(a, op == 4, c->dev, st, &c->launches); break;
+    case Op::DECODE_KNOWN:
+    case Op::DECODE_UNKNOWN: e = launch_decode(a, op == Op::DECODE_KNOWN, lanes, c->counter(), c->dev, st, &c->launches); break;
+    case Op::MEASURE_KNOWN:
+    case Op::MEASURE_UNKNOWN: e = launch_measure(a, op == Op::MEASURE_KNOWN, c->dev, st, &c->launches); break;
     }
-    if (e != cudaSuccess) return cuda_fail(e, "kernel launch");
-    return LZ4B200_OK;
+    return launched(e, "kernel launch");
+}
+
+// A Wrap of the batch a into whole packets: prep (each payload behind its header's place, capacity = its input length,
+// LZ4Codec.cs:518-523) -> the batch codec, unchanged, on the codec's view w -> finish (the headers, the stored inputs,
+// out_len = the packet sizes).
+int run_wrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, Op op, cudaStream_t st, int32_t hc_large)
+{
+    int rc = launched(launch_wrap_prep(a, w, st, &c->launches), "wrap prep launch"); if (rc) return rc;
+    const BatchArgs enc{a.src, a.src_off, w.len, a.dst, w.off, w.cap, w.res, a.n_blocks};
+    rc = run_device(c, enc, op, st, 0, hc_large); if (rc) return rc;
+    return launched(launch_wrap_finish(a, w, st, &c->launches), "wrap finish launch");
 }
 
 // Host-memory batch: chunks of at most host_chunk_bytes (src + dst bytes) go through the slots in turn, and a slot's
 // outputs land in the caller's memory when the slot comes round again, so chunks overlap and land in block order.  On the
 // device the output slots of a chunk are dense: block i starts at the sum of dst_cap over the earlier blocks of its
-// chunk, so slots adjacent in dst are adjacent there too.  The measure pass (op 4 / 5) has no output: its chunks are
-// weighed by src_len alone, dst_cap may be null (INT32_MAX per block), and only out_len comes back (NONE).
+// chunk, so slots adjacent in dst are adjacent there too.  The measure pass has no output: its chunks are weighed by
+// src_len alone, dst_cap may be null (INT32_MAX per block), and only out_len comes back (NONE).
 // Only bytes a block PRODUCED ever reach the caller's buffer (the reference's safe codec leaves everything behind the
 // return value untouched, its native ones spill at most 7 bytes).  A chunk's outputs land in one of four ways:
 //  PER_BLOCK  chunks of at most 8 blocks: one copy per block to dst + dst_off[i];
@@ -229,29 +277,26 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, int op /*0 enc fast, 1 enc hc
 //             adjacent in dst, straight into dst when it is page-locked, else through the slot's pinned buffer;
 //  SCATTER    encoders and the unknown-size decoder: compacted on the device, one copy of exactly the produced bytes
 //             into the slot's pinned buffer, scattered to dst + dst_off[i] from there;
-//  APPEND     the packed encode (dst_off == nullptr): compacted likewise and appended at dst + written (straight into dst
-//             when it is page-locked); out_off[i] receives block i's offset there, out_off[n] the total.
+//  APPEND     the packed forms (dst_off == nullptr): compacted likewise, or framed (STREAM_ENCODE), and appended at
+//             dst + written (straight into dst when it is page-locked); out_off[i] receives block i's offset there,
+//             out_off[n] the total.
 // Mixed memory: src_dev = the source is already device memory (the kernels read the caller's buffer at the caller's
 // offsets; nothing is staged), dst_dev = the destination is device memory (the kernels write the caller's slots in place;
 // nothing is compacted or landed, only out_len comes back: NONE).  A chunk is weighed by what it stages, so the slots'
 // device buffers stay within host_chunk_bytes whatever the batch.  The slots start behind everything enqueued on
 // `caller` before the call: a producer of src, or a reader of dst's old contents.
-// frames (the LZ4Stream and Wrap / Unwrap calls, see Framing): an APPEND LZ4Stream encode lands the chunks' frames instead
-// of the compacted blocks (out_off[i] = where frame i starts); a Wrap encode lands whole packets in any mode; a decode
-// also copies the stored chunks' or packets' payloads.
-// The packed decode into device memory (dst_dev, op 3, dst_off == nullptr, out_off set; lz4_packed.cuh): nobody stored the
-// decoded sizes, so a stage measures its blocks, scans the sizes and places its blocks behind the earlier stages' -- the
-// running total is carried from stage to stage in the context's `carry` cells, the slot's is the one its stage leaves --
-// then decodes them in place behind the stage's "fits" flag.  Only the placement steps are chained (the slot's `carried`
-// event, waited on by the next stage's stream); everything else of neighbouring stages overlaps as in any other call.
-// out_off[i] receives block i's offset, out_off[n] the total, whether it fits dst_total_cap or not.
-int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
-             const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op,
-             int64_t* out_off, int64_t dst_total_cap, bool src_dev = false, bool dst_dev = false, cudaStream_t caller = nullptr,
-             const Framing* frames = nullptr)
+// PLACED_DECODE (dst_dev, dst_off == nullptr, out_off set; lz4_packed.cuh): nobody stored the decoded sizes, so a stage
+// measures its blocks, scans the sizes and places its blocks behind the earlier stages' -- the running total is carried
+// from stage to stage in the context's `carry` cells, the slot's is the one its stage leaves -- then decodes them in place
+// behind the stage's "fits" flag.  Only the placement steps are chained (the slot's `carried` event, waited on by the next
+// stage's stream); everything else of neighbouring stages overlaps as in any other call.  out_off[i] receives block i's
+// offset, out_off[n] the total, whether it fits dst_total_cap or not.
+int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
+             const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
+             int64_t dst_total_cap, bool src_dev = false, bool dst_dev = false, cudaStream_t caller = nullptr,
+             const uint8_t* stored = nullptr)
 {
-    const bool measure = op >= 4, wrap = frames && frames->wrap, stored_copy = frames && frames->stored;
-    const bool carry = dst_dev && !dst_off;
+    const bool measure = is_measure(op), framed = kind == Stage::FRAMED_DECODE, placed = kind == Stage::PLACED_DECODE;
     for (int32_t i = 0; i < n; i++)
         if (src_len[i] < 0 || (dst_cap && dst_cap[i] < 0)) return fail(LZ4B200_E_ARG, "negative block length");
     const bool src_pageable = !src_dev && is_pageable(src), dst_pageable = !measure && !dst_dev && is_pageable(dst);
@@ -294,7 +339,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
                 // a known-size decode produced dst_cap bytes when it succeeded, a stored copy (aux > 0: the decoder saw
                 // the neutral entry and failed it) always
                 const int32_t b = p.b0 + i, r = h.out[i];
-                const int64_t nbytes = op == 2 ? (r >= 0 || (stored_copy && h.aux[i] > 0) ? dst_cap[b] : 0) : std::max(r, 0);
+                const int64_t nbytes = op == Op::DECODE_KNOWN ? (r >= 0 || (framed && h.aux[i] > 0) ? dst_cap[b] : 0) : std::max(r, 0);
                 if (nbytes > 0)
                     CU(cudaMemcpyAsync(dst + dst_off[b], (uint8_t*)sl.dst.p + h.dof[i], (size_t)nbytes, cudaMemcpyDeviceToHost, sl.stream));
             }
@@ -323,7 +368,7 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
                 par_memcpy(dst + written, staged, (size_t)total);
             }
         }
-        if (carry) {
+        if (placed) {
             std::memcpy(out_off + p.b0, h.dof, sizeof(int64_t) * (size_t)m);
             written = h.off[0];
         }
@@ -346,8 +391,8 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         int rc = retire(s); if (rc) return rc;
         Slot& sl = c->slot[s];
         const int32_t m = b1 - b0;
-        const Mode mode = measure || dst_dev ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == 2 ? RUNS : SCATTER;
-        CU(sl.meta.reserve((size_t)m * (wrap ? WRAP_META_BYTES : META_BYTES) + (carry ? sizeof(int64_t) : 0)));
+        const Mode mode = measure || dst_dev ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == Op::DECODE_KNOWN ? RUNS : SCATTER;
+        CU(sl.meta.reserve((size_t)m * (kind == Stage::WRAP_ENCODE ? WRAP_META_BYTES : META_BYTES) + (placed ? sizeof(int64_t) : 0)));
         CU(sl.hmeta.reserve((size_t)m * META_BYTES + sizeof(int64_t) * (size_t)(m + 2)));
         const Meta h(sl.hmeta.p, m), d(sl.meta.p, m);
         int64_t slo = 0, shi = 0, dsum = 0;
@@ -357,19 +402,21 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         }
         for (int32_t i = 0; i < m; i++) {
             h.so[i] = src_off[b0 + i] - slo;
-            if (dst_dev) h.dof[i] = carry ? 0 : dst_off[b0 + i];
+            if (dst_dev) h.dof[i] = placed ? 0 : dst_off[b0 + i];
             else { h.dof[i] = dsum; dsum += measure ? 0 : dst_cap[b0 + i]; }
             h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap ? dst_cap[b0 + i] : INT32_MAX;
-            if (stored_copy) {
-                const bool stored = frames->stored[b0 + i] != 0;
-                h.aux[i] = stored ? h.sl[i] : 0;
-                if (stored) h.sl[i] = h.dc[i] = 0;
+            if (framed) {
+                const bool st = stored[b0 + i] != 0;
+                h.aux[i] = st ? h.sl[i] : 0;
+                if (st) h.sl[i] = h.dc[i] = 0;
             }
         }
         const size_t sbytes = (size_t)(shi - slo);
         if (!src_dev) CU(sl.src.reserve(sbytes + 64));
         if (!dst_dev) CU(sl.dst.reserve((size_t)dsum + 64));
-        CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, (size_t)m * (stored_copy ? 28 : 24), cudaMemcpyHostToDevice, sl.stream));
+        // up: the four arrays the kernels read, and a framed decode's stored lengths
+        const size_t up = (size_t)((uint8_t*)(framed ? h.out : h.aux) - (uint8_t*)h.so);
+        CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, up, cudaMemcpyHostToDevice, sl.stream));
         if (sbytes) {
             const uint8_t* from = src + slo;
             if (src_pageable && m > 8) { CU(sl.hsrc.reserve(sbytes)); par_memcpy(sl.hsrc.p, from, sbytes); from = (const uint8_t*)sl.hsrc.p; }
@@ -377,25 +424,26 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
         }
         const BatchArgs a{src_dev ? src : (const uint8_t*)sl.src.p, d.so, d.sl, dst_dev ? dst : (uint8_t*)sl.dst.p, d.dof, d.dc, d.out, m};
         int lanes = 0;
-        if ((op == 2 || op == 3) && c->decode_lanes_auto && !carry) {      // (a packed stage's decoded size is known on the device only)
+        if (is_decode(op) && c->decode_lanes_auto && !placed) {      // (a placed stage's decoded size is known on the device only)
             double cs = 0, rs = 0;
             for (int32_t i = b0; i < b1; i++) { cs += src_len[i]; rs += dst_cap[i]; }
             lanes = lanes_for_ratio(rs > 0 ? cs / rs : 1.0, m, c->dev);
         }
         int32_t hc_large = 0;
-        if (op == 1) for (int32_t i = b0; i < b1; i++) hc_large += src_len[i] > 65536;
-        if (wrap) {
-            // prep (payload at dof + 8, capacity = the input length) -> encode -> finish: whole packets in the slot
-            WrapScratch w;
-            w.off = (int64_t*)((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m);
-            w.len = (int32_t*)(w.off + m); w.cap = w.len + m; w.res = w.cap + m;
-            cudaError_t e = launch_wrap_prep(a, w, sl.stream, &c->launches);
-            if (e != cudaSuccess) return cuda_fail(e, "wrap prep launch");
-            const BatchArgs enc{a.src, a.src_off, w.len, a.dst, w.off, w.cap, w.res, m};
-            rc = run_device(c, enc, op, sl.stream, lanes, hc_large); if (rc) return rc;
-            e = launch_wrap_finish(a, w, sl.stream, &c->launches);
-            if (e != cudaSuccess) return cuda_fail(e, "wrap finish launch");
-        } else if (carry) {
+        if (op == Op::ENCODE_HC) for (int32_t i = b0; i < b1; i++) hc_large += src_len[i] > 65536;
+        switch (kind) {
+        case Stage::CODEC:
+        case Stage::STREAM_ENCODE:
+            rc = run_device(c, a, op, sl.stream, lanes, hc_large);
+            break;
+        case Stage::WRAP_ENCODE:
+            rc = run_wrap(c, a, wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), op, sl.stream, hc_large);
+            break;
+        case Stage::FRAMED_DECODE:
+            rc = run_device(c, a, op, sl.stream, lanes);
+            if (!rc) rc = launched(launch_stream_stored(a, d.aux, sl.stream, &c->launches), "stored copy launch");
+            break;
+        case Stage::PLACED_DECODE: {
             // measure -> scan -> placement, behind the previous stage's -> decode behind the stage's flag
             CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
             const int prev = (s + NSLOT - 1) % NSLOT;
@@ -409,32 +457,31 @@ int run_host(lz4b200_ctx* c, const uint8_t* src, const int64_t* src_off, const i
                                    b0 > 0 ? c->carry + prev : nullptr, d.dof, c->carry + s);
             if (e != cudaSuccess) return cuda_fail(e, "packed placement launch");
             CU(cudaEventRecord(sl.carried, sl.stream));
-            e = launch_decode(a, false, c->decode_lanes_auto ? 0 : c->decode_lanes, c->counter(), c->dev, sl.stream, &c->launches, fits);
+            e = launch_decode(a, false, c->pinned_lanes(), c->counter(), c->dev, sl.stream, &c->launches, fits);
             if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
             CU(cudaMemcpyAsync(h.dof, d.dof, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, sl.stream));
             CU(cudaMemcpyAsync(h.off, c->carry + s, sizeof(int64_t), cudaMemcpyDeviceToHost, sl.stream));
-        } else {
-            rc = run_device(c, a, op, sl.stream, lanes, hc_large); if (rc) return rc;
+            break;
         }
-        if (stored_copy) {
-            cudaError_t e = launch_stream_stored(a, d.aux, sl.stream, &c->launches);
-            if (e != cudaSuccess) return cuda_fail(e, "stored copy launch");
         }
-        if (mode >= SCATTER && frames && !wrap) {
-            // the frames of the chunks, back to back: sizes -> scan -> headers + payloads
-            CU(sl.packed.reserve((size_t)dsum + (size_t)m * STREAM_HEADER_MAX + 64)); CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1)));
-            CU(sl.scan.reserve(compact_tmp_bytes(m)));
-            cudaError_t e = launch_stream_frame_size(a, d.aux, sl.stream, &c->launches);
-            if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, d.aux, nullptr, (int64_t*)sl.offs.p, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
-            if (e == cudaSuccess) e = launch_stream_frame(a, frames->hc, (uint8_t*)sl.packed.p, (const int64_t*)sl.offs.p, sl.stream, &c->launches);
-            if (e != cudaSuccess) return cuda_fail(e, "stream frame launch");
-            CU(cudaMemcpyAsync(h.off, sl.offs.p, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDeviceToHost, sl.stream));
-        } else if (mode >= SCATTER) {
-            CU(sl.packed.reserve((size_t)dsum + 64)); CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
-            cudaError_t e = launch_compact(a.dst, a.dst_off, a.out_len, (uint8_t*)sl.packed.p, (int64_t*)sl.offs.p, m,
-                                           sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
-            if (e != cudaSuccess) return cuda_fail(e, "compact launch");
-            CU(cudaMemcpyAsync(h.off, sl.offs.p, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDeviceToHost, sl.stream));
+        if (rc) return rc;
+        if (mode >= SCATTER) {
+            // the outputs back to back: compacted, or an LZ4Stream encode's frames (sizes -> scan -> headers + payloads)
+            const bool frames = kind == Stage::STREAM_ENCODE;
+            CU(sl.packed.reserve((size_t)dsum + (frames ? (size_t)m * STREAM_HEADER_MAX : 0) + 64));
+            CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
+            uint8_t* packed = (uint8_t*)sl.packed.p;
+            int64_t* offs = (int64_t*)sl.offs.p;
+            cudaError_t e;
+            if (frames) {
+                e = launch_stream_frame_size(a, d.aux, sl.stream, &c->launches);
+                if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, d.aux, nullptr, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
+                if (e == cudaSuccess) e = launch_stream_frame(a, op == Op::ENCODE_HC, packed, offs, sl.stream, &c->launches);
+            } else {
+                e = launch_compact(a.dst, a.dst_off, a.out_len, packed, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
+            }
+            rc = launched(e, frames ? "stream frame launch" : "compact launch"); if (rc) return rc;
+            CU(cudaMemcpyAsync(h.off, offs, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDeviceToHost, sl.stream));
         }
         CU(cudaMemcpyAsync(h.out, a.out_len, sizeof(int32_t) * (size_t)m, cudaMemcpyDeviceToHost, sl.stream));
         if (mode == RUNS) {
@@ -469,21 +516,19 @@ int check_side(const lz4b200_ctx* c, const void* p, bool device, const char* wha
 }
 
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
-// packed encode (lz4b200_encode_batch_packed, or its _from_device form with MEM_DEVICE_TO_HOST); the measure pass
-// (op 4 / 5) has no dst, dst_off or out_off.
+// packed encode (lz4b200_encode_batch_packed, or its _from_device form with MEM_DEVICE_TO_HOST); the measure pass has no
+// dst, dst_off or out_off.
 int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
-          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int op, int mem, void* stream,
+          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, Op op, int mem, void* stream,
           int64_t* out_off = nullptr, int64_t dst_total_cap = 0)
 {
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0) return fail(LZ4B200_E_ARG, "negative block count");
     if (n == 0) return LZ4B200_OK;
-    const bool measure = op >= 4;
+    const bool measure = is_measure(op);
     if (!src_off || !src_len || !out_len || !src || (!measure && (!(dst_off || out_off) || !dst_cap || !dst)))
         return fail(LZ4B200_E_ARG, "null argument");
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    CallGuard g(c); if (g.rc) return g.rc;
     if (mem == LZ4B200_MEM_DEVICE) {
         BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
         return run_device(c, a, op, (cudaStream_t)stream);
@@ -497,8 +542,8 @@ int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t
         int rc = check_side(c, src, src_dev, "src"); if (rc) return rc;
         rc = check_side(c, dst, dst_dev, "dst"); if (rc) return rc;
     }
-    return run_host(c, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, op, out_off, dst_total_cap,
-                    src_dev, dst_dev, (cudaStream_t)stream);
+    return run_host(c, Stage::CODEC, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, out_off,
+                    dst_total_cap, src_dev, dst_dev, (cudaStream_t)stream);
 }
 
 // The single-block entry points are re-entrant like the reference's (SURVEY 8b "Threading"): every calling thread gets
@@ -519,54 +564,25 @@ lz4b200_ctx* default_ctx()
     return g_thread_ctx.c;
 }
 
-int single(const char* source, char* dest, int isize, int ocap, int op)
+int single(const char* source, char* dest, int isize, int ocap, Op op)
 {
+    const int failed = is_encode(op) ? 0 : -1;     // encoders report failure (0), decoders an error (<0)
     lz4b200_ctx* c = default_ctx();
-    if (!c) return op >= 2 ? -1 : 0;               // no device: encoders report failure (0), decoders an error (<0)
-    if (!source || !dest || isize < 0 || ocap < 0) return op >= 2 ? -1 : 0;
-    int64_t so = 0, dof = 0; int32_t sl = isize, dc = ocap, out = op >= 2 ? -1 : 0;
+    if (!c || !source || !dest || isize < 0 || ocap < 0) return failed;
+    int64_t so = 0, dof = 0; int32_t sl = isize, dc = ocap, out = failed;
     // zero-length buffers still need valid pointers for the staging copies
     int rc = batch(c, source, &so, &sl, dest, &dof, &dc, &out, 1, op, LZ4B200_MEM_HOST, nullptr);
-    if (rc != LZ4B200_OK) return op >= 2 ? -1 : 0;
+    if (rc != LZ4B200_OK) return failed;
     return out;
 }
-
-// The device Wrap / Unwrap calls: the context's scratch for n packets (with `packed`, also the scan scratch and the
-// capacities + "fits" flag of the packed unwrap), grown like compact_tmp, and `st` ordered behind the previous call that
-// used it (on whatever stream).  The caller holds the lock and records compact_done on `st` when its launches are in.
-int frame_scratch(lz4b200_ctx* c, int32_t n, bool packed, cudaStream_t st, WrapScratch* w)
-{
-    const size_t nn = (size_t)n;
-    const size_t need = nn * sizeof(int64_t) + 3 * nn * sizeof(int32_t);
-    const size_t caps_bytes = sizeof(int32_t) * (nn + 1);
-    if (need > c->wrap_tmp.cap || (packed && (compact_tmp_bytes(n) > c->compact_tmp.cap || caps_bytes > c->packed_caps.cap))) {
-        CU(cudaDeviceSynchronize());               // the scratch may still be in use by an earlier call
-        CU(c->wrap_tmp.reserve(need));
-        if (packed) { CU(c->compact_tmp.reserve(compact_tmp_bytes(n))); CU(c->packed_caps.reserve(caps_bytes)); }
-    }
-    CU(cudaStreamWaitEvent(st, c->compact_done, 0));
-    w->off = (int64_t*)c->wrap_tmp.p;
-    w->len = (int32_t*)(w->off + n);
-    w->cap = w->len + n;
-    w->res = w->cap + n;
-    return LZ4B200_OK;
-}
-
-// argument checks, the lock and the device of the device Wrap / Unwrap calls (n > 0)
-#define FRAME_CALL_PROLOGUE(c, n)                                                                     \
-    if (!(c)) return fail(LZ4B200_E_ARG, "null context");                                             \
-    if ((n) < 0) return fail(LZ4B200_E_ARG, "negative packet count");                                 \
-    std::lock_guard<std::mutex> lock((c)->mu);                                                        \
-    DeviceGuard g((c)->device);                                                                       \
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
 
 // The LZ4Stream calls run the pipeline over at most this many chunks at a time: it bounds the host metadata by chunk
 // count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.
 constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
 
 // The LZ4Stream of n bytes in host or device memory (src_dev), written into host memory: each run of chunks is encoded
-// (capacity = the chunk's length, LZ4Stream.cs:243-246) and its frames land back to back (Framing, APPEND).  Returns the
-// stream's size.  Only a chunk whose frame does not fit an int32 is refused for its size.
+// (capacity = the chunk's length, LZ4Stream.cs:243-246) and its frames land back to back (STREAM_ENCODE, APPEND).  Returns
+// the stream's size.  Only a chunk whose frame does not fit an int32 is refused for its size.
 int64_t stream_encode(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_size, int high_compression, void* dst,
                       int64_t dst_cap, bool src_dev, void* stream)
 {
@@ -574,15 +590,12 @@ int64_t stream_encode(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_
     if (std::min<int64_t>(block_size, n) > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "a chunk's frame must fit an int32");
     if (dst_cap < lz4b200_stream_bound(n, block_size)) return fail(LZ4B200_E_ARG, "dst_cap < lz4b200_stream_bound(n, block_size)");
     if (n == 0) return 0;
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    CallGuard g(c); if (g.rc) return g.rc;
     if (src_dev) {
         int rc = check_side(c, src, true, "src"); if (rc) return rc;
         rc = check_side(c, dst, false, "dst"); if (rc) return rc;
     }
     const int64_t chunks = (n + block_size - 1) / block_size;
-    const Framing f{high_compression != 0, nullptr, false};
     std::vector<int64_t> so, at; std::vector<int32_t> len, res;
     int64_t w = 0;
     for (int64_t c0 = 0; c0 < chunks; c0 += STREAM_RUN_CHUNKS) {
@@ -592,8 +605,9 @@ int64_t stream_encode(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_
             so[i] = (c0 + i) * block_size;
             len[i] = (int32_t)std::min<int64_t>(block_size, n - so[i]);
         }
-        int rc = run_host(c, (const uint8_t*)src, so.data(), len.data(), (uint8_t*)dst + w, nullptr, len.data(), res.data(), m,
-                          high_compression ? 1 : 0, at.data(), dst_cap - w, src_dev, false, (cudaStream_t)stream, &f);
+        int rc = run_host(c, Stage::STREAM_ENCODE, encode_op(high_compression != 0), (const uint8_t*)src, so.data(), len.data(),
+                          (uint8_t*)dst + w, nullptr, len.data(), res.data(), m, at.data(), dst_cap - w, src_dev, false,
+                          (cudaStream_t)stream);
         if (rc) return rc;
         w += at[m];
     }
@@ -605,9 +619,7 @@ int64_t stream_encode(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_
 int64_t stream_decode(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int64_t dst_cap, bool dst_dev, void* stream)
 {
     if (!c || n < 0 || (n > 0 && !src)) return fail(LZ4B200_E_ARG, "bad argument");
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    CallGuard g(c); if (g.rc) return g.rc;
     if (dst_dev) { int rc = check_side(c, src, false, "src"); if (rc) return rc; }
     std::vector<StreamChunk> chunks;
     const int64_t total = stream_walk((const uint8_t*)src, n, &chunks);
@@ -626,9 +638,9 @@ int64_t stream_decode(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int
     for (int64_t e0 = 0; e0 < entries; e0 += STREAM_RUN_CHUNKS) {
         const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, entries - e0);
         res.assign(m, -1);
-        const Framing f{false, stored.data() + e0, false};
-        int rc = run_host(c, (const uint8_t*)src, so.data() + e0, len.data() + e0, (uint8_t*)dst, dof.data() + e0, raw.data() + e0,
-                          res.data(), m, 2, nullptr, 0, false, dst_dev, (cudaStream_t)stream, &f);
+        int rc = run_host(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, (const uint8_t*)src, so.data() + e0, len.data() + e0,
+                          (uint8_t*)dst, dof.data() + e0, raw.data() + e0, res.data(), m, nullptr, 0, false, dst_dev,
+                          (cudaStream_t)stream, stored.data() + e0);
         if (rc) return rc;
         // a compressed chunk decodes from exactly its compLen bytes (LZ4Codec.Safe.cs:539-542)
         for (int32_t i = 0; i < m; i++)
@@ -655,16 +667,13 @@ int wrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, const 
         if (dst_off && (int64_t)dst_cap[i] < (int64_t)src_len[i] + WRAP_HEADER) return fail(LZ4B200_E_ARG, "dst_cap[i] < src_len[i] + 8");
         pcap[i] = src_len[i] + WRAP_HEADER;
     }
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    CallGuard g(c); if (g.rc) return g.rc;
     if (src_dev) {
         int rc = check_side(c, src, true, "src"); if (rc) return rc;
         rc = check_side(c, dst, false, "dst"); if (rc) return rc;
     }
-    const Framing f{false, nullptr, true};
-    return run_host(c, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, pcap.data(), out_len, n,
-                    high_compression ? 1 : 0, out_off, dst_total_cap, src_dev, false, (cudaStream_t)stream, &f);
+    return run_host(c, Stage::WRAP_ENCODE, encode_op(high_compression != 0), (const uint8_t*)src, src_off, src_len, (uint8_t*)dst,
+                    dst_off, pcap.data(), out_len, n, out_off, dst_total_cap, src_dev, false, (cudaStream_t)stream);
 }
 
 // Unwrap n packets in host memory into host or device memory (dst_dev): into the caller's slots, or packed (dst_off ==
@@ -673,7 +682,7 @@ int wrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, const 
 // apart in a large batch cost a cache and TLB miss each, and one thread would then take longer than the link.  A rejected
 // packet gets its status before any device work (E_FORMAT, or E_ARG above its capacity), an empty one 0.  Every other
 // packet is one entry of a known-size decode: a compressed one decodes its stored bytes into raw bytes, a stored one is
-// copied (Framing::stored).
+// copied (FRAMED_DECODE).
 int unwrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
                    const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
                    int64_t dst_total_cap, bool dst_dev, void* stream)
@@ -682,9 +691,7 @@ int unwrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, cons
     if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
     if (n == 0) { if (out_off) out_off[0] = 0; return LZ4B200_OK; }
     if (!src || !src_off || !src_len || !dst || !out_len || (dst_off ? !dst_cap : !out_off)) return fail(LZ4B200_E_ARG, "null argument");
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    CallGuard g(c); if (g.rc) return g.rc;
     if (dst_dev) {
         int rc = check_side(c, src, false, "src"); if (rc) return rc;
         rc = check_side(c, dst, true, "dst"); if (rc) return rc;
@@ -720,9 +727,8 @@ int unwrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, cons
     if (so.empty()) return LZ4B200_OK;
     const int32_t m = (int32_t)so.size();
     res.assign((size_t)m, -1);
-    const Framing f{false, stored.data(), false};
-    int rc = run_host(c, s, so.data(), len.data(), (uint8_t*)dst, dof.data(), cap.data(), res.data(), m, 2, nullptr, 0, false,
-                      dst_dev, (cudaStream_t)stream, &f);
+    int rc = run_host(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, s, so.data(), len.data(), (uint8_t*)dst, dof.data(), cap.data(),
+                      res.data(), m, nullptr, 0, false, dst_dev, (cudaStream_t)stream, stored.data());
     if (rc) return rc;
     // a compressed packet decodes from exactly its stored bytes (LZ4Codec.cs:595); one that does not is that packet's
     // E_FORMAT, not the call's
@@ -789,20 +795,17 @@ void lz4b200_destroy(lz4b200_ctx* c)
     if (!c) return;
     DeviceGuard g(c->device);
     cudaDeviceSynchronize();
-    for (int i = 0; i < NSLOT; i++) {
-        Slot& s = c->slot[i];
-        s.src.release(); s.dst.release(); s.meta.release(); s.hmeta.release(); s.packed.release(); s.offs.release(); s.scan.release(); s.hsrc.release(); s.hout.release();
+    for (Slot& s : c->slot) {
         if (s.done) cudaEventDestroy(s.done);
         if (s.carried) cudaEventDestroy(s.carried);
         if (s.stream) cudaStreamDestroy(s.stream);
     }
-    c->hc_arena.release(); c->compact_tmp.release(); c->packed_caps.release(); c->wrap_tmp.release();
     if (c->hc_done) cudaEventDestroy(c->hc_done);
     if (c->compact_done) cudaEventDestroy(c->compact_done);
     if (c->entry) cudaEventDestroy(c->entry);
     if (c->counters) cudaFree(c->counters);
     if (c->carry) cudaFree(c->carry);
-    delete c;
+    delete c;                                      // (the buffers free themselves, on the context's device)
 }
 
 int lz4b200_synchronize(lz4b200_ctx* c)
@@ -817,7 +820,7 @@ int lz4b200_encode_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off
                          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int mode, int mem, void* stream)
 {
     if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
-    return batch(c, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, mode == LZ4B200_MODE_HC ? 1 : 0, mem, stream);
+    return batch(c, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, encode_op(mode == LZ4B200_MODE_HC), mem, stream);
 }
 
 int lz4b200_encode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
@@ -828,7 +831,7 @@ int lz4b200_encode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
     if (n < 0 || !out_off) return fail(LZ4B200_E_ARG, "bad argument");
     if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
-    return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, mode == LZ4B200_MODE_HC ? 1 : 0, LZ4B200_MEM_HOST,
+    return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, encode_op(mode == LZ4B200_MODE_HC), LZ4B200_MEM_HOST,
                  nullptr, out_off, dst_total_cap);
 }
 
@@ -840,7 +843,7 @@ int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* c, const void* src, con
     if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
     if (n < 0 || !out_off) return fail(LZ4B200_E_ARG, "bad argument");
     if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
-    return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, mode == LZ4B200_MODE_HC ? 1 : 0,
+    return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, encode_op(mode == LZ4B200_MODE_HC),
                  LZ4B200_MEM_DEVICE_TO_HOST, stream, out_off, dst_total_cap);
 }
 
@@ -872,14 +875,16 @@ int64_t lz4b200_stream_decode_to_device(lz4b200_ctx* c, const void* src, int64_t
 int lz4b200_decode_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
                          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int known_len, int mem, void* stream)
 {
-    return batch(c, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, known_len ? 2 : 3, mem, stream);
+    return batch(c, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN,
+                 mem, stream);
 }
 
 int lz4b200_measure_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, const int32_t* dst_cap,
                           int32_t* out_len, int32_t n, int known_len, int mem, void* stream)
 {
     if (known_len && !dst_cap) return fail(LZ4B200_E_ARG, "dst_cap may be NULL only when known_len == 0");
-    return batch(c, src, src_off, src_len, nullptr, nullptr, dst_cap, out_len, n, known_len ? 4 : 5, mem, stream);
+    return batch(c, src, src_off, src_len, nullptr, nullptr, dst_cap, out_len, n, known_len ? Op::MEASURE_KNOWN : Op::MEASURE_UNKNOWN,
+                 mem, stream);
 }
 
 // measure -> scan -> capacities + "fits" -> decode, all enqueued on `stream`: the decoders leave at once (pick gate)
@@ -889,19 +894,11 @@ int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
 {
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    CallGuard g(c); if (g.rc) return g.rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    const size_t caps_bytes = sizeof(int32_t) * ((size_t)n + 1);
-    if (compact_tmp_bytes(n) > c->compact_tmp.cap || caps_bytes > c->packed_caps.cap) {
-        CU(cudaDeviceSynchronize());               // both scratch buffers may still be in use by an earlier call
-        CU(c->compact_tmp.reserve(compact_tmp_bytes(n))); CU(c->packed_caps.reserve(caps_bytes));
-    }
-    // the scan scratch and the capacities are the context's: calls on different streams are serialised on them
-    CU(cudaStreamWaitEvent(st, c->compact_done, 0));
+    int rc = call_scratch(c, st, compact_tmp_bytes(n), sizeof(int32_t) * ((size_t)n + 1)); if (rc) return rc;
     int32_t* caps = (int32_t*)c->packed_caps.p;
     int* fits = (int*)(caps + n);
     const BatchArgs m{(const uint8_t*)src, src_off, src_len, nullptr, nullptr, nullptr, out_len, n};
@@ -910,7 +907,7 @@ int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, caps, fits, st, &c->launches);
     if (e == cudaSuccess) {
         const BatchArgs d{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, caps, out_len, n};
-        e = launch_decode(d, false, c->decode_lanes_auto ? 0 : c->decode_lanes, c->counter(), c->dev, st, &c->launches, fits);
+        e = launch_decode(d, false, c->pinned_lanes(), c->counter(), c->dev, st, &c->launches, fits);
     }
     if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
     CU(cudaEventRecord(c->compact_done, st));
@@ -926,26 +923,21 @@ int lz4b200_decode_batch_packed_to_device(lz4b200_ctx* c, const void* src, const
     if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
     if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
-    if (!g.ok) return fail(LZ4B200_E_CUDA, "cudaSetDevice failed");
+    CallGuard g(c); if (g.rc) return g.rc;
     int rc = check_side(c, src, false, "src"); if (rc) return rc;
     rc = check_side(c, dst, true, "dst"); if (rc) return rc;
-    return run_host(c, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, nullptr, nullptr, out_len, n, 3, out_off, dst_total_cap,
-                    false, true, (cudaStream_t)stream);
+    return run_host(c, Stage::PLACED_DECODE, Op::DECODE_UNKNOWN, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, nullptr,
+                    nullptr, out_len, n, out_off, dst_total_cap, false, true, (cudaStream_t)stream);
 }
 
 int lz4b200_compact(lz4b200_ctx* c, const void* slots, const int64_t* slot_off, const int32_t* len, void* packed,
                     int64_t* out_off, int32_t n, void* stream)
 {
     if (!c || !slot_off || !len || !out_off || n < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
+    CallGuard g(c); if (g.rc) return g.rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
-    if (compact_tmp_bytes(n) > c->compact_tmp.cap) { CU(cudaDeviceSynchronize()); CU(c->compact_tmp.reserve(compact_tmp_bytes(n))); }
-    // one scan scratch per context: compactions on different streams are serialised on it
-    CU(cudaStreamWaitEvent(st, c->compact_done, 0));
+    int rc = call_scratch(c, st, compact_tmp_bytes(n)); if (rc) return rc;
     cudaError_t e = launch_compact((const uint8_t*)slots, slot_off, len, (uint8_t*)packed, out_off, n,
                                    c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "compact launch");
@@ -957,20 +949,16 @@ int lz4b200_compact(lz4b200_ctx* c, const void* slots, const int64_t* slot_off, 
 int lz4b200_wrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, int high_compression,
                               void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
 {
-    FRAME_CALL_PROLOGUE(c, n)
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
+    CallGuard g(c); if (g.rc) return g.rc;
     if (n == 0) return LZ4B200_OK;
     if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     cudaStream_t st = (cudaStream_t)stream;
-    WrapScratch w;
-    int rc = frame_scratch(c, n, false, st, &w); if (rc) return rc;
+    int rc = call_scratch(c, st, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    // the same encode as lz4b200_encode_batch(MEM_DEVICE): HC sizes its arena as if every block were above 64 KiB
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
-    cudaError_t e = launch_wrap_prep(a, w, st, &c->launches);
-    if (e != cudaSuccess) return cuda_fail(e, "wrap prep launch");
-    // every packet's payload, capacity = its input length (LZ4Codec.cs:518-523); the same path as lz4b200_encode_batch(MEM_DEVICE)
-    const BatchArgs enc{(const uint8_t*)src, src_off, w.len, (uint8_t*)dst, w.off, w.cap, w.res, n};
-    rc = run_device(c, enc, high_compression ? 1 : 0, st); if (rc) return rc;
-    e = launch_wrap_finish(a, w, st, &c->launches);
-    if (e != cudaSuccess) return cuda_fail(e, "wrap finish launch");
+    rc = run_wrap(c, a, wrap_scratch_at(c->wrap_tmp.p, n), encode_op(high_compression != 0), st, -1); if (rc) return rc;
     CU(cudaEventRecord(c->compact_done, st));
     return LZ4B200_OK;
 }
@@ -978,18 +966,20 @@ int lz4b200_wrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* sr
 int lz4b200_unwrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
                                 const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
 {
-    FRAME_CALL_PROLOGUE(c, n)
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
+    CallGuard g(c); if (g.rc) return g.rc;
     if (n == 0) return LZ4B200_OK;
     if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     cudaStream_t st = (cudaStream_t)stream;
-    WrapScratch w;
-    int rc = frame_scratch(c, n, false, st, &w); if (rc) return rc;
+    int rc = call_scratch(c, st, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    const WrapScratch w = wrap_scratch_at(c->wrap_tmp.p, n);
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
     cudaError_t e = launch_unwrap_prep(a, w, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "unwrap prep launch");
     // the compressed packets, known size (LZ4Codec.cs:595); stored and rejected ones are neutral entries
     const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, dst_off, w.cap, w.res, n};
-    rc = run_device(c, dec, 2, st); if (rc) return rc;
+    rc = run_device(c, dec, Op::DECODE_KNOWN, st); if (rc) return rc;
     e = launch_unwrap_finish(a, w, nullptr, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "unwrap finish launch");
     CU(cudaEventRecord(c->compact_done, st));
@@ -1000,13 +990,15 @@ int lz4b200_unwrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* 
 int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
                                 int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n, void* stream)
 {
-    FRAME_CALL_PROLOGUE(c, n)
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
+    CallGuard g(c); if (g.rc) return g.rc;
     if (!out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
     cudaStream_t st = (cudaStream_t)stream;
     if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    WrapScratch w;
-    int rc = frame_scratch(c, n, true, st, &w); if (rc) return rc;
+    int rc = call_scratch(c, st, compact_tmp_bytes(n), sizeof(int32_t) * ((size_t)n + 1), n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    const WrapScratch w = wrap_scratch_at(c->wrap_tmp.p, n);
     int32_t* caps = (int32_t*)c->packed_caps.p;
     int* fits = (int*)(caps + n);
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, nullptr, out_len, n};
@@ -1015,7 +1007,7 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, caps, fits, st, &c->launches);
     if (e == cudaSuccess) {
         const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, out_off, caps, w.res, n};
-        e = launch_decode(dec, true, c->decode_lanes_auto ? 0 : c->decode_lanes, c->counter(), c->dev, st, &c->launches, fits);
+        e = launch_decode(dec, true, c->pinned_lanes(), c->counter(), c->dev, st, &c->launches, fits);
     }
     if (e == cudaSuccess) e = launch_unwrap_finish(a, w, fits, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "packed unwrap launch");
@@ -1023,7 +1015,7 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     return LZ4B200_OK;
 }
 
-// ---- Wrap / Unwrap packets with a side in host memory: the host pipeline (run_host, Framing) ----
+// ---- Wrap / Unwrap packets with a side in host memory: the host pipeline (run_host, WRAP_ENCODE / FRAMED_DECODE) ----
 int lz4b200_wrap_batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, int high_compression,
                        void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n)
 {
@@ -1070,8 +1062,7 @@ int lz4b200_synth_fill(lz4b200_ctx* c, void* dst, int64_t n_blocks, int32_t bloc
                        int64_t first_block, void* stream)
 {
     if (!c || !dst) return fail(LZ4B200_E_ARG, "bad argument");
-    std::lock_guard<std::mutex> lock(c->mu);
-    DeviceGuard g(c->device);
+    CallGuard g(c); if (g.rc) return g.rc;
     cudaError_t e = launch_synth((uint8_t*)dst, n_blocks, block_size, cls, seed, first_block, c->dev,
                                  (cudaStream_t)stream, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "synth launch");
@@ -1165,9 +1156,9 @@ int lz4b200_peer_copy(void* dst, const void* src, int64_t bytes, void* stream)
     return LZ4B200_OK;
 }
 
-int lz4b200_compress_limitedOutput(const char* s, char* d, int isize, int cap) { return single(s, d, isize, cap, 0); }
-int lz4b200_compressHC_limitedOutput(const char* s, char* d, int isize, int cap) { return single(s, d, isize, cap, 1); }
-int lz4b200_uncompress(const char* s, char* d, int isize, int osize) { return single(s, d, isize, osize, 2); }
-int lz4b200_uncompress_unknownOutputSize(const char* s, char* d, int isize, int cap) { return single(s, d, isize, cap, 3); }
+int lz4b200_compress_limitedOutput(const char* s, char* d, int isize, int cap) { return single(s, d, isize, cap, Op::ENCODE_FAST); }
+int lz4b200_compressHC_limitedOutput(const char* s, char* d, int isize, int cap) { return single(s, d, isize, cap, Op::ENCODE_HC); }
+int lz4b200_uncompress(const char* s, char* d, int isize, int osize) { return single(s, d, isize, osize, Op::DECODE_KNOWN); }
+int lz4b200_uncompress_unknownOutputSize(const char* s, char* d, int isize, int cap) { return single(s, d, isize, cap, Op::DECODE_UNKNOWN); }
 
 }  // extern "C"

@@ -77,7 +77,7 @@ __global__ void __launch_bounds__(256) lz4_decode_pick_kernel(const int32_t* src
 }
 
 template <int G, bool KNOWN, bool STAGED>
-static cudaError_t launch_one(const BatchArgs& a, uint32_t* counter, const DeviceInfo& dev, cudaStream_t stream, const int* pick = nullptr, int code = 0)
+static cudaError_t launch_one(const BatchArgs& a, uint32_t* counter, const DeviceInfo& dev, cudaStream_t stream, const int* pick, int code)
 {
     int per_sm = 0;
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lz4_decode_kernel<G, KNOWN, STAGED>, DEC_THREADS, 0);
@@ -94,7 +94,7 @@ static cudaError_t launch_one(const BatchArgs& a, uint32_t* counter, const Devic
 
 template <int G>
 static cudaError_t launch_g(const BatchArgs& a, bool known, bool staged, uint32_t* counter, const DeviceInfo& dev, cudaStream_t stream,
-                            const int* pick = nullptr, int code = 0)
+                            const int* pick, int code)
 {
     if (staged) return known ? launch_one<G, true, true>(a, counter, dev, stream, pick, code) : launch_one<G, false, true>(a, counter, dev, stream, pick, code);
     return known ? launch_one<G, true, false>(a, counter, dev, stream, pick, code) : launch_one<G, false, false>(a, counter, dev, stream, pick, code);
@@ -136,7 +136,7 @@ static bool lpb_pays(int64_t n_blocks, const DeviceInfo& dev, bool middle_class)
 }
 
 template <bool KNOWN, class GEO>
-static cudaError_t launch_lpb(const BatchArgs& a, uint32_t* counter, const DeviceInfo& dev, cudaStream_t stream, const int* pick = nullptr, int takes108 = 1)
+static cudaError_t launch_lpb(const BatchArgs& a, uint32_t* counter, const DeviceInfo& dev, cudaStream_t stream, const int* pick, int takes108)
 {
     int warps = dev.smem_optin / (int)sizeof(LpbShared<GEO>);
     if (warps > lpb_warps<GEO>()) warps = lpb_warps<GEO>();
@@ -162,13 +162,18 @@ cudaError_t launch_decode(const BatchArgs& a, bool known_len, int lanes, uint32_
     if (e != cudaSuccess) return e;
     if (launches) ++*launches;
     int* pick = (int*)(counter + 1);                 // (the context hands out counters in fours: [block counter, pick, two more counters])
-    if (lanes != 0 && gate) {
-        // a pinned decoder behind a gate: the pick kernel passes the gate on as that kernel's code (or 0)
+    if (lanes != 0) {
+        // a pinned decoder.  Behind a gate the pick kernel goes first and passes the gate on as that kernel's code (or 0);
+        // without one the kernel gets no pick, and then ignores code and takes108.
         const int code = lanes == 1 ? 104 : lanes;
-        lz4_decode_pick_kernel<<<1, 256, 0, stream>>>(a.src_len, a.dst_cap, a.n_blocks, pick, gate, code);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        if (launches) ++*launches;
-        const bool staged = lanes >= 100;
+        if (gate) {
+            lz4_decode_pick_kernel<<<1, 256, 0, stream>>>(a.src_len, a.dst_cap, a.n_blocks, pick, gate, code);
+            if ((e = cudaGetLastError()) != cudaSuccess) return e;
+            if (launches) ++*launches;
+        } else {
+            pick = nullptr;
+        }
+        const bool staged = lanes >= 100;            // lanes = 100 + G selects the output-staged variant
         switch (lanes % 100) {
         case 1:  return known_len ? launch_lpb<true, LpbDefault>(a, counter, dev, stream, pick, 0) : launch_lpb<false, LpbDefault>(a, counter, dev, stream, pick, 0);
         case 4:  return launch_g<4>(a, known_len, staged, counter, dev, stream, pick, code);
@@ -177,41 +182,31 @@ cudaError_t launch_decode(const BatchArgs& a, bool known_len, int lanes, uint32_
         default: return launch_g<32>(a, known_len, staged, counter, dev, stream, pick, code);
         }
     }
-    if (lanes == 0) {
-        // auto: pick on the device, enqueue the four candidates (three of them return at once)
-        lz4_decode_pick_kernel<<<1, 256, 0, stream>>>(a.src_len, a.dst_cap, a.n_blocks, pick, gate, 0);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-        if (launches) *launches += 2;
-        if ((e = launch_g<32>(a, known_len, false, counter, dev, stream, pick, 32)) != cudaSuccess) return e;
-        if ((e = launch_g<16>(a, known_len, false, counter, dev, stream, pick, 16)) != cudaSuccess) return e;
-        // Sequence-dense classes.  The lane-per-block decoder works a batch off in waves of one block per lane; it gets the
-        // whole waves, the group kernels the rest (a last wave that is 46 % full, as in a 262 144-block batch, costs the
-        // token-dense class a quarter of its rate).  Batches below one wave: lpb_pays().
-        const int64_t wave = (int64_t)dev.num_sms * 32 * lpb_warps<LpbDefault>();
-        const int64_t head = a.n_blocks >= wave ? a.n_blocks / wave * wave : (lpb_pays(a.n_blocks, dev, false) ? a.n_blocks : 0);
-        const bool head108 = a.n_blocks >= wave || lpb_pays(a.n_blocks, dev, true);
-        if (head > 0) {
-            BatchArgs h = a; h.n_blocks = (int32_t)head;
-            if (launches) ++*launches;
-            e = known_len ? launch_lpb<true, LpbDefault>(h, counter, dev, stream, pick, head108 ? 1 : 0) : launch_lpb<false, LpbDefault>(h, counter, dev, stream, pick, head108 ? 1 : 0);
-            if (e != cudaSuccess) return e;
-        }
-        // the rest of the batch (or all of it) for the group kernels; class 108 also takes the head when the lanes did not
-        uint32_t* tc = counter + 2;
-        const int64_t skip104 = head, skip108 = head108 ? head : 0;
-        auto tail = [&](int64_t skip) { BatchArgs r = a; r.src_off += skip; r.src_len += skip; r.dst_off += skip; r.dst_cap += skip; r.out_len += skip; r.n_blocks = (int32_t)(a.n_blocks - skip); return r; };
-        if (a.n_blocks - skip108 > 0) { if (launches) ++*launches; if ((e = launch_g<8>(tail(skip108), known_len, true, tc, dev, stream, pick, 108)) != cudaSuccess) return e; }
-        if (a.n_blocks - skip104 > 0) { if (launches) ++*launches; if ((e = launch_g<4>(tail(skip104), known_len, true, tc + 1, dev, stream, pick, 104)) != cudaSuccess) return e; }
-        return cudaSuccess;
+    // auto: pick on the device, enqueue the four candidates (three of them return at once)
+    lz4_decode_pick_kernel<<<1, 256, 0, stream>>>(a.src_len, a.dst_cap, a.n_blocks, pick, gate, 0);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    if (launches) *launches += 2;
+    if ((e = launch_g<32>(a, known_len, false, counter, dev, stream, pick, 32)) != cudaSuccess) return e;
+    if ((e = launch_g<16>(a, known_len, false, counter, dev, stream, pick, 16)) != cudaSuccess) return e;
+    // Sequence-dense classes.  The lane-per-block decoder works a batch off in waves of one block per lane; it gets the
+    // whole waves, the group kernels the rest (a last wave that is 46 % full, as in a 262 144-block batch, costs the
+    // token-dense class a quarter of its rate).  Batches below one wave: lpb_pays().
+    const int64_t wave = (int64_t)dev.num_sms * 32 * lpb_warps<LpbDefault>();
+    const int64_t head = a.n_blocks >= wave ? a.n_blocks / wave * wave : (lpb_pays(a.n_blocks, dev, false) ? a.n_blocks : 0);
+    const bool head108 = a.n_blocks >= wave || lpb_pays(a.n_blocks, dev, true);
+    if (head > 0) {
+        BatchArgs h = a; h.n_blocks = (int32_t)head;
+        if (launches) ++*launches;
+        e = known_len ? launch_lpb<true, LpbDefault>(h, counter, dev, stream, pick, head108 ? 1 : 0) : launch_lpb<false, LpbDefault>(h, counter, dev, stream, pick, head108 ? 1 : 0);
+        if (e != cudaSuccess) return e;
     }
-    const bool staged = lanes >= 100;            // lanes = 100 + G selects the output-staged variant
-    switch (lanes % 100) {
-    case 1:  return known_len ? launch_lpb<true, LpbDefault>(a, counter, dev, stream) : launch_lpb<false, LpbDefault>(a, counter, dev, stream);
-    case 4:  return launch_g<4>(a, known_len, staged, counter, dev, stream);
-    case 8:  return launch_g<8>(a, known_len, staged, counter, dev, stream);
-    case 16: return launch_g<16>(a, known_len, staged, counter, dev, stream);
-    default: return launch_g<32>(a, known_len, staged, counter, dev, stream);
-    }
+    // the rest of the batch (or all of it) for the group kernels; class 108 also takes the head when the lanes did not
+    uint32_t* tc = counter + 2;
+    const int64_t skip104 = head, skip108 = head108 ? head : 0;
+    auto tail = [&](int64_t skip) { BatchArgs r = a; r.src_off += skip; r.src_len += skip; r.dst_off += skip; r.dst_cap += skip; r.out_len += skip; r.n_blocks = (int32_t)(a.n_blocks - skip); return r; };
+    if (a.n_blocks - skip108 > 0) { if (launches) ++*launches; if ((e = launch_g<8>(tail(skip108), known_len, true, tc, dev, stream, pick, 108)) != cudaSuccess) return e; }
+    if (a.n_blocks - skip104 > 0) { if (launches) ++*launches; if ((e = launch_g<4>(tail(skip104), known_len, true, tc + 1, dev, stream, pick, 104)) != cudaSuccess) return e; }
+    return cudaSuccess;
 }
 
 // ---- measure pass (lz4_measure.cuh): one thread per block, no shared memory ---------------------------------------------
