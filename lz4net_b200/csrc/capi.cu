@@ -14,6 +14,7 @@
 #include "../../include/lz4b200.h"
 #include "framing.h"
 #include "kernels.h"
+#include "lz4_packed.cuh"
 #include "lz4_stream.cuh"
 #include "lz4_wrap.cuh"
 
@@ -453,7 +454,7 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
             if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, d.out, nullptr, (int64_t*)sl.offs.p, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
             if (e != cudaSuccess) return cuda_fail(e, "packed measure launch");
             if (b0 > 0) CU(cudaStreamWaitEvent(sl.stream, c->slot[prev].carried, 0));
-            e = launch_packed_prep(d.out, (const int64_t*)sl.offs.p, m, dst_total_cap, d.dc, fits, sl.stream, &c->launches,
+            e = launch_packed_prep(d.out, (const int64_t*)sl.offs.p, m, dst_total_cap, PACKED_ROOM_UNKNOWN, d.dc, fits, sl.stream, &c->launches,
                                    b0 > 0 ? c->carry + prev : nullptr, d.dof, c->carry + s);
             if (e != cudaSuccess) return cuda_fail(e, "packed placement launch");
             CU(cudaEventRecord(sl.carried, sl.stream));
@@ -904,7 +905,7 @@ int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     const BatchArgs m{(const uint8_t*)src, src_off, src_len, nullptr, nullptr, nullptr, out_len, n};
     cudaError_t e = launch_measure(m, false, c->dev, st, &c->launches);
     if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, out_len, nullptr, out_off, n, c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
-    if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, caps, fits, st, &c->launches);
+    if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, PACKED_ROOM_UNKNOWN, caps, fits, st, &c->launches);
     if (e == cudaSuccess) {
         const BatchArgs d{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, caps, out_len, n};
         e = launch_decode(d, false, c->pinned_lanes(), c->counter(), c->dev, st, &c->launches, fits);
@@ -1004,7 +1005,7 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, nullptr, out_len, n};
     cudaError_t e = launch_unwrap_prep(a, w, st, &c->launches);
     if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, out_len, nullptr, out_off, n, c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
-    if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, caps, fits, st, &c->launches);
+    if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, 0, caps, fits, st, &c->launches);
     if (e == cudaSuccess) {
         const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, out_off, caps, w.res, n};
         e = launch_decode(dec, true, c->pinned_lanes(), c->counter(), c->dev, st, &c->launches, fits);

@@ -138,15 +138,15 @@ def _ptrs(addrs):
     return (C.c_void_p * len(addrs))(*addrs)
 
 
-def decode(blocks, caps, lanes=32, known=True, sched_seed=1, src_skew=0, dst_skew=0):
+def decode(blocks, caps, lanes=32, known=True, sched_seed=1, src_skew=0, dst_skew=0, fence=None, pad=0):
     """blocks: list of bytes (compressed); caps: list of int. Returns (results, outputs).  src_skew shifts the
-    compressed bytes inside their buffer to exercise unaligned stream starts."""
+    compressed bytes inside their buffer to exercise unaligned stream starts; fence / pad: see _staged."""
     n = len(blocks)
     isz = np.array([len(b) for b in blocks], np.int32)
     cps = np.array(caps, np.int32)
     res = np.zeros(n, np.int32)
     out = _Slots(caps, dst_skew)
-    with _staged(blocks, src_skew) as src:
+    with _staged(blocks, src_skew, fence, pad) as src:
         args = (int(known), n, _ptrs(src), isz.ctypes.data, _ptrs(out.ptrs), cps.ctypes.data, res.ctypes.data, sched_seed)
         if lanes in (1, 2):      # lane-per-block decoder (1: the kernel's geometry, 2: larger rings / 64-byte runs / one sequence per iteration)
             lib().emu_decode_lpb(lanes - 1, *args)

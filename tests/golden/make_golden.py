@@ -5,7 +5,8 @@
 
 golden_v1.json: encoder outputs on named inputs.  reference_v1.json: the reference's side of tests/test_oracle.py's
 port-versus-reference checks (return values and output digests), and the one input on which r93's LZ4HC gives up at
-LZ4_compressBound (tests/test_kernels_emu.py).
+LZ4_compressBound (tests/test_kernels_emu.py).  constructed_v1.json: what both reference decoders return on the
+constructed streams of tests/lz4seq.py, one case per line.
 
 The reference ships no golden vectors of its own (SURVEY.md 8c); these are outputs of the reference itself on
 reproducible inputs (tests/cases.py), including the reference-defined AutoTest text (src/LZ4/LZ4Codec.cs:175-184).
@@ -18,7 +19,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 import oracle  # noqa: E402
-from tests import cases  # noqa: E402
+from tests import cases, lz4seq  # noqa: E402
 
 
 def sha(b):
@@ -66,6 +67,18 @@ def main():
         json.dump(ref, f, separators=(",", ":"))
         f.write("\n")
     print("wrote", path)
+
+    digest, rows = t.records_constructed("ref")
+    past = sum(r[0] > len(c.stream) for c, r in zip(lz4seq.corpus(t.CONSTRUCTED_SEED), rows))
+    head = {"source": ref["source"], "generator": "tests/lz4seq.py", "seed": t.CONSTRUCTED_SEED, "corpus": digest,
+            "rows": t._digest(*(json.dumps(r) for r in rows)), "known_reads_past_isize": past,
+            "row": "[known-size result, unknown-size result, output digest]; -1 = rejected; a known-size result above the "
+                   "stream's length = accepted by reading past isize"}
+    with open(t.CONSTRUCTED, "w") as f:
+        f.write(json.dumps(head, separators=(",", ":"))[:-1] + ',"cases":[\n')
+        f.write(",\n".join(json.dumps(r, separators=(",", ":")) for r in rows))
+        f.write("\n]}\n")
+    print("wrote", t.CONSTRUCTED, len(rows), "cases,", past, "known-size decodes accepted only by reading past isize")
 
 
 if __name__ == "__main__":

@@ -15,6 +15,8 @@ from tests import cases
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden", "golden_v1.json")
 REF = os.path.join(os.path.dirname(__file__), "golden", "reference_v1.json")
+CONSTRUCTED = os.path.join(os.path.dirname(__file__), "golden", "constructed_v1.json")
+CONSTRUCTED_SEED = 1                                 # tests/lz4seq.py's corpus(seed) that constructed_v1.json records
 
 
 def _sha(b: bytes) -> str:
@@ -96,6 +98,22 @@ def records_corrupt_streams(impl):
         r, o = oracle.decode_unknown(bytes(c), len(data), impl=impl)
         streams.append(bytes(c)); out.append([max(r, -1), _digest(o)[:8] if r >= 0 else None])
     return _digest(*streams), out
+
+
+def records_constructed(impl):
+    """tests/lz4seq.py's corpus: (digest of every case's name, stream and cap, [known-size result, unknown-size result,
+    output digest] per case).  Results of a rejected stream are -1.  A known-size result past the end of the stream is
+    kept as it is -- the reference's LZ4_uncompress reads as far as the stream's tokens say, unbounded by design -- and
+    the bytes it decoded that way are not part of the digest."""
+    from tests import lz4seq
+    corpus = lz4seq.corpus(CONSTRUCTED_SEED)
+    rows = []
+    for c in corpus:
+        rk, ok = oracle.decode_known(c.stream, c.cap, impl=impl)
+        ru, ou = oracle.decode_unknown(c.stream, c.cap, impl=impl)
+        rows.append([max(rk, -1), max(ru, -1),
+                     _digest(ok if 0 <= rk <= len(c.stream) else b"-", ou if ru >= 0 else b"-")[:8]])
+    return _digest(*(p for c in corpus for p in (c.name, c.stream, c.cap))), rows
 
 
 def test_bound():
@@ -196,3 +214,30 @@ def test_mt_run_port_matches_single_calls():
         out = np.zeros(n * bs + 64, np.uint8)
         _, used = oracle.mt_run("decode", "port", comp, do, clen, out, so, sl, 3)
         assert np.array_equal(used, clen) and np.array_equal(out[:n * bs], raw), kind
+
+
+def test_port_equals_reference_on_constructed_streams():
+    """tests/lz4seq.py's constructed streams -- every end-of-block rule, offset and length threshold at the exact byte,
+    truncated, extended and under shifted caps: the port returns what the reference returned (constructed_v1.json, made
+    by make_golden.py), with the two documented exceptions:
+    * offset 0: the port rejects it (the reference copies output bytes nobody has written yet);
+    * a known-size decode the reference accepts only by reading past the end of the stream: the port, like every decoder
+      of this project, reads nothing outside [src, src + isize) and rejects it."""
+    from tests import lz4seq
+    stored = json.load(open(CONSTRUCTED))
+    want = stored["cases"]
+    assert _digest(*(json.dumps(w) for w in want)) == stored["rows"], "constructed_v1.json differs from what make_golden.py wrote"
+    corpus = lz4seq.corpus(CONSTRUCTED_SEED)
+    digest, got = records_constructed("port")
+    assert digest == stored["corpus"], "tests/lz4seq.py no longer makes the corpus the fixture was made from"
+    offset0 = 0
+    for c, w, g in zip(corpus, want, got):
+        if "/off0/" in c.name:
+            assert g[:2] == [-1, -1], c.name
+            offset0 += w[0] >= 0 or w[1] >= 0
+        elif w[0] > len(c.stream):
+            assert g[0] == -1 and g[1:] == w[1:], c.name
+        else:
+            assert g == w, (c.name, g, w)
+    past = sum(w[0] > len(c.stream) for c, w in zip(corpus, want))
+    assert offset0 > 0 and past == stored["known_reads_past_isize"] > 0

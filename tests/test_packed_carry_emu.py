@@ -26,6 +26,8 @@ def _lib():
         l = C.CDLL(emu.build(os.path.join(os.path.dirname(os.path.abspath(emu.__file__)), "simt_emu", "emu_packed.cpp")))
         l.emu_packed_place.restype = None
         l.emu_packed_place.argtypes = [_P, _P, _I, _P, _L, _P, _P, _P, _P, _U64]
+        l.emu_packed_place_room.restype = None
+        l.emu_packed_place_room.argtypes = [_P, _P, _I, _P, _L, _P, _P, _P, _P, _I, _U64]
         _plib = l
     return _plib
 
@@ -146,3 +148,27 @@ def test_a_batch_in_one_piece_gets_capacities_and_the_flag_only(n):
         _lib().emu_packed_place(sizes.ctypes.data, off.ctypes.data, n, None, total_cap, cap.ctypes.data, None, fits.ctypes.data,
                                 None, 3)
         assert cap[:n].tolist() == np.maximum(sizes, 0).tolist() and cap[n] == -77 and fits[0] == want
+
+
+@pytest.mark.parametrize("n", [1, 31, 32, 257])
+def test_unknown_size_decodes_get_room_beyond_the_size(n):
+    """lz4b200_decode_batch_packed and lz4b200_decode_batch_packed_to_device measured their blocks at INT32_MAX, and r93's
+    unknown-size rules look 12 bytes past the output cursor: their blocks get capacity size + 12 (at most INT32_MAX; 0 for
+    a malformed block).  Offsets, total and flag are those of room 0."""
+    sizes = np.random.default_rng(n).integers(-5, 5000, n).astype(np.int32)
+    sizes[0] = I32_MAX - 5
+    off = _scan(sizes)
+    want_cap = [0 if s < 0 else min(int(s) + 12, I32_MAX) for s in sizes]
+    for stage_base in (None, np.array([1000], np.int64)):
+        for total_cap in (int(off[n]) + 1000, int(off[n]) + 999):
+            cap = np.full(n + 1, -77, np.int32)
+            abs_off = np.full(n + 1, -77, np.int64)
+            fits = np.full(1, -77, np.int32)
+            total = np.full(1, -77, np.int64)
+            base = None if stage_base is None else stage_base.ctypes.data
+            _lib().emu_packed_place_room(sizes.ctypes.data, off.ctypes.data, n, base, total_cap, cap.ctypes.data,
+                                         abs_off.ctypes.data, fits.ctypes.data, total.ctypes.data, 12, 5)
+            b = 0 if stage_base is None else 1000
+            assert cap[:n].tolist() == want_cap and cap[n] == -77
+            assert abs_off[:n].tolist() == (b + off[:n]).tolist() and total[0] == b + off[n]
+            assert fits[0] == int(b + off[n] <= total_cap)
