@@ -164,6 +164,39 @@ int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* ctx,
 int lz4b200_compact(lz4b200_ctx* ctx, const void* slots, const int64_t* slot_off, const int32_t* len,
                     void* packed, int64_t* out_off, int32_t n_blocks, void* stream);
 
+/* ---- CUDA graphs: capturing the device-memory calls -------------------------------------------------------------
+ * The device-memory entry points -- lz4b200_encode_batch / decode_batch / measure_batch with LZ4B200_MEM_DEVICE,
+ * decode_batch_packed, compact, wrap_batch_device, unwrap_batch_device, unwrap_batch_packed and synth_fill -- may be
+ * enqueued on a stream that is capturing a CUDA graph, in any capture mode:
+ *   - Replaying the graph does exactly what the same call would do enqueued on the replay stream at replay time: the same
+ *     kernels, byte-identical outputs, the same out_len and out_off, for whatever the captured input buffers hold then.
+ *     The pointers and n_blocks are fixed at capture.
+ *   - Captured calls, eager calls and replays of graphs of one context, on any streams, stay ordered on the context's
+ *     shared scratch in host enqueue order, as eager calls are (one HC encode at a time, one user of the scan scratch,
+ *     capacities and packet view at a time).  Graphs that hold calls of one context may be replayed concurrently.
+ *     Calls of one capture that the capture forks onto several streams are ordered too, as long as one thread at a
+ *     time captures calls of the context (one context per caller thread, as above).
+ *   - A captured call never allocates, frees or synchronises.  When the context's scratch is too small for it, or its
+ *     4096 counter sets for captured calls are used up, it returns LZ4B200_E_ARG, enqueues nothing and leaves the
+ *     capture valid; lz4b200_last_error() says what is missing.  Call lz4b200_reserve before capturing.
+ *   - Scratch that a captured call referenced is never freed before lz4b200_destroy: a later growth (an eager call, or
+ *     lz4b200_reserve, or set_option("hc_concurrency")) allocates a new buffer and keeps the old one.  A context that
+ *     never captured frees and grows its scratch as before; every context holds the 64 KiB of counter sets.  Do not
+ *     replay a graph after lz4b200_destroy of a context it holds calls of.
+ *   - lz4b200_launch_count counts the launches a call enqueues when it is captured, not replays.
+ * Every other call that takes a `stream` synchronises with the host (the mixed-memory batches, the packed encode from
+ * and decode to device memory, the LZ4Stream and the Wrap / Unwrap calls between device and host memory): on a capturing
+ * stream it returns LZ4B200_E_ARG before any CUDA work, and the capture stays valid.  lz4b200_peer_copy is not covered.
+ * The calls without a stream (host-memory batches, single-block functions, lz4b200_synchronize, lz4b200_reserve) use
+ * the legacy default stream or synchronise the device: they must not be made while any thread of the process captures
+ * in cudaStreamCaptureModeGlobal.
+ *
+ * reserve: grows, eagerly, every piece of device scratch a device-memory call of at most max_blocks blocks takes; with
+ * high_compression != 0 also the HC state arena, as an HC device batch of max_blocks blocks sizes it under the current
+ * "hc_kernel", "hc_warps_per_sm" and "hc_concurrency" (changing those later may need more).  Afterwards any such call can
+ * be captured.  LZ4B200_E_ARG for a NULL context or max_blocks < 0. */
+int lz4b200_reserve(lz4b200_ctx* ctx, int32_t max_blocks, int high_compression);
+
 /* ---- single-block entry points (host pointers), 1:1 with the reference's native API -------------------------- */
 /* original/lz4.h:59-60  LZ4_compress_limitedOutput */
 int lz4b200_compress_limitedOutput(const char* source, char* dest, int isize, int maxOutputSize);

@@ -13,6 +13,20 @@ work already queued on the current torch stream, and move only compressed bytes 
 stream_decode_to_device do the same for the LZ4Stream format: a device tensor's bytes as a stream in host memory, and back.
 wrap_to_host, wrap_to_host_packed, unwrap_to_device and unwrap_to_device_packed do it for Wrap packets: inputs in a device
 tensor, packets in a host array, and back.
+
+The asynchronous helpers (synth_fill, encode, decode, measure, decode_packed, compact, wrap, wrap_packed, unwrap,
+unwrap_packed) can be captured in a CUDA graph: reserve the scratch of the largest batch first, then capture, then replay
+with new contents in the same tensors:
+
+    ctx.reserve(n_blocks, hc=True)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        batch.encode(ctx, raw, src_off, src_len, slots, dst_off, dst_cap, out_len, hc=True)
+        batch.compact(ctx, slots, dst_off, out_len, packed, out_off)
+    g.replay()
+
+A call whose scratch was not reserved raises Lz4B200Error (E_ARG) and leaves the capture valid.  The synchronous helpers
+refuse a capturing stream the same way.
 """
 from __future__ import annotations
 

@@ -69,6 +69,11 @@ class Context:
     def synchronize(self):
         native.check(native.lib().lz4b200_synchronize(self._h), "synchronize")
 
+    def reserve(self, max_blocks: int, hc: bool = False):
+        """Grow the device scratch of device-memory calls of at most max_blocks blocks (with hc: the HC arena too), so that
+        they can be captured in a CUDA graph (lz4b200_reserve)."""
+        native.check(native.lib().lz4b200_reserve(self._h, int(max_blocks), int(hc)), "reserve")
+
     @property
     def launches(self) -> int:
         return int(native.lib().lz4b200_launch_count(self._h))

@@ -44,7 +44,8 @@ int cuda_fail(cudaError_t e, const char* what)
 #define CU(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return cuda_fail(e_, #x); } while (0)
 
 constexpr int NSLOT = 3;                       // pipeline depth of host-memory batches
-constexpr int NCOUNTER = 256;
+constexpr int NCOUNTER = 256;                 // the eager calls' ring of counter sets (four words each)
+constexpr int NCAPTURED = 4096;                // counter sets for captured calls, never recycled (64 KiB behind the ring)
 constexpr size_t HOST_CHUNK_BYTES_DEFAULT = 128u << 20; // src + dst bytes per pipeline stage (on H100 the best of 32..512 MiB: profiles/README.md)
 
 // Grow-only buffers that free themselves (the context's device is current when a context is destroyed): device memory,
@@ -69,6 +70,55 @@ struct Buf {
 };
 using DevBuf = Buf<false>;
 using PinBuf = Buf<true>;
+
+// Device scratch that a captured call may reference (the context's call scratch and HC arena).  A graph keeps the address
+// it captured, so once a captured call has referenced the buffer (held), growing it retires the old buffer to the
+// context's list, which lz4b200_destroy frees, instead of freeing it.  A buffer no capture referenced grows as a DevBuf.
+struct SharedBuf : DevBuf {
+    bool held = false;
+    cudaError_t grow(size_t n, std::vector<void*>& retired)
+    {
+        if (n <= cap) return cudaSuccess;
+        drop(retired);
+        return reserve(n);
+    }
+    void drop(std::vector<void*>& retired)
+    {
+        if (held && p) { retired.push_back(p); p = nullptr; cap = 0; }
+        held = false;
+        release();
+    }
+};
+
+// Whether a call's stream is capturing (a CUDA graph being recorded), and which capture.
+struct Capture { bool on = false; unsigned long long id = 0; };
+
+// The order of the calls that share one piece of the context's scratch, whatever streams they are on: each waits on
+// `done`, then records it.  Inside a capture the wait and the record are external event nodes, so that a replay waits for
+// the call enqueued before it and the call enqueued after it waits for the replay, as eager calls do.  An external wait
+// sees the event as it was when the graph was launched, so captured calls of the one capture are also chained through
+// `inner`, an ordinary captured record / wait, in case the capture forks them onto separate streams.  `inner` remembers
+// one capture: while two threads capture calls of one context, a capture's forked calls may miss that inner order (one
+// context per caller thread, include/lz4b200.h).
+struct Chain {
+    cudaEvent_t done = nullptr, inner = nullptr;
+    unsigned long long inner_id = 0;       // the capture that last recorded `inner` (0: none)
+    cudaError_t wait(cudaStream_t st, const Capture& cap) const
+    {
+        if (!cap.on) return cudaStreamWaitEvent(st, done, 0);
+        cudaError_t e = cudaStreamWaitEvent(st, done, cudaEventWaitExternal);
+        if (e == cudaSuccess && inner_id == cap.id) e = cudaStreamWaitEvent(st, inner, 0);
+        return e;
+    }
+    cudaError_t record(cudaStream_t st, const Capture& cap)
+    {
+        if (!cap.on) return cudaEventRecord(done, st);
+        cudaError_t e = cudaEventRecordWithFlags(done, st, cudaEventRecordExternal);
+        if (e == cudaSuccess) e = cudaEventRecord(inner, st);
+        if (e == cudaSuccess) inner_id = cap.id;
+        return e;
+    }
+};
 
 // Pageable host memory (a managed caller's `fixed` byte[]): cudaMemcpyAsync from / to it is staged by the driver through
 // its own small pinned buffers, synchronously (several times slower than from pinned memory).  The library
@@ -154,13 +204,15 @@ enum class Stage {
 struct lz4b200_ctx {
     int device = 0;
     DeviceInfo dev{};
-    uint32_t* counters = nullptr;
+    uint32_t* counters = nullptr;          // NCOUNTER words of the ring, then NCAPTURED sets of the capture pool
     int next_counter = 0;
-    DevBuf hc_arena, compact_tmp;
-    DevBuf packed_caps;                    // lz4b200_decode_batch_packed: per-block capacities + the "fits" flag (serialised like compact_tmp)
-    DevBuf wrap_tmp;                       // the device Wrap / Unwrap calls: the codec's view of the packets (serialised like compact_tmp)
-    cudaEvent_t hc_done = nullptr;         // the HC state arena is shared: HC launches are chained through this event
-    cudaEvent_t compact_done = nullptr;    // likewise compact_tmp, packed_caps and wrap_tmp (call_scratch)
+    int next_captured = 0;                 // capture pool sets handed out
+    SharedBuf hc_arena, compact_tmp;
+    SharedBuf packed_caps;                 // lz4b200_decode_batch_packed: per-block capacities + the "fits" flag (serialised like compact_tmp)
+    SharedBuf wrap_tmp;                    // the device Wrap / Unwrap calls: the codec's view of the packets (serialised like compact_tmp)
+    std::vector<void*> retired;            // shared scratch a graph may still reference: freed by lz4b200_destroy
+    Chain hc_done;                         // the HC state arena is shared: HC launches are chained through this event
+    Chain compact_done;                    // likewise compact_tmp, packed_caps and wrap_tmp (call_scratch)
     cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
     int64_t* carry = nullptr;              // the packed decode into device memory: NSLOT cells, the running output offset behind each slot's stage
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
@@ -176,7 +228,13 @@ struct lz4b200_ctx {
     int64_t launches = 0;
     std::mutex mu;
 
-    uint32_t* counter() { uint32_t* c = counters + next_counter; next_counter = (next_counter + 4) % NCOUNTER; return c; }   // fours: [block counter, decoder pick, two more counters]
+    // fours: [block counter, decoder pick, two more counters].  A captured call keeps its set for every replay: it takes one
+    // of the capture pool, which admit() has checked is not used up.
+    uint32_t* counter(const Capture& cap = {})
+    {
+        if (cap.on) return counters + NCOUNTER + 4 * next_captured++;
+        uint32_t* c = counters + next_counter; next_counter = (next_counter + 4) % NCOUNTER; return c;
+    }
     int pinned_lanes() const { return decode_lanes_auto ? 0 : decode_lanes; }   // 0: the decoder is picked on the device
 };
 
@@ -197,17 +255,71 @@ struct CallGuard {
         : lock(c->mu), dev(c->device), rc(dev.ok ? LZ4B200_OK : fail(LZ4B200_E_CUDA, "cudaSetDevice failed")) {}
 };
 
-// The context's call scratch (compact_tmp, packed_caps, wrap_tmp) is shared by the device calls on every stream.  A call
-// grows the buffers it needs to at least these sizes -- behind one cudaDeviceSynchronize, since an earlier call may still
-// be using them -- and orders `st` behind the last call that used them.  The caller records compact_done on `st` once its
-// launches are in.
-int call_scratch(lz4b200_ctx* c, cudaStream_t st, size_t compact_bytes, size_t caps_bytes = 0, size_t wrap_bytes = 0)
+// Whether `st` is capturing.  Every call that takes a stream asks this before any other work on it.
+int capture_of(cudaStream_t st, Capture* cap)
 {
-    if (compact_bytes > c->compact_tmp.cap || caps_bytes > c->packed_caps.cap || wrap_bytes > c->wrap_tmp.cap) {
-        CU(cudaDeviceSynchronize());
-        CU(c->compact_tmp.reserve(compact_bytes)); CU(c->packed_caps.reserve(caps_bytes)); CU(c->wrap_tmp.reserve(wrap_bytes));
-    }
-    CU(cudaStreamWaitEvent(st, c->compact_done, 0));
+    cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
+    CU(cudaStreamGetCaptureInfo(st, &s, &cap->id));
+    cap->on = s != cudaStreamCaptureStatusNone;
+    return LZ4B200_OK;
+}
+
+// The calls that synchronise refuse a capturing stream before any CUDA work, which leaves the caller's capture valid.
+int refuse_capture(void* stream, const char* what)
+{
+    Capture cap;
+    int rc = capture_of((cudaStream_t)stream, &cap); if (rc) return rc;
+    return cap.on ? fail(LZ4B200_E_ARG, std::string(what) + " synchronises with the host: it cannot be enqueued on a capturing stream")
+                  : LZ4B200_OK;
+}
+
+// The HC arena a device batch of n blocks needs (hc_large: blocks above 64 KiB, -1 = not known), under the current options.
+size_t hc_arena_bytes(const lz4b200_ctx* c, int32_t n, int32_t hc_large)
+{
+    if (c->hc_kernel < 0) return hc_auto_scratch_bytes(n, hc_large, c->dev);
+    if (c->hc_kernel) return hcw_scratch_bytes(n, hc_large, c->hc_kernel, c->hc_warps_per_sm, c->dev);
+    return hc_scratch_bytes((int)std::min<int64_t>(c->hc_concurrency, std::max(n, 1)));
+}
+
+// Grows the shared scratch to at least these sizes, behind one cudaDeviceSynchronize, since an earlier call may still be
+// using it.  Eager calls and lz4b200_reserve only.
+int grow_scratch(lz4b200_ctx* c, size_t compact_bytes, size_t caps_bytes, size_t wrap_bytes, size_t hc_bytes = 0)
+{
+    if (compact_bytes <= c->compact_tmp.cap && caps_bytes <= c->packed_caps.cap && wrap_bytes <= c->wrap_tmp.cap && hc_bytes <= c->hc_arena.cap)
+        return LZ4B200_OK;
+    CU(cudaDeviceSynchronize());
+    CU(c->compact_tmp.grow(compact_bytes, c->retired)); CU(c->packed_caps.grow(caps_bytes, c->retired));
+    CU(c->wrap_tmp.grow(wrap_bytes, c->retired)); CU(c->hc_arena.grow(hc_bytes, c->retired));
+    return LZ4B200_OK;
+}
+
+// A captured call never allocates, frees or synchronises: it enqueues nothing unless the scratch it needs is already there
+// at its size (lz4b200_reserve grows it) and the capture pool has the counter sets it takes.  The buffers it references
+// are then held for the graph.  hc_blocks: the blocks of an HC encode inside the call (-1: none).  Eager calls pass.
+int admit(lz4b200_ctx* c, const Capture& cap, int counters, size_t compact_bytes, size_t caps_bytes = 0, size_t wrap_bytes = 0,
+          int32_t hc_blocks = -1)
+{
+    if (!cap.on) return LZ4B200_OK;
+    const size_t hc_bytes = hc_blocks >= 0 ? hc_arena_bytes(c, hc_blocks, -1) : 0;
+    if (compact_bytes > c->compact_tmp.cap || caps_bytes > c->packed_caps.cap || wrap_bytes > c->wrap_tmp.cap || hc_bytes > c->hc_arena.cap)
+        return fail(LZ4B200_E_ARG, "the context's scratch is too small to capture this call: call lz4b200_reserve(ctx, n_blocks, "
+                                   "high_compression) before capturing");
+    if (c->next_captured + counters > NCAPTURED)
+        return fail(LZ4B200_E_ARG, "the context's " + std::to_string(NCAPTURED) + " counter sets for captured calls are used up");
+    if (compact_bytes) c->compact_tmp.held = true;
+    if (caps_bytes) c->packed_caps.held = true;
+    if (wrap_bytes) c->wrap_tmp.held = true;
+    if (hc_blocks >= 0) c->hc_arena.held = true;
+    return LZ4B200_OK;
+}
+
+// The context's call scratch (compact_tmp, packed_caps, wrap_tmp) is shared by the device calls on every stream.  A call
+// grows the buffers it needs to at least these sizes (an eager call: a captured one has been admitted at them) and orders
+// `st` behind the last call that used them.  The caller records compact_done on `st` once its launches are in.
+int call_scratch(lz4b200_ctx* c, cudaStream_t st, const Capture& cap, size_t compact_bytes, size_t caps_bytes = 0, size_t wrap_bytes = 0)
+{
+    if (!cap.on) { int rc = grow_scratch(c, compact_bytes, caps_bytes, wrap_bytes); if (rc) return rc; }
+    CU(c->compact_done.wait(st, cap));
     return LZ4B200_OK;
 }
 
@@ -224,31 +336,28 @@ int lanes_for_ratio(double ratio, int64_t n_blocks, const DeviceInfo& dev)
     return g == 104 && n_blocks >= (int64_t)dev.num_sms * 32 * 8 ? 1 : g;
 }
 
-// hc_large: blocks above 64 KiB in an HC batch (-1 = not known: a device-memory batch)
-int run_device(lz4b200_ctx* c, const BatchArgs& a, Op op, cudaStream_t st, int lanes = 0, int32_t hc_large = -1)
+// hc_large: blocks above 64 KiB in an HC batch (-1 = not known: a device-memory batch).  A captured call (cap) has been
+// admitted with the arena and the counter set it takes.
+int run_device(lz4b200_ctx* c, const BatchArgs& a, Op op, cudaStream_t st, int lanes = 0, int32_t hc_large = -1, const Capture& cap = {})
 {
     if (!lanes) lanes = c->pinned_lanes();
     cudaError_t e = cudaSuccess;
     switch (op) {
-    case Op::ENCODE_FAST: e = launch_encode_fast(a, c->counter(), c->encode_ctas_per_sm, c->encode_tune, c->encode_variant, c->dev, st, &c->launches); break;
+    case Op::ENCODE_FAST: e = launch_encode_fast(a, c->counter(cap), c->encode_ctas_per_sm, c->encode_tune, c->encode_variant, c->dev, st, &c->launches); break;
     case Op::ENCODE_HC: {
         const int conc = (int)std::min<int64_t>(c->hc_concurrency, std::max(a.n_blocks, 1));
-        const size_t need = c->hc_kernel < 0 ? hc_auto_scratch_bytes(a.n_blocks, hc_large, c->dev)
-                          : (c->hc_kernel ? hcw_scratch_bytes(a.n_blocks, hc_large, c->hc_kernel, c->hc_warps_per_sm, c->dev) : hc_scratch_bytes(conc));
-        if (need > c->hc_arena.cap) {
-            CU(cudaDeviceSynchronize());           // the arena may still be in use by an earlier launch
-            CU(c->hc_arena.reserve(need));
-        }
+        if (!cap.on) { int rc = grow_scratch(c, 0, 0, 0, hc_arena_bytes(c, a.n_blocks, hc_large)); if (rc) return rc; }
         // one arena per context: an HC launch may not overlap the previous one, whatever stream it was given
-        CU(cudaStreamWaitEvent(st, c->hc_done, 0));
-        e = c->hc_kernel < 0 ? launch_encode_hc_auto(a, c->hc_arena.p, hc_large, c->counter(), c->dev, st, &c->launches)
-          : c->hc_kernel ? launch_encode_hcw(a, c->hc_arena.p, c->hc_kernel, c->hc_warps_per_sm, hc_large, c->counter(), c->dev, st, &c->launches)
-                              : launch_encode_hc(a, c->hc_arena.p, conc, c->counter(), c->dev, st, &c->launches);
-        if (e == cudaSuccess) e = cudaEventRecord(c->hc_done, st);
+        CU(c->hc_done.wait(st, cap));
+        uint32_t* counter = c->counter(cap);
+        e = c->hc_kernel < 0 ? launch_encode_hc_auto(a, c->hc_arena.p, hc_large, counter, c->dev, st, &c->launches)
+          : c->hc_kernel ? launch_encode_hcw(a, c->hc_arena.p, c->hc_kernel, c->hc_warps_per_sm, hc_large, counter, c->dev, st, &c->launches)
+                              : launch_encode_hc(a, c->hc_arena.p, conc, counter, c->dev, st, &c->launches);
+        if (e == cudaSuccess) e = c->hc_done.record(st, cap);
         break;
     }
     case Op::DECODE_KNOWN:
-    case Op::DECODE_UNKNOWN: e = launch_decode(a, op == Op::DECODE_KNOWN, lanes, c->counter(), c->dev, st, &c->launches); break;
+    case Op::DECODE_UNKNOWN: e = launch_decode(a, op == Op::DECODE_KNOWN, lanes, c->counter(cap), c->dev, st, &c->launches); break;
     case Op::MEASURE_KNOWN:
     case Op::MEASURE_UNKNOWN: e = launch_measure(a, op == Op::MEASURE_KNOWN, c->dev, st, &c->launches); break;
     }
@@ -258,11 +367,11 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, Op op, cudaStream_t st, int l
 // A Wrap of the batch a into whole packets: prep (each payload behind its header's place, capacity = its input length,
 // LZ4Codec.cs:518-523) -> the batch codec, unchanged, on the codec's view w -> finish (the headers, the stored inputs,
 // out_len = the packet sizes).
-int run_wrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, Op op, cudaStream_t st, int32_t hc_large)
+int run_wrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, Op op, cudaStream_t st, int32_t hc_large, const Capture& cap = {})
 {
     int rc = launched(launch_wrap_prep(a, w, st, &c->launches), "wrap prep launch"); if (rc) return rc;
     const BatchArgs enc{a.src, a.src_off, w.len, a.dst, w.off, w.cap, w.res, a.n_blocks};
-    rc = run_device(c, enc, op, st, 0, hc_large); if (rc) return rc;
+    rc = run_device(c, enc, op, st, 0, hc_large, cap); if (rc) return rc;
     return launched(launch_wrap_finish(a, w, st, &c->launches), "wrap finish launch");
 }
 
@@ -531,16 +640,20 @@ int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t
         return fail(LZ4B200_E_ARG, "null argument");
     CallGuard g(c); if (g.rc) return g.rc;
     if (mem == LZ4B200_MEM_DEVICE) {
+        Capture cap;
+        int rc = capture_of((cudaStream_t)stream, &cap); if (rc) return rc;
+        rc = admit(c, cap, measure ? 0 : 1, 0, 0, 0, op == Op::ENCODE_HC ? n : -1); if (rc) return rc;
         BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
-        return run_device(c, a, op, (cudaStream_t)stream);
+        return run_device(c, a, op, (cudaStream_t)stream, 0, -1, cap);
     }
     const bool src_dev = mem == LZ4B200_MEM_DEVICE_TO_HOST, dst_dev = mem == LZ4B200_MEM_HOST_TO_DEVICE;
     if (mem != LZ4B200_MEM_HOST && !src_dev && !dst_dev)
         return fail(LZ4B200_E_ARG, "mem must be LZ4B200_MEM_HOST, _DEVICE, _DEVICE_TO_HOST or _HOST_TO_DEVICE");
     if (src_dev || dst_dev) {
+        int rc = refuse_capture(stream, "a mixed-memory batch"); if (rc) return rc;
         // the measure pass has no destination: MEM_HOST and MEM_DEVICE already cover both places its source can be
         if (measure) return fail(LZ4B200_E_ARG, "measure_batch takes LZ4B200_MEM_HOST or LZ4B200_MEM_DEVICE");
-        int rc = check_side(c, src, src_dev, "src"); if (rc) return rc;
+        rc = check_side(c, src, src_dev, "src"); if (rc) return rc;
         rc = check_side(c, dst, dst_dev, "dst"); if (rc) return rc;
     }
     return run_host(c, Stage::CODEC, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, out_off,
@@ -593,7 +706,8 @@ int64_t stream_encode(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_
     if (n == 0) return 0;
     CallGuard g(c); if (g.rc) return g.rc;
     if (src_dev) {
-        int rc = check_side(c, src, true, "src"); if (rc) return rc;
+        int rc = refuse_capture(stream, "lz4b200_stream_encode_from_device"); if (rc) return rc;
+        rc = check_side(c, src, true, "src"); if (rc) return rc;
         rc = check_side(c, dst, false, "dst"); if (rc) return rc;
     }
     const int64_t chunks = (n + block_size - 1) / block_size;
@@ -621,7 +735,10 @@ int64_t stream_decode(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int
 {
     if (!c || n < 0 || (n > 0 && !src)) return fail(LZ4B200_E_ARG, "bad argument");
     CallGuard g(c); if (g.rc) return g.rc;
-    if (dst_dev) { int rc = check_side(c, src, false, "src"); if (rc) return rc; }
+    if (dst_dev) {
+        int rc = refuse_capture(stream, "lz4b200_stream_decode_to_device"); if (rc) return rc;
+        rc = check_side(c, src, false, "src"); if (rc) return rc;
+    }
     std::vector<StreamChunk> chunks;
     const int64_t total = stream_walk((const uint8_t*)src, n, &chunks);
     if (total < 0) return fail((int)total, "malformed LZ4Stream");
@@ -670,7 +787,8 @@ int wrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, const 
     }
     CallGuard g(c); if (g.rc) return g.rc;
     if (src_dev) {
-        int rc = check_side(c, src, true, "src"); if (rc) return rc;
+        int rc = refuse_capture(stream, "a Wrap from device memory"); if (rc) return rc;
+        rc = check_side(c, src, true, "src"); if (rc) return rc;
         rc = check_side(c, dst, false, "dst"); if (rc) return rc;
     }
     return run_host(c, Stage::WRAP_ENCODE, encode_op(high_compression != 0), (const uint8_t*)src, src_off, src_len, (uint8_t*)dst,
@@ -694,7 +812,8 @@ int unwrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, cons
     if (!src || !src_off || !src_len || !dst || !out_len || (dst_off ? !dst_cap : !out_off)) return fail(LZ4B200_E_ARG, "null argument");
     CallGuard g(c); if (g.rc) return g.rc;
     if (dst_dev) {
-        int rc = check_side(c, src, false, "src"); if (rc) return rc;
+        int rc = refuse_capture(stream, "an Unwrap into device memory"); if (rc) return rc;
+        rc = check_side(c, src, false, "src"); if (rc) return rc;
         rc = check_side(c, dst, true, "dst"); if (rc) return rc;
     }
     const uint8_t* s = (const uint8_t*)src;
@@ -776,10 +895,12 @@ int lz4b200_create(lz4b200_ctx** out, int device)
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device); c->dev.num_sms = v;
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device); c->dev.smem_per_sm = v;
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device); c->dev.smem_optin = v;
-    cudaError_t e = cudaMalloc(&c->counters, sizeof(uint32_t) * NCOUNTER);
+    cudaError_t e = cudaMalloc(&c->counters, sizeof(uint32_t) * (NCOUNTER + 4 * NCAPTURED));
     if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * NSLOT);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->hc_done, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->compact_done, cudaEventDisableTiming);
+    for (Chain* ch : {&c->hc_done, &c->compact_done}) {
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->done, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->inner, cudaEventDisableTiming);
+    }
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->entry, cudaEventDisableTiming);
     for (int i = 0; i < NSLOT && e == cudaSuccess; i++) {
         e = cudaStreamCreateWithFlags(&c->slot[i].stream, cudaStreamNonBlocking);
@@ -801,11 +922,14 @@ void lz4b200_destroy(lz4b200_ctx* c)
         if (s.carried) cudaEventDestroy(s.carried);
         if (s.stream) cudaStreamDestroy(s.stream);
     }
-    if (c->hc_done) cudaEventDestroy(c->hc_done);
-    if (c->compact_done) cudaEventDestroy(c->compact_done);
+    for (Chain* ch : {&c->hc_done, &c->compact_done}) {
+        if (ch->done) cudaEventDestroy(ch->done);
+        if (ch->inner) cudaEventDestroy(ch->inner);
+    }
     if (c->entry) cudaEventDestroy(c->entry);
     if (c->counters) cudaFree(c->counters);
     if (c->carry) cudaFree(c->carry);
+    for (void* p : c->retired) cudaFree(p);
     delete c;                                      // (the buffers free themselves, on the context's device)
 }
 
@@ -897,9 +1021,13 @@ int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
     CallGuard g(c); if (g.rc) return g.rc;
     cudaStream_t st = (cudaStream_t)stream;
+    Capture cap;
+    int rc = capture_of(st, &cap); if (rc) return rc;
     if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    int rc = call_scratch(c, st, compact_tmp_bytes(n), sizeof(int32_t) * ((size_t)n + 1)); if (rc) return rc;
+    const size_t compact_bytes = compact_tmp_bytes(n), caps_bytes = sizeof(int32_t) * ((size_t)n + 1);
+    rc = admit(c, cap, 1, compact_bytes, caps_bytes); if (rc) return rc;
+    rc = call_scratch(c, st, cap, compact_bytes, caps_bytes); if (rc) return rc;
     int32_t* caps = (int32_t*)c->packed_caps.p;
     int* fits = (int*)(caps + n);
     const BatchArgs m{(const uint8_t*)src, src_off, src_len, nullptr, nullptr, nullptr, out_len, n};
@@ -908,10 +1036,10 @@ int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, PACKED_ROOM_UNKNOWN, caps, fits, st, &c->launches);
     if (e == cudaSuccess) {
         const BatchArgs d{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, caps, out_len, n};
-        e = launch_decode(d, false, c->pinned_lanes(), c->counter(), c->dev, st, &c->launches, fits);
+        e = launch_decode(d, false, c->pinned_lanes(), c->counter(cap), c->dev, st, &c->launches, fits);
     }
     if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
-    CU(cudaEventRecord(c->compact_done, st));
+    CU(c->compact_done.record(st, cap));
     return LZ4B200_OK;
 }
 
@@ -925,7 +1053,8 @@ int lz4b200_decode_batch_packed_to_device(lz4b200_ctx* c, const void* src, const
     if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     CallGuard g(c); if (g.rc) return g.rc;
-    int rc = check_side(c, src, false, "src"); if (rc) return rc;
+    int rc = refuse_capture(stream, "lz4b200_decode_batch_packed_to_device"); if (rc) return rc;
+    rc = check_side(c, src, false, "src"); if (rc) return rc;
     rc = check_side(c, dst, true, "dst"); if (rc) return rc;
     return run_host(c, Stage::PLACED_DECODE, Op::DECODE_UNKNOWN, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, nullptr,
                     nullptr, out_len, n, out_off, dst_total_cap, false, true, (cudaStream_t)stream);
@@ -937,12 +1066,15 @@ int lz4b200_compact(lz4b200_ctx* c, const void* slots, const int64_t* slot_off, 
     if (!c || !slot_off || !len || !out_off || n < 0) return fail(LZ4B200_E_ARG, "bad argument");
     CallGuard g(c); if (g.rc) return g.rc;
     cudaStream_t st = (cudaStream_t)stream;
+    Capture cap;
+    int rc = capture_of(st, &cap); if (rc) return rc;
     if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
-    int rc = call_scratch(c, st, compact_tmp_bytes(n)); if (rc) return rc;
+    rc = admit(c, cap, 0, compact_tmp_bytes(n)); if (rc) return rc;
+    rc = call_scratch(c, st, cap, compact_tmp_bytes(n)); if (rc) return rc;
     cudaError_t e = launch_compact((const uint8_t*)slots, slot_off, len, (uint8_t*)packed, out_off, n,
                                    c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "compact launch");
-    CU(cudaEventRecord(c->compact_done, st));
+    CU(c->compact_done.record(st, cap));
     return LZ4B200_OK;
 }
 
@@ -956,11 +1088,14 @@ int lz4b200_wrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* sr
     if (n == 0) return LZ4B200_OK;
     if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     cudaStream_t st = (cudaStream_t)stream;
-    int rc = call_scratch(c, st, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    Capture cap;
+    int rc = capture_of(st, &cap); if (rc) return rc;
+    rc = admit(c, cap, 1, 0, 0, n * WRAP_SCRATCH_BYTES, high_compression ? n : -1); if (rc) return rc;
+    rc = call_scratch(c, st, cap, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
     // the same encode as lz4b200_encode_batch(MEM_DEVICE): HC sizes its arena as if every block were above 64 KiB
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
-    rc = run_wrap(c, a, wrap_scratch_at(c->wrap_tmp.p, n), encode_op(high_compression != 0), st, -1); if (rc) return rc;
-    CU(cudaEventRecord(c->compact_done, st));
+    rc = run_wrap(c, a, wrap_scratch_at(c->wrap_tmp.p, n), encode_op(high_compression != 0), st, -1, cap); if (rc) return rc;
+    CU(c->compact_done.record(st, cap));
     return LZ4B200_OK;
 }
 
@@ -973,17 +1108,20 @@ int lz4b200_unwrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* 
     if (n == 0) return LZ4B200_OK;
     if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     cudaStream_t st = (cudaStream_t)stream;
-    int rc = call_scratch(c, st, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    Capture cap;
+    int rc = capture_of(st, &cap); if (rc) return rc;
+    rc = admit(c, cap, 1, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    rc = call_scratch(c, st, cap, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
     const WrapScratch w = wrap_scratch_at(c->wrap_tmp.p, n);
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
     cudaError_t e = launch_unwrap_prep(a, w, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "unwrap prep launch");
     // the compressed packets, known size (LZ4Codec.cs:595); stored and rejected ones are neutral entries
     const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, dst_off, w.cap, w.res, n};
-    rc = run_device(c, dec, Op::DECODE_KNOWN, st); if (rc) return rc;
+    rc = run_device(c, dec, Op::DECODE_KNOWN, st, 0, -1, cap); if (rc) return rc;
     e = launch_unwrap_finish(a, w, nullptr, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "unwrap finish launch");
-    CU(cudaEventRecord(c->compact_done, st));
+    CU(c->compact_done.record(st, cap));
     return LZ4B200_OK;
 }
 
@@ -996,9 +1134,13 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     CallGuard g(c); if (g.rc) return g.rc;
     if (!out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
     cudaStream_t st = (cudaStream_t)stream;
+    Capture cap;
+    int rc = capture_of(st, &cap); if (rc) return rc;
     if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    int rc = call_scratch(c, st, compact_tmp_bytes(n), sizeof(int32_t) * ((size_t)n + 1), n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    const size_t compact_bytes = compact_tmp_bytes(n), caps_bytes = sizeof(int32_t) * ((size_t)n + 1), wrap_bytes = n * WRAP_SCRATCH_BYTES;
+    rc = admit(c, cap, 1, compact_bytes, caps_bytes, wrap_bytes); if (rc) return rc;
+    rc = call_scratch(c, st, cap, compact_bytes, caps_bytes, wrap_bytes); if (rc) return rc;
     const WrapScratch w = wrap_scratch_at(c->wrap_tmp.p, n);
     int32_t* caps = (int32_t*)c->packed_caps.p;
     int* fits = (int*)(caps + n);
@@ -1008,11 +1150,11 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, 0, caps, fits, st, &c->launches);
     if (e == cudaSuccess) {
         const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, out_off, caps, w.res, n};
-        e = launch_decode(dec, true, c->pinned_lanes(), c->counter(), c->dev, st, &c->launches, fits);
+        e = launch_decode(dec, true, c->pinned_lanes(), c->counter(cap), c->dev, st, &c->launches, fits);
     }
     if (e == cudaSuccess) e = launch_unwrap_finish(a, w, fits, st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "packed unwrap launch");
-    CU(cudaEventRecord(c->compact_done, st));
+    CU(c->compact_done.record(st, cap));
     return LZ4B200_OK;
 }
 
@@ -1070,6 +1212,17 @@ int lz4b200_synth_fill(lz4b200_ctx* c, void* dst, int64_t n_blocks, int32_t bloc
     return LZ4B200_OK;
 }
 
+// Everything a device call of at most max_blocks blocks takes from the shared scratch, grown as an eager call grows it.
+int lz4b200_reserve(lz4b200_ctx* c, int32_t max_blocks, int high_compression)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (max_blocks < 0) return fail(LZ4B200_E_ARG, "negative block count");
+    if (max_blocks == 0) return LZ4B200_OK;
+    CallGuard g(c); if (g.rc) return g.rc;
+    return grow_scratch(c, compact_tmp_bytes(max_blocks), sizeof(int32_t) * ((size_t)max_blocks + 1), max_blocks * WRAP_SCRATCH_BYTES,
+                        high_compression ? hc_arena_bytes(c, max_blocks, -1) : 0);
+}
+
 int lz4b200_set_option(lz4b200_ctx* c, const char* key, int64_t value)
 {
     if (!c || !key) return fail(LZ4B200_E_ARG, "bad argument");
@@ -1093,7 +1246,7 @@ int lz4b200_set_option(lz4b200_ctx* c, const char* key, int64_t value)
         if (value < 32 || value > (1 << 20)) return fail(LZ4B200_E_ARG, "hc_concurrency out of range");
         DeviceGuard g(c->device);
         cudaDeviceSynchronize();
-        c->hc_arena.release();
+        c->hc_arena.drop(c->retired);
         c->hc_concurrency = (int)value;
     }
     else if (k == "hc_kernel") { if (value < -1 || value > 2) return fail(LZ4B200_E_ARG, "hc_kernel must be -1 (chosen per batch), 0 (thread per block), 1 or 2 (warp per block: blocks <= 64 KiB in shared memory / read through L1)"); c->hc_kernel = (int)value; }
