@@ -8,6 +8,8 @@
 // calls between device and host memory go through it too, skipping the copy of whichever side is already on the device;
 // so does the packed unknown-size decode from host into device memory, whose output offset is carried across the stages
 // on the device (lz4_packed.cuh).  What a stage runs is named by its caller (Stage); the codec operation by Op.
+// The device-memory calls enter through one path (DeviceCall): each states what it takes from the context (Need), which
+// admits it to a CUDA graph capture or grows an eager call's scratch; lz4b200_reserve grows to the same needs.
 // The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
 // caller's bytes are on; the host only reads headers (framing.cpp).  There is no CPU codec in this library: if the device
 // or the kernel image is unusable every entry point reports an error.
@@ -212,7 +214,7 @@ struct lz4b200_ctx {
     SharedBuf wrap_tmp;                    // the device Wrap / Unwrap calls: the codec's view of the packets (serialised like compact_tmp)
     std::vector<void*> retired;            // shared scratch a graph may still reference: freed by lz4b200_destroy
     Chain hc_done;                         // the HC state arena is shared: HC launches are chained through this event
-    Chain compact_done;                    // likewise compact_tmp, packed_caps and wrap_tmp (call_scratch)
+    Chain compact_done;                    // likewise compact_tmp, packed_caps and wrap_tmp (DeviceCall)
     cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
     int64_t* carry = nullptr;              // the packed decode into device memory: NSLOT cells, the running output offset behind each slot's stage
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
@@ -255,7 +257,7 @@ struct CallGuard {
         : lock(c->mu), dev(c->device), rc(dev.ok ? LZ4B200_OK : fail(LZ4B200_E_CUDA, "cudaSetDevice failed")) {}
 };
 
-// Whether `st` is capturing.  Every call that takes a stream asks this before any other work on it.
+// Whether `st` is capturing.  Every call that takes a stream asks this before it takes any scratch or synchronises.
 int capture_of(cudaStream_t st, Capture* cap)
 {
     cudaStreamCaptureStatus s = cudaStreamCaptureStatusNone;
@@ -273,55 +275,74 @@ int refuse_capture(void* stream, const char* what)
                   : LZ4B200_OK;
 }
 
-// The HC arena a device batch of n blocks needs (hc_large: blocks above 64 KiB, -1 = not known), under the current options.
-size_t hc_arena_bytes(const lz4b200_ctx* c, int32_t n, int32_t hc_large)
+// What a device call takes: counter sets of the capture pool when captured (0 or 1), and bytes of the scan scratch, the
+// packed calls' capacities + "fits" flag, the packet view and the HC arena.  need_of: a call family's need at n blocks
+// (pieces: the ones it uses), for the calls and lz4b200_reserve alike; the HC arena under the current options, for
+// hc_large blocks above 64 KiB (-1 = not known).
+struct Need { int counters = 0; size_t scan = 0, caps = 0, wrap = 0, hc = 0; };
+enum : unsigned { SCAN = 1, CAPS = 2, WRAP = 4, HC = 8 };
+Need need_of(const lz4b200_ctx* c, int32_t n, unsigned pieces, int counters, int32_t hc_large = -1)
 {
-    if (c->hc_kernel < 0) return hc_auto_scratch_bytes(n, hc_large, c->dev);
-    if (c->hc_kernel) return hcw_scratch_bytes(n, hc_large, c->hc_kernel, c->hc_warps_per_sm, c->dev);
-    return hc_scratch_bytes((int)std::min<int64_t>(c->hc_concurrency, std::max(n, 1)));
+    Need d{counters};
+    if (pieces & SCAN) d.scan = compact_tmp_bytes(n);
+    if (pieces & CAPS) d.caps = sizeof(int32_t) * ((size_t)n + 1);
+    if (pieces & WRAP) d.wrap = (size_t)n * WRAP_SCRATCH_BYTES;
+    if (pieces & HC)
+        d.hc = c->hc_kernel < 0 ? hc_auto_scratch_bytes(n, hc_large, c->dev)
+             : c->hc_kernel ? hcw_scratch_bytes(n, hc_large, c->hc_kernel, c->hc_warps_per_sm, c->dev)
+                            : hc_scratch_bytes((int)std::min<int64_t>(c->hc_concurrency, std::max(n, 1)));
+    return d;
 }
 
-// Grows the shared scratch to at least these sizes, behind one cudaDeviceSynchronize, since an earlier call may still be
-// using it.  Eager calls and lz4b200_reserve only.
-int grow_scratch(lz4b200_ctx* c, size_t compact_bytes, size_t caps_bytes, size_t wrap_bytes, size_t hc_bytes = 0)
+bool covers(const lz4b200_ctx* c, const Need& d)
 {
-    if (compact_bytes <= c->compact_tmp.cap && caps_bytes <= c->packed_caps.cap && wrap_bytes <= c->wrap_tmp.cap && hc_bytes <= c->hc_arena.cap)
-        return LZ4B200_OK;
+    return d.scan <= c->compact_tmp.cap && d.caps <= c->packed_caps.cap && d.wrap <= c->wrap_tmp.cap && d.hc <= c->hc_arena.cap;
+}
+
+// Grows the shared scratch to cover `d`, behind one cudaDeviceSynchronize, since an earlier call may still be using it.
+// Eager calls and lz4b200_reserve only.
+int grow_scratch(lz4b200_ctx* c, const Need& d)
+{
+    if (covers(c, d)) return LZ4B200_OK;
     CU(cudaDeviceSynchronize());
-    CU(c->compact_tmp.grow(compact_bytes, c->retired)); CU(c->packed_caps.grow(caps_bytes, c->retired));
-    CU(c->wrap_tmp.grow(wrap_bytes, c->retired)); CU(c->hc_arena.grow(hc_bytes, c->retired));
+    CU(c->compact_tmp.grow(d.scan, c->retired)); CU(c->packed_caps.grow(d.caps, c->retired));
+    CU(c->wrap_tmp.grow(d.wrap, c->retired)); CU(c->hc_arena.grow(d.hc, c->retired));
     return LZ4B200_OK;
 }
 
 // A captured call never allocates, frees or synchronises: it enqueues nothing unless the scratch it needs is already there
 // at its size (lz4b200_reserve grows it) and the capture pool has the counter sets it takes.  The buffers it references
-// are then held for the graph.  hc_blocks: the blocks of an HC encode inside the call (-1: none).  Eager calls pass.
-int admit(lz4b200_ctx* c, const Capture& cap, int counters, size_t compact_bytes, size_t caps_bytes = 0, size_t wrap_bytes = 0,
-          int32_t hc_blocks = -1)
+// are then held for the graph.
+int admit(lz4b200_ctx* c, const Need& d)
 {
-    if (!cap.on) return LZ4B200_OK;
-    const size_t hc_bytes = hc_blocks >= 0 ? hc_arena_bytes(c, hc_blocks, -1) : 0;
-    if (compact_bytes > c->compact_tmp.cap || caps_bytes > c->packed_caps.cap || wrap_bytes > c->wrap_tmp.cap || hc_bytes > c->hc_arena.cap)
+    if (!covers(c, d))
         return fail(LZ4B200_E_ARG, "the context's scratch is too small to capture this call: call lz4b200_reserve(ctx, n_blocks, "
                                    "high_compression) before capturing");
-    if (c->next_captured + counters > NCAPTURED)
+    if (c->next_captured + d.counters > NCAPTURED)
         return fail(LZ4B200_E_ARG, "the context's " + std::to_string(NCAPTURED) + " counter sets for captured calls are used up");
-    if (compact_bytes) c->compact_tmp.held = true;
-    if (caps_bytes) c->packed_caps.held = true;
-    if (wrap_bytes) c->wrap_tmp.held = true;
-    if (hc_blocks >= 0) c->hc_arena.held = true;
+    if (d.scan) c->compact_tmp.held = true;
+    if (d.caps) c->packed_caps.held = true;
+    if (d.wrap) c->wrap_tmp.held = true;
+    if (d.hc) c->hc_arena.held = true;
     return LZ4B200_OK;
 }
 
-// The context's call scratch (compact_tmp, packed_caps, wrap_tmp) is shared by the device calls on every stream.  A call
-// grows the buffers it needs to at least these sizes (an eager call: a captured one has been admitted at them) and orders
-// `st` behind the last call that used them.  The caller records compact_done on `st` once its launches are in.
-int call_scratch(lz4b200_ctx* c, cudaStream_t st, const Capture& cap, size_t compact_bytes, size_t caps_bytes = 0, size_t wrap_bytes = 0)
-{
-    if (!cap.on) { int rc = grow_scratch(c, compact_bytes, caps_bytes, wrap_bytes); if (rc) return rc; }
-    CU(c->compact_done.wait(st, cap));
-    return LZ4B200_OK;
-}
+// The way into every device-memory call, after its argument checks: the context's lock and device; then enter(need) admits
+// a captured call or grows an eager one's scratch and, if it takes call scratch (compact_tmp, packed_caps, wrap_tmp: shared
+// by the device calls on every stream), orders the stream behind the last such call.  Such a call closes with done() once
+// its launches are in; one that fails records nothing, so a failed captured call leaves no event node in the graph.
+struct DeviceCall : CallGuard {
+    lz4b200_ctx* c; cudaStream_t st; Capture cap;
+    DeviceCall(lz4b200_ctx* c, void* stream) : CallGuard(c), c(c), st((cudaStream_t)stream) {}
+    int enter(const Need& d)
+    {
+        int rc = capture_of(st, &cap); if (rc) return rc;
+        rc = cap.on ? admit(c, d) : grow_scratch(c, d); if (rc) return rc;
+        if (d.scan || d.caps || d.wrap) CU(c->compact_done.wait(st, cap));
+        return LZ4B200_OK;
+    }
+    int done() { CU(c->compact_done.record(st, cap)); return LZ4B200_OK; }
+};
 
 int launched(cudaError_t e, const char* what) { return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, what); }
 
@@ -346,7 +367,7 @@ int run_device(lz4b200_ctx* c, const BatchArgs& a, Op op, cudaStream_t st, int l
     case Op::ENCODE_FAST: e = launch_encode_fast(a, c->counter(cap), c->encode_ctas_per_sm, c->encode_tune, c->encode_variant, c->dev, st, &c->launches); break;
     case Op::ENCODE_HC: {
         const int conc = (int)std::min<int64_t>(c->hc_concurrency, std::max(a.n_blocks, 1));
-        if (!cap.on) { int rc = grow_scratch(c, 0, 0, 0, hc_arena_bytes(c, a.n_blocks, hc_large)); if (rc) return rc; }
+        if (!cap.on) { int rc = grow_scratch(c, need_of(c, a.n_blocks, HC, 0, hc_large)); if (rc) return rc; }
         // one arena per context: an HC launch may not overlap the previous one, whatever stream it was given
         CU(c->hc_done.wait(st, cap));
         uint32_t* counter = c->counter(cap);
@@ -373,6 +394,18 @@ int run_wrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, Op op, cu
     const BatchArgs enc{a.src, a.src_off, w.len, a.dst, w.off, w.cap, w.res, a.n_blocks};
     rc = run_device(c, enc, op, st, 0, hc_large, cap); if (rc) return rc;
     return launched(launch_wrap_finish(a, w, st, &c->launches), "wrap finish launch");
+}
+
+// The placement of the packed decodes (lz4_packed.cuh): n sizes scanned into the offsets `off`, then each block's capacity
+// (its size + room) and the "fits" flag.  A pipeline stage places behind the previous one (waits on `after`, starts from
+// `base`: null for the first stage) and leaves its absolute offsets and the running total (lz4_packed.cuh).
+cudaError_t place(lz4b200_ctx* c, const int32_t* size, int64_t* off, int32_t n, const DevBuf& scan, int64_t total_cap,
+                  int32_t room, int32_t* caps, int* fits, cudaStream_t st, cudaEvent_t after = nullptr,
+                  const int64_t* base = nullptr, int64_t* abs_off = nullptr, int64_t* total = nullptr)
+{
+    cudaError_t e = launch_compact(nullptr, nullptr, size, nullptr, off, n, scan.p, scan.cap, c->dev, st, &c->launches);
+    if (e == cudaSuccess && after) e = cudaStreamWaitEvent(st, after, 0);
+    return e == cudaSuccess ? launch_packed_prep(size, off, n, total_cap, room, caps, fits, st, &c->launches, base, abs_off, total) : e;
 }
 
 // Host-memory batch: chunks of at most host_chunk_bytes (src + dst bytes) go through the slots in turn, and a slot's
@@ -560,12 +593,10 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
             int* fits = (int*)d.off;
             BatchArgs sizes = a; sizes.dst_cap = nullptr;
             cudaError_t e = launch_measure(sizes, false, c->dev, sl.stream, &c->launches);
-            if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, d.out, nullptr, (int64_t*)sl.offs.p, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
-            if (e != cudaSuccess) return cuda_fail(e, "packed measure launch");
-            if (b0 > 0) CU(cudaStreamWaitEvent(sl.stream, c->slot[prev].carried, 0));
-            e = launch_packed_prep(d.out, (const int64_t*)sl.offs.p, m, dst_total_cap, PACKED_ROOM_UNKNOWN, d.dc, fits, sl.stream, &c->launches,
-                                   b0 > 0 ? c->carry + prev : nullptr, d.dof, c->carry + s);
-            if (e != cudaSuccess) return cuda_fail(e, "packed placement launch");
+            if (e == cudaSuccess) e = place(c, d.out, (int64_t*)sl.offs.p, m, sl.scan, dst_total_cap, PACKED_ROOM_UNKNOWN, d.dc, fits,
+                                            sl.stream, b0 > 0 ? c->slot[prev].carried : nullptr, b0 > 0 ? c->carry + prev : nullptr,
+                                            d.dof, c->carry + s);
+            if (e != cudaSuccess) return cuda_fail(e, "packed measure / placement launch");
             CU(cudaEventRecord(sl.carried, sl.stream));
             e = launch_decode(a, false, c->pinned_lanes(), c->counter(), c->dev, sl.stream, &c->launches, fits);
             if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
@@ -638,14 +669,13 @@ int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t
     const bool measure = is_measure(op);
     if (!src_off || !src_len || !out_len || !src || (!measure && (!(dst_off || out_off) || !dst_cap || !dst)))
         return fail(LZ4B200_E_ARG, "null argument");
-    CallGuard g(c); if (g.rc) return g.rc;
     if (mem == LZ4B200_MEM_DEVICE) {
-        Capture cap;
-        int rc = capture_of((cudaStream_t)stream, &cap); if (rc) return rc;
-        rc = admit(c, cap, measure ? 0 : 1, 0, 0, 0, op == Op::ENCODE_HC ? n : -1); if (rc) return rc;
+        DeviceCall call(c, stream); if (call.rc) return call.rc;
+        int rc = call.enter(need_of(c, n, op == Op::ENCODE_HC ? HC : 0, measure ? 0 : 1)); if (rc) return rc;
         BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
-        return run_device(c, a, op, (cudaStream_t)stream, 0, -1, cap);
+        return run_device(c, a, op, call.st, 0, -1, call.cap);
     }
+    CallGuard g(c); if (g.rc) return g.rc;
     const bool src_dev = mem == LZ4B200_MEM_DEVICE_TO_HOST, dst_dev = mem == LZ4B200_MEM_HOST_TO_DEVICE;
     if (mem != LZ4B200_MEM_HOST && !src_dev && !dst_dev)
         return fail(LZ4B200_E_ARG, "mem must be LZ4B200_MEM_HOST, _DEVICE, _DEVICE_TO_HOST or _HOST_TO_DEVICE");
@@ -1019,28 +1049,21 @@ int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
 {
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    CallGuard g(c); if (g.rc) return g.rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    Capture cap;
-    int rc = capture_of(st, &cap); if (rc) return rc;
-    if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
+    DeviceCall call(c, stream); if (call.rc) return call.rc;
+    if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), call.st)); return LZ4B200_OK; }     // out_off[0] = total = 0
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    const size_t compact_bytes = compact_tmp_bytes(n), caps_bytes = sizeof(int32_t) * ((size_t)n + 1);
-    rc = admit(c, cap, 1, compact_bytes, caps_bytes); if (rc) return rc;
-    rc = call_scratch(c, st, cap, compact_bytes, caps_bytes); if (rc) return rc;
+    int rc = call.enter(need_of(c, n, SCAN | CAPS, 1)); if (rc) return rc;
     int32_t* caps = (int32_t*)c->packed_caps.p;
     int* fits = (int*)(caps + n);
     const BatchArgs m{(const uint8_t*)src, src_off, src_len, nullptr, nullptr, nullptr, out_len, n};
-    cudaError_t e = launch_measure(m, false, c->dev, st, &c->launches);
-    if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, out_len, nullptr, out_off, n, c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
-    if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, PACKED_ROOM_UNKNOWN, caps, fits, st, &c->launches);
+    cudaError_t e = launch_measure(m, false, c->dev, call.st, &c->launches);
+    if (e == cudaSuccess) e = place(c, out_len, out_off, n, c->compact_tmp, dst_total_cap, PACKED_ROOM_UNKNOWN, caps, fits, call.st);
     if (e == cudaSuccess) {
         const BatchArgs d{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, caps, out_len, n};
-        e = launch_decode(d, false, c->pinned_lanes(), c->counter(cap), c->dev, st, &c->launches, fits);
+        e = launch_decode(d, false, c->pinned_lanes(), c->counter(call.cap), c->dev, call.st, &c->launches, fits);
     }
     if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
-    CU(c->compact_done.record(st, cap));
-    return LZ4B200_OK;
+    return call.done();
 }
 
 // The same from host memory, through the pipeline (run_host): the sizes stay on the device, a stage at a time.
@@ -1064,18 +1087,13 @@ int lz4b200_compact(lz4b200_ctx* c, const void* slots, const int64_t* slot_off, 
                     int64_t* out_off, int32_t n, void* stream)
 {
     if (!c || !slot_off || !len || !out_off || n < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    CallGuard g(c); if (g.rc) return g.rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    Capture cap;
-    int rc = capture_of(st, &cap); if (rc) return rc;
-    if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
-    rc = admit(c, cap, 0, compact_tmp_bytes(n)); if (rc) return rc;
-    rc = call_scratch(c, st, cap, compact_tmp_bytes(n)); if (rc) return rc;
+    DeviceCall call(c, stream); if (call.rc) return call.rc;
+    if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), call.st)); return LZ4B200_OK; }     // out_off[0] = total = 0
+    int rc = call.enter(need_of(c, n, SCAN, 0)); if (rc) return rc;
     cudaError_t e = launch_compact((const uint8_t*)slots, slot_off, len, (uint8_t*)packed, out_off, n,
-                                   c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
+                                   c->compact_tmp.p, c->compact_tmp.cap, c->dev, call.st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "compact launch");
-    CU(c->compact_done.record(st, cap));
-    return LZ4B200_OK;
+    return call.done();
 }
 
 // ---- Wrap / Unwrap packets in device memory (lz4_wrap.cuh): prep -> the batch codec, unchanged -> finish, on `stream` ----
@@ -1084,19 +1102,14 @@ int lz4b200_wrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* sr
 {
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
-    CallGuard g(c); if (g.rc) return g.rc;
+    DeviceCall call(c, stream); if (call.rc) return call.rc;
     if (n == 0) return LZ4B200_OK;
     if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    cudaStream_t st = (cudaStream_t)stream;
-    Capture cap;
-    int rc = capture_of(st, &cap); if (rc) return rc;
-    rc = admit(c, cap, 1, 0, 0, n * WRAP_SCRATCH_BYTES, high_compression ? n : -1); if (rc) return rc;
-    rc = call_scratch(c, st, cap, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    int rc = call.enter(need_of(c, n, WRAP | (high_compression ? HC : 0), 1)); if (rc) return rc;
     // the same encode as lz4b200_encode_batch(MEM_DEVICE): HC sizes its arena as if every block were above 64 KiB
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
-    rc = run_wrap(c, a, wrap_scratch_at(c->wrap_tmp.p, n), encode_op(high_compression != 0), st, -1, cap); if (rc) return rc;
-    CU(c->compact_done.record(st, cap));
-    return LZ4B200_OK;
+    rc = run_wrap(c, a, wrap_scratch_at(c->wrap_tmp.p, n), encode_op(high_compression != 0), call.st, -1, call.cap); if (rc) return rc;
+    return call.done();
 }
 
 int lz4b200_unwrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
@@ -1104,25 +1117,18 @@ int lz4b200_unwrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* 
 {
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
-    CallGuard g(c); if (g.rc) return g.rc;
+    DeviceCall call(c, stream); if (call.rc) return call.rc;
     if (n == 0) return LZ4B200_OK;
     if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    cudaStream_t st = (cudaStream_t)stream;
-    Capture cap;
-    int rc = capture_of(st, &cap); if (rc) return rc;
-    rc = admit(c, cap, 1, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
-    rc = call_scratch(c, st, cap, 0, 0, n * WRAP_SCRATCH_BYTES); if (rc) return rc;
+    int rc = call.enter(need_of(c, n, WRAP, 1)); if (rc) return rc;
     const WrapScratch w = wrap_scratch_at(c->wrap_tmp.p, n);
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
-    cudaError_t e = launch_unwrap_prep(a, w, st, &c->launches);
-    if (e != cudaSuccess) return cuda_fail(e, "unwrap prep launch");
+    rc = launched(launch_unwrap_prep(a, w, call.st, &c->launches), "unwrap prep launch"); if (rc) return rc;
     // the compressed packets, known size (LZ4Codec.cs:595); stored and rejected ones are neutral entries
     const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, dst_off, w.cap, w.res, n};
-    rc = run_device(c, dec, Op::DECODE_KNOWN, st, 0, -1, cap); if (rc) return rc;
-    e = launch_unwrap_finish(a, w, nullptr, st, &c->launches);
-    if (e != cudaSuccess) return cuda_fail(e, "unwrap finish launch");
-    CU(c->compact_done.record(st, cap));
-    return LZ4B200_OK;
+    rc = run_device(c, dec, Op::DECODE_KNOWN, call.st, 0, -1, call.cap); if (rc) return rc;
+    rc = launched(launch_unwrap_finish(a, w, nullptr, call.st, &c->launches), "unwrap finish launch"); if (rc) return rc;
+    return call.done();
 }
 
 // sizes from the headers -> scan into out_off -> capacities + "fits" -> decode and stored copies, both behind the flag
@@ -1131,31 +1137,24 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
 {
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
-    CallGuard g(c); if (g.rc) return g.rc;
+    DeviceCall call(c, stream); if (call.rc) return call.rc;
     if (!out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    cudaStream_t st = (cudaStream_t)stream;
-    Capture cap;
-    int rc = capture_of(st, &cap); if (rc) return rc;
-    if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }     // out_off[0] = total = 0
+    if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), call.st)); return LZ4B200_OK; }     // out_off[0] = total = 0
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
-    const size_t compact_bytes = compact_tmp_bytes(n), caps_bytes = sizeof(int32_t) * ((size_t)n + 1), wrap_bytes = n * WRAP_SCRATCH_BYTES;
-    rc = admit(c, cap, 1, compact_bytes, caps_bytes, wrap_bytes); if (rc) return rc;
-    rc = call_scratch(c, st, cap, compact_bytes, caps_bytes, wrap_bytes); if (rc) return rc;
+    int rc = call.enter(need_of(c, n, SCAN | CAPS | WRAP, 1)); if (rc) return rc;
     const WrapScratch w = wrap_scratch_at(c->wrap_tmp.p, n);
     int32_t* caps = (int32_t*)c->packed_caps.p;
     int* fits = (int*)(caps + n);
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, nullptr, out_len, n};
-    cudaError_t e = launch_unwrap_prep(a, w, st, &c->launches);
-    if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, out_len, nullptr, out_off, n, c->compact_tmp.p, c->compact_tmp.cap, c->dev, st, &c->launches);
-    if (e == cudaSuccess) e = launch_packed_prep(out_len, out_off, n, dst_total_cap, 0, caps, fits, st, &c->launches);
+    cudaError_t e = launch_unwrap_prep(a, w, call.st, &c->launches);
+    if (e == cudaSuccess) e = place(c, out_len, out_off, n, c->compact_tmp, dst_total_cap, 0, caps, fits, call.st);
     if (e == cudaSuccess) {
         const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, out_off, caps, w.res, n};
-        e = launch_decode(dec, true, c->pinned_lanes(), c->counter(cap), c->dev, st, &c->launches, fits);
+        e = launch_decode(dec, true, c->pinned_lanes(), c->counter(call.cap), c->dev, call.st, &c->launches, fits);
     }
-    if (e == cudaSuccess) e = launch_unwrap_finish(a, w, fits, st, &c->launches);
+    if (e == cudaSuccess) e = launch_unwrap_finish(a, w, fits, call.st, &c->launches);
     if (e != cudaSuccess) return cuda_fail(e, "packed unwrap launch");
-    CU(c->compact_done.record(st, cap));
-    return LZ4B200_OK;
+    return call.done();
 }
 
 // ---- Wrap / Unwrap packets with a side in host memory: the host pipeline (run_host, WRAP_ENCODE / FRAMED_DECODE) ----
@@ -1219,8 +1218,7 @@ int lz4b200_reserve(lz4b200_ctx* c, int32_t max_blocks, int high_compression)
     if (max_blocks < 0) return fail(LZ4B200_E_ARG, "negative block count");
     if (max_blocks == 0) return LZ4B200_OK;
     CallGuard g(c); if (g.rc) return g.rc;
-    return grow_scratch(c, compact_tmp_bytes(max_blocks), sizeof(int32_t) * ((size_t)max_blocks + 1), max_blocks * WRAP_SCRATCH_BYTES,
-                        high_compression ? hc_arena_bytes(c, max_blocks, -1) : 0);
+    return grow_scratch(c, need_of(c, max_blocks, SCAN | CAPS | WRAP | (high_compression ? HC : 0), 0));
 }
 
 int lz4b200_set_option(lz4b200_ctx* c, const char* key, int64_t value)
