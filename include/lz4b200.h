@@ -158,6 +158,42 @@ int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* ctx,
                                             const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off,
                                             int32_t* out_len, int32_t n_blocks, int mode, void* stream);
 
+/* ---- offload without blocking: device memory <-> page-locked host memory, asynchronous on `stream` ------------------
+ * The two calls below do what lz4b200_encode_batch_packed_from_device and lz4b200_decode_batch(LZ4B200_MEM_HOST_TO_DEVICE)
+ * do -- the same out_len, offsets and bytes -- but only ENQUEUE their work on `stream` and return without waiting for any
+ * device work: the thread that launches a model's kernels can offload a cache to host RAM, or prefetch it back, and keep
+ * launching while the transfer runs.
+ *   - Ordering: the call's device work runs after everything enqueued on `stream` before the call, and anything enqueued on
+ *     `stream` after it sees all of its results.  Calls of one context are ordered among themselves on any streams.
+ *   - Lifetime: the caller keeps src, dst, out_off and out_len alive and untouched until `stream` has passed the call (a
+ *     cudaStreamSynchronize, or an event recorded behind it).  The offset, length and capacity arrays are host arrays
+ *     read during the call only.
+ *   - The host side is page-locked memory the device can address: cudaHostAlloc / cudaMallocHost, torch pin_memory(), or a
+ *     lz4b200_host_register'd range.  Pageable memory, device memory, or memory without a device address there is
+ *     LZ4B200_E_ARG.  out_off / out_len may be device memory of the context's GPU or page-locked host memory.
+ *   - LZ4B200_E_ARG for a NULL argument, a negative length or memory of the wrong kind, before any device work.  A stream
+ *     that is capturing a CUDA graph is LZ4B200_E_ARG before any CUDA work; the capture stays valid.
+ *   - Never a wait on device work, except once when the context's buffers for these calls (or its HC arena) must grow: a
+ *     call that needs no more than an earlier call of the same context never waits.
+ *
+ * encode_batch_packed_from_device_async: src is device memory of the context's GPU; dst is page-locked host memory.
+ *   out_len[i] and out_off[0..n] (n_blocks+1 entries, out_off[n] the total) are written by the device and equal what
+ *   lz4b200_encode_batch_packed_from_device gives for the same arguments; if out_off[n] <= dst_total_cap, dst[0, out_off[n])
+ *   holds the same bytes.  A destination too small is still LZ4B200_OK (the total is known only on the device): out_off and
+ *   out_len are filled, nothing outside [dst, dst + dst_total_cap) is written and the bytes inside it are unspecified, as in
+ *   lz4b200_decode_batch_packed_to_device; the caller sees out_off[n] > dst_total_cap after synchronising.  n_blocks == 0 is
+ *   LZ4B200_OK with out_off[0] = 0 written on the stream. */
+int lz4b200_encode_batch_packed_from_device_async(lz4b200_ctx* ctx, const void* src, const int64_t* src_off,
+                                                  const int32_t* src_len, const int32_t* dst_cap, void* dst,
+                                                  int64_t dst_total_cap, int64_t* out_off, int32_t* out_len,
+                                                  int32_t n_blocks, int mode, void* stream);
+/* decode_batch_to_device_async: lz4b200_decode_batch(..., known_len, LZ4B200_MEM_HOST_TO_DEVICE, stream) without blocking.
+ *   src is page-locked host memory; dst is device memory of the context's GPU.  out_len[i] and the bytes written equal what
+ *   the synchronous call gives; nothing is written outside [dst_off[i], dst_off[i] + dst_cap[i]). */
+int lz4b200_decode_batch_to_device_async(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                         void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len,
+                                         int32_t n_blocks, int known_len, void* stream);
+
 /* Compaction of fixed-stride encoder slots into one contiguous payload (device memory only): the batched form of
  * the Buffer.BlockCopy trim in LZ4Codec.Encode (src/LZ4/LZ4Codec.cs:357-364).  out_off[i] (int64, n_blocks+1
  * entries) = exclusive prefix sum of max(len[i],0); block i's bytes are copied to packed + out_off[i]. */
@@ -186,7 +222,9 @@ int lz4b200_compact(lz4b200_ctx* ctx, const void* slots, const int64_t* slot_off
  *   - lz4b200_launch_count counts the launches a call enqueues when it is captured, not replays.
  * Every other call that takes a `stream` synchronises with the host (the mixed-memory batches, the packed encode from
  * and decode to device memory, the LZ4Stream and the Wrap / Unwrap calls between device and host memory): on a capturing
- * stream it returns LZ4B200_E_ARG before any CUDA work, and the capture stays valid.  lz4b200_peer_copy is not covered.
+ * stream it returns LZ4B200_E_ARG before any CUDA work, and the capture stays valid.  So do
+ * lz4b200_encode_batch_packed_from_device_async and lz4b200_decode_batch_to_device_async, which do not synchronise but
+ * hand the device host metadata that a graph would have to keep alive.  lz4b200_peer_copy is not covered.
  * The calls without a stream (host-memory batches, single-block functions, lz4b200_synchronize, lz4b200_reserve) use
  * the legacy default stream or synchronise the device: they must not be made while any thread of the process captures
  * in cudaStreamCaptureModeGlobal.

@@ -76,6 +76,25 @@ public:
             throw std::runtime_error(lz4b200_last_error());
         return out;
     }
+    // Offload without blocking: blocks of device memory encoded back to back into page-locked host memory, and blocks of
+    // page-locked host memory decoded into device memory (lz4b200_encode_batch_packed_from_device_async,
+    // lz4b200_decode_batch_to_device_async).  Enqueued on `stream`, they return at once; src, dst, out_off and out_len stay
+    // the caller's, alive and untouched, until the stream has passed the call.
+    void encode_packed_to_host_async(const void* src, const int64_t* src_off, const int32_t* src_len, const int32_t* dst_cap,
+                                     void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
+                                     bool hc, void* stream)
+    {
+        if (lz4b200_encode_batch_packed_from_device_async(h_, src, src_off, src_len, dst_cap, dst, dst_total_cap, out_off, out_len, n,
+                                                          hc ? LZ4B200_MODE_HC : LZ4B200_MODE_FAST, stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
+    void decode_from_host_async(const void* src, const int64_t* src_off, const int32_t* src_len, void* dst, const int64_t* dst_off,
+                                const int32_t* dst_cap, int32_t* out_len, int32_t n, bool known, void* stream)
+    {
+        if (lz4b200_decode_batch_to_device_async(h_, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, known ? 1 : 0,
+                                                 stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
 private:
     lz4b200_ctx* h_ = nullptr;
 };

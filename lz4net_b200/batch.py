@@ -27,6 +27,10 @@ with new contents in the same tensors:
 
 A call whose scratch was not reserved raises Lz4B200Error (E_ARG) and leaves the capture valid.  The synchronous helpers
 refuse a capturing stream the same way.
+
+encode_to_host_packed_async and decode_from_host_async move blocks between a device tensor and a page-locked CPU tensor
+without blocking the calling thread: they enqueue their work on a stream and return, so a thread that launches a model's
+kernels can offload to host RAM, or prefetch back, and keep launching.  They refuse a capturing stream.
 """
 from __future__ import annotations
 
@@ -174,6 +178,54 @@ def decode_from_host_packed(ctx: Context, comp: np.ndarray, src_off, src_len, ou
         ctx.handle, _h(comp, np.uint8), _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), out.nbytes, off, res, n,
         _stream()), "decode_batch_packed_to_device")
     return int(out_off[n])
+
+
+def _pinned(t: torch.Tensor, dtype, n: int, what: str, device_ok: bool = False) -> int:
+    """Address of a contiguous tensor of this dtype and at least n items that the device reaches after the call has
+    returned: page-locked CPU memory, or with device_ok a CUDA tensor.  An empty tensor where none is needed is not read."""
+    if n == 0 and isinstance(t, torch.Tensor) and t.numel() == 0:
+        return t.data_ptr()
+    if not (isinstance(t, torch.Tensor) and t.dtype == dtype and t.is_contiguous() and t.numel() >= n):
+        raise TypeError(f"{what}: expected a contiguous torch {dtype} tensor of at least {n} items")
+    if not ((device_ok and t.is_cuda) or (t.device.type == "cpu" and t.is_pinned())):
+        raise TypeError(f"{what}: expected a page-locked CPU tensor (pin_memory())" + (" or a CUDA tensor" if device_ok else ""))
+    return t.data_ptr()
+
+
+def _stream_of(stream) -> int:
+    return stream.cuda_stream if stream is not None else _stream()
+
+
+def encode_to_host_packed_async(ctx: Context, raw: torch.Tensor, src_off, src_len, dst_cap, dst: torch.Tensor, out_off: torch.Tensor,
+                                out_len: torch.Tensor, hc: bool = False, stream=None):
+    """encode_to_host_packed without blocking (lz4b200_encode_batch_packed_from_device_async): block i of raw + src_off[i] is
+    encoded and its bytes land at dst + out_off[i], back to back, out_off[n] = the total.  dst is a page-locked CPU uint8
+    tensor; out_off (int64[n+1]) and out_len (int32[n]) are CUDA or page-locked CPU tensors, written by the device;
+    src_off / src_len / dst_cap are numpy arrays, read during the call.  Enqueued on `stream` (default: the current torch
+    stream) behind the work already there; returns at once.  The caller keeps raw, dst, out_off and out_len alive and
+    untouched until the stream has passed the call.  When the total exceeds dst.numel() the call still succeeds: out_off and
+    out_len are filled and the bytes of dst are unspecified; check out_off[n] after synchronising."""
+    n = len(src_off)
+    d, off, res = (_pinned(dst, torch.uint8, 0, "dst"), _pinned(out_off, torch.int64, n + 1, "out_off", True),
+                   _pinned(out_len, torch.int32, n, "out_len", True))
+    native.check(native.lib().lz4b200_encode_batch_packed_from_device_async(
+        ctx.handle, _d(raw), _h(src_off, np.int64), _h(src_len, np.int32, n), _h(dst_cap, np.int32, n), d, dst.numel(), off, res,
+        n, native.MODE_HC if hc else native.MODE_FAST, _stream_of(stream)), "encode_batch_packed_from_device_async")
+
+
+def decode_from_host_async(ctx: Context, comp: torch.Tensor, src_off, src_len, out: torch.Tensor, dst_off, dst_cap,
+                           out_len: torch.Tensor, known: bool = True, stream=None):
+    """decode_from_host without blocking (lz4b200_decode_batch_to_device_async): block i of comp + src_off[i] is decoded in
+    place at out + dst_off[i], nothing written outside its dst_cap[i] bytes.  comp is a page-locked CPU uint8 tensor;
+    out_len (int32[n]) a CUDA or page-locked CPU tensor, written by the device; src_off / src_len / dst_off / dst_cap are
+    numpy arrays, read during the call.  Enqueued on `stream` (default: the current torch stream) behind the work already
+    there; returns at once.  The caller keeps comp, out and out_len alive and untouched until the stream has passed the
+    call."""
+    n = len(src_off)
+    c, res = _pinned(comp, torch.uint8, 0, "comp"), _pinned(out_len, torch.int32, n, "out_len", True)
+    native.check(native.lib().lz4b200_decode_batch_to_device_async(
+        ctx.handle, c, _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), _h(dst_off, np.int64, n), _h(dst_cap, np.int32, n),
+        res, n, int(known), _stream_of(stream)), "decode_batch_to_device_async")
 
 
 def wrap_to_host(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, out_len, hc: bool = False):

@@ -8,6 +8,9 @@
 // calls between device and host memory go through it too, skipping the copy of whichever side is already on the device;
 // so does the packed unknown-size decode from host into device memory, whose output offset is carried across the stages
 // on the device (lz4_packed.cuh).  What a stage runs is named by its caller (Stage); the codec operation by Op.
+// The asynchronous packed encode into page-locked host memory and decode from it (run_async) cut their stages by the same
+// plan, enqueue them on streams and buffers of their own and return without waiting; the encode's stages land in host
+// memory from a kernel (lz4_land.cuh), since where a stage lands is known only on the device.
 // The device-memory calls enter through one path (DeviceCall): each states what it takes from the context (Need), which
 // admits it to a CUDA graph capture or grows an eager call's scratch; lz4b200_reserve grows to the same needs.
 // The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
@@ -26,6 +29,7 @@
 #include <cstdio>
 #include <cstring>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -160,6 +164,20 @@ struct Slot {
     PinBuf hmeta, hsrc, hout;              // pinned: chunk metadata, staged pageable sources, staged outputs
 };
 
+// The stages of the asynchronous calls (run_async) go through buffers and streams of their own: a synchronous call drains
+// the slots above before it returns, and an asynchronous stage may still be in flight then.  Two, so that one stage's
+// transfer overlaps the next one's kernels.
+constexpr int NASYNC = 2;
+struct AsyncSlot {
+    cudaStream_t stream = nullptr;
+    cudaEvent_t done = nullptr;            // the slot's last stage of the call is enqueued (the caller's stream joins it)
+    cudaEvent_t carried = nullptr;         // the encode: the stage's landing step, which leaves the running total, is enqueued
+    DevBuf io, meta, offs, scan;           // io: the encode's dense output slots, or the decode's staged source
+};
+// The page-locked metadata of one asynchronous call, which the device reads after the call has returned: taken again once
+// `done`, recorded behind the call, has fired.
+struct MetaBlock { PinBuf buf; cudaEvent_t done = nullptr; bool used = false; };
+
 // One chunk's metadata, laid out the same in the slot's hmeta (host) and meta (device, which has no packed_off):
 // int64 src_off[m] | int64 dst_off[m] | int32 src_len[m] | int32 dst_cap[m] | int32 aux[m] | int32 out_len[m] |
 // int64 packed_off[m+1].  aux is used by the LZ4Stream and Unwrap calls only: the frame sizes of an encode (written on the
@@ -215,8 +233,10 @@ struct lz4b200_ctx {
     std::vector<void*> retired;            // shared scratch a graph may still reference: freed by lz4b200_destroy
     Chain hc_done;                         // the HC state arena is shared: HC launches are chained through this event
     Chain compact_done;                    // likewise compact_tmp, packed_caps and wrap_tmp (DeviceCall)
+    Chain async_done;                      // likewise the asynchronous calls' stage buffers, carry cells and streams (run_async)
     cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
-    int64_t* carry = nullptr;              // the packed decode into device memory: NSLOT cells, the running output offset behind each slot's stage
+    int64_t* carry = nullptr;              // the running output offset behind each slot's stage: NSLOT cells for the packed decode into device
+                                           // memory, then NASYNC for the asynchronous packed encode
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
     bool decode_lanes_auto = true;         // host-memory batches: chosen per chunk from the compression ratio
     int encode_ctas_per_sm = 0;            // encoder warps (= blocks in flight) per SM: 0 = as many as shared memory holds tables for (14)
@@ -227,6 +247,8 @@ struct lz4b200_ctx {
     int hc_kernel = -1;                  // -1: chosen per batch (encode.cu launch_encode_hc_auto); 0: one thread per block (any block size); one warp per block (on a static index for blocks <= 64 KiB, over a sliding 64 KiB window above; what neither describes goes to 0): 1 = block <= 64 KiB staged in shared memory, 2 = nothing in shared memory
     int hc_warps_per_sm = 0;             // warp kernels: blocks in flight per SM (0 = 3 for kernel 1, 32 for kernel 2)
     Slot slot[NSLOT];
+    AsyncSlot aslot[NASYNC];
+    std::vector<std::unique_ptr<MetaBlock>> meta_pool;    // the asynchronous calls' metadata (take_meta)
     int64_t launches = 0;
     std::mutex mu;
 
@@ -408,6 +430,71 @@ cudaError_t place(lz4b200_ctx* c, const int32_t* size, int64_t* off, int32_t n, 
     return e == cudaSuccess ? launch_packed_prep(size, off, n, total_cap, room, caps, fits, st, &c->launches, base, abs_off, total) : e;
 }
 
+// ---- the stage plan of the host pipeline, shared by run_host and the asynchronous calls (run_async) ------------------
+// A stage [b0, b1) is weighed by the bytes it stages: src_len[i] when count_src, plus dst_cap[i] when dst_cap is given
+// (not for a destination already on the device, nor for the measure pass).  Blocks join it while it stays within
+// host_chunk_bytes; it takes at least one.
+int32_t stage_end(const lz4b200_ctx* c, const int32_t* src_len, const int32_t* dst_cap, int32_t b0, int32_t n, bool count_src)
+{
+    int64_t bytes = 0; int32_t b1 = b0;
+    while (b1 < n) {
+        const int64_t w = (count_src ? (int64_t)src_len[b1] : 0) + (dst_cap ? dst_cap[b1] : 0);
+        if (b1 > b0 && bytes + w > (int64_t)c->host_chunk_bytes) break;
+        bytes += w; b1++;
+    }
+    return b1;
+}
+
+// Host bytes of a stage's Meta of m blocks (packed_off included).
+size_t meta_host_bytes(int32_t m) { return (size_t)m * META_BYTES + sizeof(int64_t) * (size_t)(m + 2); }
+
+// What fill_stage leaves besides the metadata: the source range the stage stages, [slo, shi) (0, 0 when the source is on
+// the device), and the bytes of its dense output slots (0 when the destination is).
+struct StageSpan { int64_t slo = 0, shi = 0, dsum = 0; };
+
+// The stage's metadata in h: source offsets relative to the staged range, destination offsets (dense slots, or the
+// caller's own when the destination is on the device; 0 for a placed decode, which places on the device), lengths and
+// capacities; a framed decode's stored entries (stored != null) become neutral, their lengths in aux.
+StageSpan fill_stage(const Meta& h, int32_t b0, int32_t b1, const int64_t* src_off, const int32_t* src_len, const int64_t* dst_off,
+                     const int32_t* dst_cap, bool src_dev, bool dst_dev, bool measure, bool placed, const uint8_t* stored)
+{
+    StageSpan sp;
+    const int32_t m = b1 - b0;
+    if (!src_dev) {
+        sp.slo = INT64_MAX; sp.shi = INT64_MIN;
+        for (int32_t i = b0; i < b1; i++) { sp.slo = std::min(sp.slo, src_off[i]); sp.shi = std::max(sp.shi, src_off[i] + src_len[i]); }
+    }
+    for (int32_t i = 0; i < m; i++) {
+        h.so[i] = src_off[b0 + i] - sp.slo;
+        if (dst_dev) h.dof[i] = placed ? 0 : dst_off[b0 + i];
+        else { h.dof[i] = sp.dsum; sp.dsum += measure ? 0 : dst_cap[b0 + i]; }
+        h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap ? dst_cap[b0 + i] : INT32_MAX;
+        if (stored) {
+            const bool st = stored[b0 + i] != 0;
+            h.aux[i] = st ? h.sl[i] : 0;
+            if (st) h.sl[i] = h.dc[i] = 0;
+        }
+    }
+    return sp;
+}
+
+// The decoder of a decode stage, from its compression ratio (0: the context's pinned choice, or not a decode).
+int stage_lanes(const lz4b200_ctx* c, Op op, const int32_t* src_len, const int32_t* dst_cap, int32_t b0, int32_t b1)
+{
+    if (!is_decode(op) || !c->decode_lanes_auto) return 0;
+    double cs = 0, rs = 0;
+    for (int32_t i = b0; i < b1; i++) { cs += src_len[i]; rs += dst_cap[i]; }
+    return lanes_for_ratio(rs > 0 ? cs / rs : 1.0, b1 - b0, c->dev);
+}
+
+// The blocks above 64 KiB of an HC encode stage (they size the HC arena).
+int32_t stage_hc_large(Op op, const int32_t* src_len, int32_t b0, int32_t b1)
+{
+    int32_t k = 0;
+    if (op == Op::ENCODE_HC) for (int32_t i = b0; i < b1; i++) k += src_len[i] > 65536;
+    return k;
+}
+
 // Host-memory batch: chunks of at most host_chunk_bytes (src + dst bytes) go through the slots in turn, and a slot's
 // outputs land in the caller's memory when the slot comes round again, so chunks overlap and land in block order.  On the
 // device the output slots of a chunk are dense: block i starts at the sum of dst_cap over the earlier blocks of its
@@ -523,38 +610,19 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
     };
 
     while (b0 < n) {
-        // ---- pick the chunk [b0, b1): bounded staged src + dst bytes ----
-        int64_t bytes = 0; int32_t b1 = b0;
-        while (b1 < n) {
-            const int64_t w = (src_dev ? 0 : (int64_t)src_len[b1]) + (measure || dst_dev ? 0 : dst_cap[b1]);
-            if (b1 > b0 && bytes + w > (int64_t)c->host_chunk_bytes) break;
-            bytes += w; b1++;
-        }
+        const int32_t b1 = stage_end(c, src_len, measure || dst_dev ? nullptr : dst_cap, b0, n, !src_dev);
         const int s = k % NSLOT; k++;
         int rc = retire(s); if (rc) return rc;
         Slot& sl = c->slot[s];
         const int32_t m = b1 - b0;
         const Mode mode = measure || dst_dev ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == Op::DECODE_KNOWN ? RUNS : SCATTER;
         CU(sl.meta.reserve((size_t)m * (kind == Stage::WRAP_ENCODE ? WRAP_META_BYTES : META_BYTES) + (placed ? sizeof(int64_t) : 0)));
-        CU(sl.hmeta.reserve((size_t)m * META_BYTES + sizeof(int64_t) * (size_t)(m + 2)));
+        CU(sl.hmeta.reserve(meta_host_bytes(m)));
         const Meta h(sl.hmeta.p, m), d(sl.meta.p, m);
-        int64_t slo = 0, shi = 0, dsum = 0;
-        if (!src_dev) {
-            slo = INT64_MAX; shi = INT64_MIN;
-            for (int32_t i = b0; i < b1; i++) { slo = std::min(slo, src_off[i]); shi = std::max(shi, src_off[i] + src_len[i]); }
-        }
-        for (int32_t i = 0; i < m; i++) {
-            h.so[i] = src_off[b0 + i] - slo;
-            if (dst_dev) h.dof[i] = placed ? 0 : dst_off[b0 + i];
-            else { h.dof[i] = dsum; dsum += measure ? 0 : dst_cap[b0 + i]; }
-            h.sl[i] = src_len[b0 + i]; h.dc[i] = dst_cap ? dst_cap[b0 + i] : INT32_MAX;
-            if (framed) {
-                const bool st = stored[b0 + i] != 0;
-                h.aux[i] = st ? h.sl[i] : 0;
-                if (st) h.sl[i] = h.dc[i] = 0;
-            }
-        }
-        const size_t sbytes = (size_t)(shi - slo);
+        const StageSpan sp = fill_stage(h, b0, b1, src_off, src_len, dst_off, dst_cap, src_dev, dst_dev, measure, placed,
+                                        framed ? stored : nullptr);
+        const int64_t slo = sp.slo, dsum = sp.dsum;
+        const size_t sbytes = (size_t)(sp.shi - slo);
         if (!src_dev) CU(sl.src.reserve(sbytes + 64));
         if (!dst_dev) CU(sl.dst.reserve((size_t)dsum + 64));
         // up: the four arrays the kernels read, and a framed decode's stored lengths
@@ -566,14 +634,9 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
             CU(cudaMemcpyAsync(sl.src.p, from, sbytes, cudaMemcpyHostToDevice, sl.stream));
         }
         const BatchArgs a{src_dev ? src : (const uint8_t*)sl.src.p, d.so, d.sl, dst_dev ? dst : (uint8_t*)sl.dst.p, d.dof, d.dc, d.out, m};
-        int lanes = 0;
-        if (is_decode(op) && c->decode_lanes_auto && !placed) {      // (a placed stage's decoded size is known on the device only)
-            double cs = 0, rs = 0;
-            for (int32_t i = b0; i < b1; i++) { cs += src_len[i]; rs += dst_cap[i]; }
-            lanes = lanes_for_ratio(rs > 0 ? cs / rs : 1.0, m, c->dev);
-        }
-        int32_t hc_large = 0;
-        if (op == Op::ENCODE_HC) for (int32_t i = b0; i < b1; i++) hc_large += src_len[i] > 65536;
+        // (a placed stage's decoded size is known on the device only)
+        const int lanes = placed ? 0 : stage_lanes(c, op, src_len, dst_cap, b0, b1);
+        const int32_t hc_large = stage_hc_large(op, src_len, b0, b1);
         switch (kind) {
         case Stage::CODEC:
         case Stage::STREAM_ENCODE:
@@ -654,6 +717,162 @@ int check_side(const lz4b200_ctx* c, const void* p, bool device, const char* wha
         return fail(LZ4B200_E_ARG, std::string(what) + " must be device memory of the context's GPU");
     if (!device && a.type == cudaMemoryTypeDevice) return fail(LZ4B200_E_ARG, std::string(what) + " must be host memory");
     return LZ4B200_OK;
+}
+
+// ---- the asynchronous calls between device memory and page-locked host memory (run_async) ---------------------------
+// The address at which the device reaches p, for a buffer the device reads or writes after an asynchronous call has
+// returned: page-locked host memory with a device address (cudaHostAlloc / cudaMallocHost, torch pin_memory(), a
+// lz4b200_host_register'd range), or, when `device_ok`, device memory of the context's GPU.
+int device_address(const lz4b200_ctx* c, const void* p, bool device_ok, const char* what, void** at)
+{
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+    if (a.type == cudaMemoryTypeHost && a.devicePointer) { *at = a.devicePointer; return LZ4B200_OK; }
+    if (device_ok && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == c->device) {
+        *at = const_cast<void*>(p);
+        return LZ4B200_OK;
+    }
+    return fail(LZ4B200_E_ARG, std::string(what) + (device_ok ? " must be device memory of the context's GPU or page-locked host memory"
+                                                              : " must be page-locked host memory the device can address"));
+}
+
+// The asynchronous calls refuse a capturing stream before any CUDA work: their metadata is host data a graph would have
+// to keep alive.
+int refuse_capture_async(void* stream, const char* what)
+{
+    Capture cap;
+    int rc = capture_of((cudaStream_t)stream, &cap); if (rc) return rc;
+    return cap.on ? fail(LZ4B200_E_ARG, std::string(what) + " cannot be enqueued on a capturing stream") : LZ4B200_OK;
+}
+
+// A page-locked metadata block of at least `bytes` whose last call the device has passed (cudaEventQuery, never waited
+// on).  The pool grows when none is free; a free block too small is grown (which may synchronise, as a growth may).
+int take_meta(lz4b200_ctx* c, size_t bytes, MetaBlock** out)
+{
+    MetaBlock *fit = nullptr, *small = nullptr;
+    for (auto& b : c->meta_pool) {
+        if (b->used) {
+            const cudaError_t q = cudaEventQuery(b->done);
+            if (q == cudaErrorNotReady) continue;
+            if (q != cudaSuccess) return cuda_fail(q, "cudaEventQuery");
+            b->used = false;
+        }
+        if (b->buf.cap >= bytes) { if (!fit || b->buf.cap < fit->buf.cap) fit = b.get(); }
+        else small = b.get();
+    }
+    if (!fit) {
+        if (!small) {
+            c->meta_pool.emplace_back(new MetaBlock());
+            small = c->meta_pool.back().get();
+            CU(cudaEventCreateWithFlags(&small->done, cudaEventDisableTiming));
+        }
+        CU(small->buf.reserve(bytes));
+        fit = small;
+    }
+    fit->used = true;
+    *out = fit;
+    return LZ4B200_OK;
+}
+
+// The stages of an asynchronous call, cut and described as run_host cuts and describes them (stage_end, fill_stage,
+// stage_lanes, stage_hc_large), enqueued on the context's NASYNC streams in turn, forked from `caller` and joined back to
+// it; nothing is waited on unless a buffer must grow.
+//  - The packed encode (enc): src is device memory, dst the device address of page-locked host memory, out_off / out_len
+//    device addresses.  A stage encodes into its dense slots (AsyncSlot::io), scans the lengths, and lands (lz4_land.cuh)
+//    behind the running total that the previous stage's landing step left in its carry cell, after the previous slot's
+//    `carried` event.
+//  - The decode: src is page-locked host memory, copied up a stage at a time on the copy engine; the decoders write dst
+//    (device memory) in place at dst_off, and the stage's results are copied to out_len (device or page-locked memory).
+// Calls are chained through async_done; the call's metadata block is taken again once the caller's stream has passed it.
+int run_async(lz4b200_ctx* c, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
+              const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
+              int64_t dst_total_cap, cudaStream_t caller)
+{
+    const bool enc = is_encode(op);
+    struct Plan { int32_t b0, b1; size_t at; StageSpan sp; };
+    std::vector<Plan> plan;
+    size_t bytes = 0;
+    for (int32_t b0 = 0; b0 < n;) {
+        const int32_t b1 = stage_end(c, src_len, enc ? dst_cap : nullptr, b0, n, !enc);
+        plan.push_back(Plan{b0, b1, bytes, {}});
+        bytes += (meta_host_bytes(b1 - b0) + 15) & ~(size_t)15;
+        b0 = b1;
+    }
+    MetaBlock* blk = nullptr;
+    int rc = take_meta(c, bytes, &blk); if (rc) return rc;
+    size_t need[NASYNC][4] = {};                                              // io, meta, offs, scan
+    for (size_t k = 0; k < plan.size(); k++) {
+        Plan& p = plan[k];
+        const int32_t m = p.b1 - p.b0;
+        p.sp = fill_stage(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, src_off, src_len, dst_off, dst_cap, enc, !enc, false,
+                          false, nullptr);
+        size_t* nd = need[k % NASYNC];
+        nd[0] = std::max(nd[0], (size_t)(enc ? p.sp.dsum : p.sp.shi - p.sp.slo) + 64);
+        nd[1] = std::max(nd[1], (size_t)m * META_BYTES);
+        if (enc) { nd[2] = std::max(nd[2], sizeof(int64_t) * (size_t)(m + 1)); nd[3] = std::max(nd[3], compact_tmp_bytes(m)); }
+    }
+    // growth: an earlier call may still be using the buffers
+    bool grow = false;
+    for (int s = 0; s < NASYNC; s++) {
+        const AsyncSlot& sl = c->aslot[s];
+        grow |= need[s][0] > sl.io.cap || need[s][1] > sl.meta.cap || need[s][2] > sl.offs.cap || need[s][3] > sl.scan.cap;
+    }
+    if (grow) {
+        CU(cudaDeviceSynchronize());
+        for (int s = 0; s < NASYNC; s++) {
+            AsyncSlot& sl = c->aslot[s];
+            CU(sl.io.reserve(need[s][0])); CU(sl.meta.reserve(need[s][1])); CU(sl.offs.reserve(need[s][2])); CU(sl.scan.reserve(need[s][3]));
+        }
+    }
+    const int used = (int)std::min<size_t>(plan.size(), NASYNC);
+    int64_t* carry = c->carry + NSLOT;
+    auto stages = [&]() -> int {
+        CU(cudaEventRecord(c->entry, caller));
+        for (int s = 0; s < used; s++) {
+            CU(cudaStreamWaitEvent(c->aslot[s].stream, c->entry, 0));
+            CU(c->async_done.wait(c->aslot[s].stream, Capture{}));
+        }
+        for (size_t k = 0; k < plan.size(); k++) {
+            const Plan& p = plan[k];
+            const int s = (int)(k % NASYNC), prev = (s + NASYNC - 1) % NASYNC;
+            AsyncSlot& sl = c->aslot[s];
+            const int32_t m = p.b1 - p.b0;
+            const Meta h((uint8_t*)blk->buf.p + p.at, m), d(sl.meta.p, m);
+            CU(cudaMemcpyAsync(sl.meta.p, h.so, (size_t)((uint8_t*)h.aux - (uint8_t*)h.so), cudaMemcpyHostToDevice, sl.stream));
+            const size_t sbytes = (size_t)(p.sp.shi - p.sp.slo);
+            if (!enc && sbytes) CU(cudaMemcpyAsync(sl.io.p, src + p.sp.slo, sbytes, cudaMemcpyHostToDevice, sl.stream));
+            const BatchArgs a{enc ? src : (const uint8_t*)sl.io.p, d.so, d.sl, enc ? (uint8_t*)sl.io.p : dst, d.dof, d.dc, d.out, m};
+            int rc = run_device(c, a, op, sl.stream, stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1),
+                                stage_hc_large(op, src_len, p.b0, p.b1));
+            if (rc) return rc;
+            if (!enc) {
+                CU(cudaMemcpyAsync(out_len + p.b0, d.out, sizeof(int32_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
+                continue;
+            }
+            int64_t* offs = (int64_t*)sl.offs.p;
+            cudaError_t e = launch_compact(nullptr, nullptr, d.out, nullptr, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
+            if (e == cudaSuccess && k > 0) e = cudaStreamWaitEvent(sl.stream, c->aslot[prev].carried, 0);
+            if (e == cudaSuccess)
+                e = launch_land((const uint8_t*)sl.io.p, d.dof, d.out, offs, m, p.sp.dsum, k > 0 ? carry + prev : nullptr, dst_total_cap,
+                                dst, out_off + p.b0, out_len + p.b0, carry + s, c->dev, sl.stream, &c->launches);
+            if (e != cudaSuccess) return cuda_fail(e, "scan / landing launch");
+            CU(cudaEventRecord(sl.carried, sl.stream));
+        }
+        return LZ4B200_OK;
+    };
+    // whatever was enqueued, the caller's stream joins it, and the chain and the metadata block are recorded behind it
+    auto join = [&]() -> int {
+        for (int s = 0; s < used; s++) {
+            CU(cudaEventRecord(c->aslot[s].done, c->aslot[s].stream));
+            CU(cudaStreamWaitEvent(caller, c->aslot[s].done, 0));
+        }
+        CU(c->async_done.record(caller, Capture{}));
+        CU(cudaEventRecord(blk->done, caller));
+        return LZ4B200_OK;
+    };
+    rc = stages();
+    const int jr = join();
+    return rc ? rc : jr;
 }
 
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
@@ -926,8 +1145,8 @@ int lz4b200_create(lz4b200_ctx** out, int device)
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device); c->dev.smem_per_sm = v;
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device); c->dev.smem_optin = v;
     cudaError_t e = cudaMalloc(&c->counters, sizeof(uint32_t) * (NCOUNTER + 4 * NCAPTURED));
-    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * NSLOT);
-    for (Chain* ch : {&c->hc_done, &c->compact_done}) {
+    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * (NSLOT + NASYNC));
+    for (Chain* ch : {&c->hc_done, &c->compact_done, &c->async_done}) {
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->done, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->inner, cudaEventDisableTiming);
     }
@@ -936,6 +1155,11 @@ int lz4b200_create(lz4b200_ctx** out, int device)
         e = cudaStreamCreateWithFlags(&c->slot[i].stream, cudaStreamNonBlocking);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->slot[i].done, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->slot[i].carried, cudaEventDisableTiming);
+    }
+    for (int i = 0; i < NASYNC && e == cudaSuccess; i++) {
+        e = cudaStreamCreateWithFlags(&c->aslot[i].stream, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->aslot[i].done, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->aslot[i].carried, cudaEventDisableTiming);
     }
     if (e != cudaSuccess) { int rc = cuda_fail(e, "context creation"); lz4b200_destroy(c); return rc; }
     *out = c;
@@ -952,7 +1176,13 @@ void lz4b200_destroy(lz4b200_ctx* c)
         if (s.carried) cudaEventDestroy(s.carried);
         if (s.stream) cudaStreamDestroy(s.stream);
     }
-    for (Chain* ch : {&c->hc_done, &c->compact_done}) {
+    for (AsyncSlot& s : c->aslot) {
+        if (s.done) cudaEventDestroy(s.done);
+        if (s.carried) cudaEventDestroy(s.carried);
+        if (s.stream) cudaStreamDestroy(s.stream);
+    }
+    for (auto& b : c->meta_pool) if (b->done) cudaEventDestroy(b->done);
+    for (Chain* ch : {&c->hc_done, &c->compact_done, &c->async_done}) {
         if (ch->done) cudaEventDestroy(ch->done);
         if (ch->inner) cudaEventDestroy(ch->inner);
     }
@@ -968,6 +1198,7 @@ int lz4b200_synchronize(lz4b200_ctx* c)
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     DeviceGuard g(c->device);
     for (int i = 0; i < NSLOT; i++) CU(cudaStreamSynchronize(c->slot[i].stream));
+    for (int i = 0; i < NASYNC; i++) CU(cudaStreamSynchronize(c->aslot[i].stream));
     return LZ4B200_OK;
 }
 
@@ -1000,6 +1231,50 @@ int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* c, const void* src, con
     if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
     return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, encode_op(mode == LZ4B200_MODE_HC),
                  LZ4B200_MEM_DEVICE_TO_HOST, stream, out_off, dst_total_cap);
+}
+
+// ---- between device memory and page-locked host memory without blocking: run_async -----------------------------------
+int lz4b200_encode_batch_packed_from_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                                  const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                                  int32_t* out_len, int32_t n, int mode, void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
+    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n > 0 && (!src || !src_off || !src_len || !dst_cap || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    for (int32_t i = 0; i < n; i++)
+        if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
+    CallGuard g(c); if (g.rc) return g.rc;
+    int rc = refuse_capture_async(stream, "lz4b200_encode_batch_packed_from_device_async"); if (rc) return rc;
+    void *off_at = nullptr, *dst_at = nullptr, *len_at = nullptr;
+    rc = device_address(c, out_off, true, "out_off", &off_at); if (rc) return rc;
+    if (n == 0) { CU(cudaMemsetAsync(off_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
+    rc = check_side(c, src, true, "src"); if (rc) return rc;
+    rc = device_address(c, dst, false, "dst", &dst_at); if (rc) return rc;
+    rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc;
+    return run_async(c, encode_op(mode == LZ4B200_MODE_HC), (const uint8_t*)src, src_off, src_len, (uint8_t*)dst_at, nullptr, dst_cap,
+                     (int32_t*)len_at, n, (int64_t*)off_at, dst_total_cap, (cudaStream_t)stream);
+}
+
+int lz4b200_decode_batch_to_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                                         const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int known_len,
+                                         void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0) return fail(LZ4B200_E_ARG, "negative block count");
+    if (n > 0 && (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    for (int32_t i = 0; i < n; i++)
+        if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
+    CallGuard g(c); if (g.rc) return g.rc;
+    int rc = refuse_capture_async(stream, "lz4b200_decode_batch_to_device_async"); if (rc) return rc;
+    if (n == 0) return LZ4B200_OK;
+    void* at = nullptr;
+    rc = device_address(c, src, false, "src", &at); if (rc) return rc;
+    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
+    rc = device_address(c, out_len, true, "out_len", &at); if (rc) return rc;
+    // (the stages copy out_len at the caller's address, which the copy engines take for either kind)
+    return run_async(c, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst,
+                     dst_off, dst_cap, out_len, n, nullptr, 0, (cudaStream_t)stream);
 }
 
 // ---- LZ4Stream (lz4_stream.cuh): the host pipeline, the frames written on the device ----------------------------------

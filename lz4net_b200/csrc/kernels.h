@@ -51,6 +51,13 @@ cudaError_t launch_compact(const uint8_t* slots, const int64_t* slot_off, const 
                            int64_t* out_off, int32_t n_blocks, void* scan_tmp, size_t scan_tmp_bytes,
                            const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 size_t      compact_tmp_bytes(int32_t n_blocks);
+// One stage of the asynchronous packed encode into mapped host memory (land.cu, lz4_land.cuh): block i of the stage's
+// dense slots (dense + dof[i], len[i] bytes; off = the scan of len, m + 1 entries) lands at dst + base + off[i] when
+// base + off[m] <= total_cap, base = *base_in (null: 0).  out_off[0..m] = base + off, out_len[0..m) = len and
+// *total_out = base + off[m] are written either way.  dense_bytes bounds off[m] (the slots' size) and sizes the launch.
+cudaError_t launch_land(const uint8_t* dense, const int64_t* dof, const int32_t* len, const int64_t* off, int32_t m,
+                        int64_t dense_bytes, const int64_t* base_in, int64_t total_cap, uint8_t* dst, int64_t* out_off,
+                        int32_t* out_len, int64_t* total_out, const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 // Wrap / Unwrap packets in device memory (wrap.cu, lz4_wrap.cuh).  The scratch holds the codec's view of the batch: payload
 // offsets, lengths and capacities per packet, and the codec's per-packet results.
 struct WrapScratch { int64_t* off; int32_t* len; int32_t* cap; int32_t* res; };
