@@ -17,6 +17,7 @@ enum EncProfSlot {
     EP_BLOCK, EP_SEQ,                       // blocks encoded, sequences parked (with the last literals)
     EP_ROUND, EP_ROUND_WIDE,                // find-match rounds, of which 64 iterations wide
     EP_EXACT,                               // rounds on the exact path
+    EP_PAIR,                                // rounds on the pair path: two iterations share a bucket, none more
     EP_PROBE, EP_PROBE_HIT,                 // post-match probes tried alone, of which hit
     EP_FLUSH, EP_LONG_LIT,                  // EMIT calls, literal runs copied by copy_long_literals
     EP_CATCHUP_LONG,                        // catch-ups finished by the whole warp (longer than EMIT's per-lane steps)

@@ -160,6 +160,7 @@ SIMT_DEV RoundOut find_round(const EncTable<GENERAL>& T, const InWords& in, int 
     }
     ENC_PROF_LAP(EP_C_SAMEHASH, tp);
     if (DUP == 2 && multi == 0u) {
+        ENC_PROF_EVENT_IF(EP_PAIR, anylost != 0u);
         uint32_t hitm[W]; int cand[W];
 #pragma unroll
         for (int s = 0; s < W; s++) {

@@ -171,6 +171,28 @@ def encode(blocks, caps=None, sched_seed=1, src_skew=0, dst_skew=0, variant=2, t
     return res.tolist(), out.take(res.tolist(), "encoder")
 
 
+ENC_EVENTS = ("blocks", "seqs", "rounds", "rounds_wide", "exact", "pair", "probes", "probe_hits")
+_enc_prof = None
+
+
+def encode_events(block, variant=2, tune=(12, 8, 24), sched_seed=1):
+    """One block through the fast encoder built with its event counters (enc_prof.cuh).  Returns (result, bytes, {event:
+    count}) with the events of ENC_EVENTS: rounds (wide, on the exact path, on the pair path) and post-match probes tried
+    alone (and hit)."""
+    global _enc_prof
+    if _enc_prof is None:
+        l = C.CDLL(build(os.path.join(_DIR, "emu_enc_prof.cpp"), ("-DLZ4B200_ENC_PROF",)))
+        l.emu_encode_events.restype = _I
+        l.emu_encode_events.argtypes = [_I, _I, _I, _I, _P, _I, _P, _I, _P, _U64]
+        _enc_prof = l
+    ev = np.zeros(len(ENC_EVENTS), np.uint64)
+    cap = _bound(len(block))
+    out = _Slots([cap])
+    with _staged([block]) as (src,):
+        r = _enc_prof.emu_encode_events(variant, *tune, src, len(block), out.ptrs[0], cap, ev.ctypes.data, sched_seed)
+    return r, out.take([r], "encoder")[0], dict(zip(ENC_EVENTS, ev.tolist()))
+
+
 def _encode_one(entry, who, block, cap, src_skew, dst_skew, fence, *args):
     """One block through a single-block encoder entry point.  Returns (result, bytes)."""
     n = len(block)

@@ -5,72 +5,14 @@ The blocks are built so that the catch-ups have known lengths.  In incompressibl
 probes with a growing step, so the positions between two probes are never inserted into the table.  Copying the bytes
 in front of an inserted probe position x to the bytes in front of a later probe position y gives a match found at y
 whose catch-up is exactly as long as the copy (or is stopped by the anchor, or by ref reaching position 0).  A small
-model of the reference's greedy parse (checked against the oracle's bytes) confirms every planted catch-up."""
+model of the reference's greedy parse (tests/encround.py, checked against the oracle's bytes) confirms every planted
+catch-up."""
 import numpy as np
 import pytest
 
 import oracle
 from tests import cases, emu
-
-LIMIT64K = 65547
-
-
-def _parse(d: bytes):
-    """The reference's greedy parse (LZ4_compress64kCtx / LZ4_compressCtx, no output limit).  Returns the sequences as
-    (anchor, ip found, ip caught up, ref caught up, match end) and the probed positions, in order."""
-    n = len(d)
-    general = n >= LIMIT64K
-    shift = 20 if general else 19
-    table = [0] * (1 << (32 - shift))
-    mv = memoryview(d)
-
-    def word(p):
-        return int.from_bytes(mv[p:p + 4], "little")
-
-    def h(p):
-        return ((word(p) * 2654435761) & 0xFFFFFFFF) >> shift
-
-    def hit(ref, ip):
-        return (not general or ref > ip - 65536) and word(ref) == word(ip)
-
-    seqs, probes = [], []
-    if n < 13:
-        return seqs, probes, 0
-    mflimit, matchlimit = n - 12, n - 5
-    anchor = 0
-    table[h(0)] = 0
-    ip = 1
-    while True:
-        attempts, fwd = 67, ip
-        while True:
-            ip = fwd
-            step = attempts >> 6
-            attempts += 1
-            fwd = ip + step
-            if fwd > mflimit:
-                return seqs, probes, anchor
-            k = h(ip); ref = table[k]; table[k] = ip
-            probes.append(ip)
-            if hit(ref, ip):
-                break
-        found = ip
-        while ip > anchor and ref > 0 and d[ip - 1] == d[ref - 1]:
-            ip -= 1; ref -= 1
-        while True:
-            m, r = ip + 4, ref + 4
-            while m < matchlimit and d[m] == d[r]:
-                m += 1; r += 1
-            seqs.append((anchor, found, ip, ref, m))
-            anchor = m
-            if m > mflimit:
-                return seqs, probes, anchor
-            table[h(m - 2)] = m - 2
-            k = h(m); ref = table[k]; table[k] = m
-            if hit(ref, m):
-                ip = found = m
-                continue
-            break
-        ip = m + 1
+from tests.encround import LIMIT64K, parse
 
 
 def _emit(d: bytes, seqs, last_anchor):
@@ -101,7 +43,8 @@ def _emit(d: bytes, seqs, last_anchor):
 
 
 def _model(d: bytes):
-    seqs, probes, last = _parse(d)
+    p = parse(d)
+    seqs, probes, last = p.seqs, p.probes, p.last
     out, starts = _emit(d, seqs, last)
     assert (len(out), out) == oracle.encode(d), "the parse model disagrees with the oracle"
     return seqs, probes, starts

@@ -27,7 +27,7 @@ from tests import emu  # noqa: E402
 
 CSRC = os.path.join(ROOT, "lz4net_b200", "csrc")
 # the order of enum EncProfSlot
-EVENTS = ["blocks", "seqs", "rounds", "rounds_wide", "exact", "probes", "probe_hits", "flushes", "long_lit", "catchup_long"]
+EVENTS = ["blocks", "seqs", "rounds", "rounds_wide", "exact", "pair", "probes", "probe_hits", "flushes", "long_lit", "catchup_long"]
 PHASES = ["loadhash", "samehash", "vote", "exact", "probe", "catchup", "count", "park", "emit", "block"]
 BLOCK = 65536
 
