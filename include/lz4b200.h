@@ -159,10 +159,11 @@ int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* ctx,
                                             int32_t* out_len, int32_t n_blocks, int mode, void* stream);
 
 /* ---- offload without blocking: device memory <-> page-locked host memory, asynchronous on `stream` ------------------
- * The two calls below do what lz4b200_encode_batch_packed_from_device and lz4b200_decode_batch(LZ4B200_MEM_HOST_TO_DEVICE)
- * do -- the same out_len, offsets and bytes -- but only ENQUEUE their work on `stream` and return without waiting for any
- * device work: the thread that launches a model's kernels can offload a cache to host RAM, or prefetch it back, and keep
- * launching while the transfer runs.
+ * The calls below do what their synchronous forms do -- lz4b200_encode_batch_packed_from_device,
+ * lz4b200_decode_batch(LZ4B200_MEM_HOST_TO_DEVICE), lz4b200_decode_batch_packed_to_device, and the Wrap / Unwrap calls
+ * between device and host memory -- with the same out_len, offsets and bytes, but only ENQUEUE their work on `stream` and
+ * return without waiting for any device work: the thread that launches a model's kernels can offload a cache to host RAM,
+ * or prefetch it back, and keep launching while the transfer runs.
  *   - Ordering: the call's device work runs after everything enqueued on `stream` before the call, and anything enqueued on
  *     `stream` after it sees all of its results.  Calls of one context are ordered among themselves on any streams.
  *   - Lifetime: the caller keeps src, dst, out_off and out_len alive and untouched until `stream` has passed the call (a
@@ -193,6 +194,54 @@ int lz4b200_encode_batch_packed_from_device_async(lz4b200_ctx* ctx, const void* 
 int lz4b200_decode_batch_to_device_async(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
                                          void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len,
                                          int32_t n_blocks, int known_len, void* stream);
+/* decode_batch_packed_to_device_async: lz4b200_decode_batch_packed_to_device without blocking.  src is page-locked host
+ *   memory; dst is device memory of the context's GPU; out_off (n_blocks+1 entries) and out_len are written by the device.
+ *   Results, bytes and the contract of a destination too small are those of the synchronous call.  n_blocks == 0 is
+ *   LZ4B200_OK with out_off[0] = 0 written on the stream. */
+int lz4b200_decode_batch_packed_to_device_async(lz4b200_ctx* ctx, const void* src, const int64_t* src_off,
+                                                const int32_t* src_len, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                                int32_t* out_len, int32_t n_blocks, void* stream);
+
+/* The same for Wrap packets (below), which describe themselves: a packet holds its raw length, so a batch restores from
+ * the packet offsets alone, and an input that does not shrink is stored raw, so a packet is never above its input + 8
+ * bytes whatever the data.
+ *
+ * wrap_batch_packed_from_device_async: lz4b200_wrap_batch_packed_from_device without blocking.  src is device memory of the
+ *   context's GPU; dst is page-locked host memory.  out_off[0..n] (n+1 entries), out_len and the bytes equal what the
+ *   synchronous call gives; sum(src_len[i] + 8) bytes of dst are always enough.  A destination too small is still
+ *   LZ4B200_OK, as in lz4b200_encode_batch_packed_from_device_async: out_off and out_len are filled and nothing outside
+ *   [dst, dst + dst_total_cap) is written.  A packet above INT32_MAX bytes (src_len[i] > INT32_MAX - 8) is LZ4B200_E_ARG.
+ *   n == 0 is LZ4B200_OK with out_off[0] = 0 written on the stream. */
+int lz4b200_wrap_batch_packed_from_device_async(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                                int high_compression, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                                int32_t* out_len, int32_t n, void* stream);
+/* The two Unwraps from page-locked host memory read the packet headers on the DEVICE, from the bytes they stage, unlike the
+ * synchronous ones, which read them on the host before any device work: the source may be written by work still queued on
+ * `stream` when the call is made -- an asynchronous Wrap landing into the same buffer, for one -- and the host would read
+ * what was there before.  The caller therefore needs only the packet offsets and lengths.
+ *
+ * unwrap_batch_to_device_async: lz4b200_unwrap_batch_to_device without blocking.  src is page-locked host memory; dst is
+ *   device memory of the context's GPU.  out_len[i] equals what the synchronous call returns for the packet: bytes restored,
+ *   LZ4B200_E_FORMAT or LZ4B200_E_ARG (a bad packet is that packet's status, never the call's).  Nothing is written outside
+ *   [dst_off[i], dst_off[i] + dst_cap[i]). */
+int lz4b200_unwrap_batch_to_device_async(lz4b200_ctx* ctx, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                         void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len,
+                                         int32_t n, void* stream);
+/* unwrap_batch_packed_to_device_async: unwrap into PACKED device output sized from the headers.  out_off[0..n] (n+1
+ *   entries) = exclusive prefix sum of max(size, 0), size = the header's unwrapped size or the packet's negative status, is
+ *   written by the device whether the total fits or not.
+ *   - out_off[n] <= dst_total_cap: out_off, out_len and the bytes equal lz4b200_unwrap_batch_packed_to_device's.
+ *   - out_off[n] > dst_total_cap: still LZ4B200_OK, under the contract of lz4b200_decode_batch_packed_to_device: nothing
+ *     outside [dst, dst + dst_total_cap) is written, the bytes inside it are unspecified, and out_len[i] is non-negative
+ *     exactly for the well-formed packets, where it equals the size.  This is weaker than the synchronous call's "dst is
+ *     untouched", on purpose: the headers are read on the device a stage at a time, so the total is known only once the
+ *     last stage has been staged, and holding the restored output back until then would take a second pass over the
+ *     packets.  (A stage is restored when everything up to its end fits.  A packet whose header is well-formed but whose
+ *     payload does not decode reports LZ4B200_E_FORMAT in a stage that was restored and its size in one that was not.)
+ *   n == 0 is LZ4B200_OK with out_off[0] = 0 written on the stream. */
+int lz4b200_unwrap_batch_packed_to_device_async(lz4b200_ctx* ctx, const void* src, const int64_t* src_off,
+                                                const int32_t* src_len, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                                int32_t* out_len, int32_t n, void* stream);
 
 /* Compaction of fixed-stride encoder slots into one contiguous payload (device memory only): the batched form of
  * the Buffer.BlockCopy trim in LZ4Codec.Encode (src/LZ4/LZ4Codec.cs:357-364).  out_off[i] (int64, n_blocks+1
@@ -222,9 +271,10 @@ int lz4b200_compact(lz4b200_ctx* ctx, const void* slots, const int64_t* slot_off
  *   - lz4b200_launch_count counts the launches a call enqueues when it is captured, not replays.
  * Every other call that takes a `stream` synchronises with the host (the mixed-memory batches, the packed encode from
  * and decode to device memory, the LZ4Stream and the Wrap / Unwrap calls between device and host memory): on a capturing
- * stream it returns LZ4B200_E_ARG before any CUDA work, and the capture stays valid.  So do
- * lz4b200_encode_batch_packed_from_device_async and lz4b200_decode_batch_to_device_async, which do not synchronise but
- * hand the device host metadata that a graph would have to keep alive.  lz4b200_peer_copy is not covered.
+ * stream it returns LZ4B200_E_ARG before any CUDA work, and the capture stays valid.  So do the asynchronous calls --
+ * lz4b200_encode_batch_packed_from_device_async, decode_batch_to_device_async, decode_batch_packed_to_device_async,
+ * wrap_batch_packed_from_device_async, unwrap_batch_to_device_async and unwrap_batch_packed_to_device_async -- which do not
+ * synchronise but hand the device host metadata that a graph would have to keep alive.  lz4b200_peer_copy is not covered.
  * The calls without a stream (host-memory batches, single-block functions, lz4b200_synchronize, lz4b200_reserve) use
  * the legacy default stream or synchronise the device: they must not be made while any thread of the process captures
  * in cudaStreamCaptureModeGlobal.

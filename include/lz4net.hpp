@@ -95,6 +95,36 @@ public:
                                                  stream) != LZ4B200_OK)
             throw std::runtime_error(lz4b200_last_error());
     }
+    // The same for the packed unknown-size decode and for Wrap packets (lz4b200_decode_batch_packed_to_device_async,
+    // lz4b200_wrap_batch_packed_from_device_async, lz4b200_unwrap_batch_to_device_async,
+    // lz4b200_unwrap_batch_packed_to_device_async).  The packed forms' out_off (n + 1 entries) is written by the device.
+    void decode_packed_from_host_async(const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                                       int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n, void* stream)
+    {
+        if (lz4b200_decode_batch_packed_to_device_async(h_, src, src_off, src_len, dst, dst_total_cap, out_off, out_len, n,
+                                                        stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
+    void wrap_packed_to_host_async(const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                                   int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n, bool hc, void* stream)
+    {
+        if (lz4b200_wrap_batch_packed_from_device_async(h_, src, src_off, src_len, hc ? 1 : 0, dst, dst_total_cap, out_off, out_len,
+                                                        n, stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
+    void unwrap_from_host_async(const void* src, const int64_t* src_off, const int32_t* src_len, void* dst, const int64_t* dst_off,
+                                const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
+    {
+        if (lz4b200_unwrap_batch_to_device_async(h_, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
+    void unwrap_packed_from_host_async(const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                                       int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n, void* stream)
+    {
+        if (lz4b200_unwrap_batch_packed_to_device_async(h_, src, src_off, src_len, dst, dst_total_cap, out_off, out_len, n,
+                                                        stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
 private:
     lz4b200_ctx* h_ = nullptr;
 };

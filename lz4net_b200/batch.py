@@ -30,7 +30,9 @@ refuse a capturing stream the same way.
 
 encode_to_host_packed_async and decode_from_host_async move blocks between a device tensor and a page-locked CPU tensor
 without blocking the calling thread: they enqueue their work on a stream and return, so a thread that launches a model's
-kernels can offload to host RAM, or prefetch back, and keep launching.  They refuse a capturing stream.
+kernels can offload to host RAM, or prefetch back, and keep launching.  decode_from_host_packed_async,
+wrap_to_host_packed_async, unwrap_to_device_async and unwrap_to_device_packed_async do the same for the packed decode and
+for Wrap packets, which carry their own sizes and never exceed input + 8 bytes.  They refuse a capturing stream.
 """
 from __future__ import annotations
 
@@ -226,6 +228,66 @@ def decode_from_host_async(ctx: Context, comp: torch.Tensor, src_off, src_len, o
     native.check(native.lib().lz4b200_decode_batch_to_device_async(
         ctx.handle, c, _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), _h(dst_off, np.int64, n), _h(dst_cap, np.int32, n),
         res, n, int(known), _stream_of(stream)), "decode_batch_to_device_async")
+
+
+def decode_from_host_packed_async(ctx: Context, comp: torch.Tensor, src_off, src_len, out: torch.Tensor, out_off: torch.Tensor,
+                                  out_len: torch.Tensor, stream=None):
+    """decode_from_host_packed without blocking (lz4b200_decode_batch_packed_to_device_async): blocks whose decoded sizes
+    nobody stored, decoded into `out` back to back, block i at out_off[i], out_off[n] = the total.  comp is a page-locked CPU
+    uint8 tensor; out_off (int64[n+1]) and out_len (int32[n]) are CUDA or page-locked CPU tensors, written by the device;
+    src_off / src_len are numpy arrays, read during the call.  Enqueued on `stream` (default: the current torch stream);
+    returns at once.  When the total exceeds out.nbytes the call still succeeds: nothing is written outside `out`, its
+    bytes are unspecified, and out_len holds the sizes; check out_off[n] after synchronising."""
+    n = len(src_off)
+    c = _pinned(comp, torch.uint8, 0, "comp")
+    off, res = _pinned(out_off, torch.int64, n + 1, "out_off", True), _pinned(out_len, torch.int32, n, "out_len", True)
+    native.check(native.lib().lz4b200_decode_batch_packed_to_device_async(
+        ctx.handle, c, _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), out.nbytes, off, res, n, _stream_of(stream)),
+        "decode_batch_packed_to_device_async")
+
+
+def wrap_to_host_packed_async(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: torch.Tensor, out_off: torch.Tensor,
+                              out_len: torch.Tensor, hc: bool = False, stream=None):
+    """wrap_to_host_packed without blocking (lz4b200_wrap_batch_packed_from_device_async): the Wrap / WrapHC packet of
+    raw + src_off[i] lands at dst + out_off[i], back to back, out_off[n] = the total; sum(src_len + 8) bytes of dst are
+    always enough.  dst is a page-locked CPU uint8 tensor; out_off (int64[n+1]) and out_len (int32[n]) are CUDA or
+    page-locked CPU tensors, written by the device; src_off / src_len are numpy arrays, read during the call.  Enqueued on
+    `stream` (default: the current torch stream); returns at once.  When the total exceeds dst.numel() the call still
+    succeeds: out_off and out_len are filled and nothing is written outside dst; check out_off[n] after synchronising."""
+    n = len(src_off)
+    d, off, res = (_pinned(dst, torch.uint8, 0, "dst"), _pinned(out_off, torch.int64, n + 1, "out_off", True),
+                   _pinned(out_len, torch.int32, n, "out_len", True))
+    native.check(native.lib().lz4b200_wrap_batch_packed_from_device_async(
+        ctx.handle, _d(raw), _h(src_off, np.int64), _h(src_len, np.int32, n), int(hc), d, dst.numel(), off, res, n,
+        _stream_of(stream)), "wrap_batch_packed_from_device_async")
+
+
+def unwrap_to_device_async(ctx: Context, packets: torch.Tensor, src_off, src_len, out: torch.Tensor, dst_off, dst_cap,
+                           out_len: torch.Tensor, stream=None):
+    """unwrap_to_device without blocking (lz4b200_unwrap_batch_to_device_async): packet i of packets + src_off[i] is
+    restored at out + dst_off[i], nothing written outside its dst_cap[i] bytes; out_len[i] = bytes restored,
+    LZ4B200_E_FORMAT or E_ARG.  The headers are read on the device, so the packets may still be being written by work
+    queued on the stream before the call.  packets is a page-locked CPU uint8 tensor; out_len (int32[n]) a CUDA or
+    page-locked CPU tensor; src_off / src_len / dst_off / dst_cap are numpy arrays, read during the call."""
+    n = len(src_off)
+    p, res = _pinned(packets, torch.uint8, 0, "packets"), _pinned(out_len, torch.int32, n, "out_len", True)
+    native.check(native.lib().lz4b200_unwrap_batch_to_device_async(
+        ctx.handle, p, _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), _h(dst_off, np.int64, n), _h(dst_cap, np.int32, n),
+        res, n, _stream_of(stream)), "unwrap_batch_to_device_async")
+
+
+def unwrap_to_device_packed_async(ctx: Context, packets: torch.Tensor, src_off, src_len, out: torch.Tensor, out_off: torch.Tensor,
+                                  out_len: torch.Tensor, stream=None):
+    """unwrap_to_device_packed without blocking (lz4b200_unwrap_batch_packed_to_device_async): packet i lands at
+    out + out_off[i] (int64[n+1], written by the device, out_off[n] = the total) when the total fits out.nbytes.  Otherwise
+    the call still succeeds: nothing is written outside `out`, its bytes are unspecified, and out_len[i] is non-negative
+    exactly for the well-formed packets, where it is the size.  The headers are read on the device."""
+    n = len(src_off)
+    p = _pinned(packets, torch.uint8, 0, "packets")
+    off, res = _pinned(out_off, torch.int64, n + 1, "out_off", True), _pinned(out_len, torch.int32, n, "out_len", True)
+    native.check(native.lib().lz4b200_unwrap_batch_packed_to_device_async(
+        ctx.handle, p, _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), out.nbytes, off, res, n, _stream_of(stream)),
+        "unwrap_batch_packed_to_device_async")
 
 
 def wrap_to_host(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, out_len, hc: bool = False):

@@ -8,9 +8,10 @@
 // calls between device and host memory go through it too, skipping the copy of whichever side is already on the device;
 // so does the packed unknown-size decode from host into device memory, whose output offset is carried across the stages
 // on the device (lz4_packed.cuh).  What a stage runs is named by its caller (Stage); the codec operation by Op.
-// The asynchronous packed encode into page-locked host memory and decode from it (run_async) cut their stages by the same
-// plan, enqueue them on streams and buffers of their own and return without waiting; the encode's stages land in host
-// memory from a kernel (lz4_land.cuh), since where a stage lands is known only on the device.
+// The asynchronous calls between device memory and page-locked host memory (run_async: the packed encode and Wrap into it,
+// the decode, packed decode and Unwrap from it) cut their stages by the same plan, enqueue them on streams and buffers of
+// their own and return without waiting; the packed encodes' stages land in host memory from a kernel (lz4_land.cuh), since
+// where a stage lands is known only on the device, and the Unwraps read their headers on the device (run_unwrap).
 // The device-memory calls enter through one path (DeviceCall): each states what it takes from the context (Need), which
 // admits it to a CUDA graph capture or grows an eager call's scratch; lz4b200_reserve grows to the same needs.
 // The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
@@ -198,6 +199,10 @@ WrapScratch wrap_scratch_at(void* p, int32_t n)
     return WrapScratch{(int64_t*)p, len, len + n, len + 2 * n};
 }
 constexpr size_t META_BYTES = 32, WRAP_META_OFFSET = 32, WRAP_META_BYTES = WRAP_META_OFFSET + WRAP_SCRATCH_BYTES;
+// An asynchronous stage's device block (AsyncSlot::meta) holds every kind's: the arrays, a Wrap's or an Unwrap's
+// WrapScratch at WRAP_META_OFFSET * m, then a packed form's "fits" flag (async_fits).
+size_t async_meta_bytes(int32_t m) { return (size_t)m * WRAP_META_BYTES + sizeof(int64_t); }
+int* async_fits(void* meta, int32_t m) { return (int*)((uint8_t*)meta + (size_t)m * WRAP_META_BYTES); }
 
 // The operations of the batch codec.
 enum class Op { ENCODE_FAST, ENCODE_HC, DECODE_KNOWN, DECODE_UNKNOWN, MEASURE_KNOWN, MEASURE_UNKNOWN };
@@ -217,6 +222,8 @@ enum class Stage {
                       // payload the stored-copy step copies while the decoder gets the neutral entry (src_len 0, dst_cap 0);
                       // in host memory it lands like a decoded block of dst_cap[i] bytes
     PLACED_DECODE,    // the packed unknown-size decode into device memory, its output offset carried across the stages
+    UNWRAP,           // asynchronous calls only: Unwrap packets whose headers are read on the device (run_unwrap) into device
+                      // memory, into the caller's slots, or packed (dst_off == nullptr) and placed like PLACED_DECODE
 };
 
 }  // namespace
@@ -416,6 +423,27 @@ int run_wrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, Op op, cu
     const BatchArgs enc{a.src, a.src_off, w.len, a.dst, w.off, w.cap, w.res, a.n_blocks};
     rc = run_device(c, enc, op, st, 0, hc_large, cap); if (rc) return rc;
     return launched(launch_wrap_finish(a, w, st, &c->launches), "wrap finish launch");
+}
+
+// What the packed Unwraps do between the prep and the decode: `place` enqueues the placement of the sizes the prep left in
+// out_len, which writes the decode's capacities (caps) and the "fits" flag that both the decode and the finish run behind.
+struct UnwrapPlacement { std::function<cudaError_t()> place; const int32_t* caps; const int* fits; };
+
+// An Unwrap of the packets of a (src / src_off / src_len; outputs at dst + dst_off, capacities dst_cap, null = no limit):
+// prep (each header, read on the device: a decode entry for a compressed packet, a neutral one for a stored or rejected
+// packet) -> [the placement of the packed forms] -> the known-size decode -> finish (the stored copies, out_len = bytes
+// restored or the packet's status).  The counterpart of run_wrap, for the device calls and the asynchronous stages alike.
+int run_unwrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, cudaStream_t st, const Capture& cap = {},
+               const UnwrapPlacement* placed = nullptr)
+{
+    int rc = launched(launch_unwrap_prep(a, w, st, &c->launches), "unwrap prep launch"); if (rc) return rc;
+    if (placed) { rc = launched(placed->place(), "unwrap placement launch"); if (rc) return rc; }
+    // the compressed packets, known size (LZ4Codec.cs:595); stored and rejected ones are neutral entries
+    const BatchArgs dec{a.src, w.off, w.len, a.dst, a.dst_off, placed ? placed->caps : w.cap, w.res, a.n_blocks};
+    const int* fits = placed ? placed->fits : nullptr;
+    rc = launched(launch_decode(dec, true, c->pinned_lanes(), c->counter(cap), c->dev, st, &c->launches, fits), "unwrap decode launch");
+    if (rc) return rc;
+    return launched(launch_unwrap_finish(a, w, fits, st, &c->launches), "unwrap finish launch");
 }
 
 // The placement of the packed decodes (lz4_packed.cuh): n sizes scanned into the offsets `off`, then each block's capacity
@@ -776,19 +804,25 @@ int take_meta(lz4b200_ctx* c, size_t bytes, MetaBlock** out)
 
 // The stages of an asynchronous call, cut and described as run_host cuts and describes them (stage_end, fill_stage,
 // stage_lanes, stage_hc_large), enqueued on the context's NASYNC streams in turn, forked from `caller` and joined back to
-// it; nothing is waited on unless a buffer must grow.
-//  - The packed encode (enc): src is device memory, dst the device address of page-locked host memory, out_off / out_len
-//    device addresses.  A stage encodes into its dense slots (AsyncSlot::io), scans the lengths, and lands (lz4_land.cuh)
-//    behind the running total that the previous stage's landing step left in its carry cell, after the previous slot's
-//    `carried` event.
-//  - The decode: src is page-locked host memory, copied up a stage at a time on the copy engine; the decoders write dst
-//    (device memory) in place at dst_off, and the stage's results are copied to out_len (device or page-locked memory).
+// it; nothing is waited on unless a buffer must grow.  What a stage runs is its kind's sequence in run_host:
+//  - The packed encodes (enc: CODEC with an encode, WRAP_ENCODE): src is device memory, dst the device address of
+//    page-locked host memory, out_off / out_len device addresses.  A stage encodes (or wraps, run_wrap: capacity src_len + 8
+//    per packet, the stage weighed by it) into its dense slots (AsyncSlot::io), scans the lengths, and lands
+//    (lz4_land.cuh) behind the running total that the previous stage's landing step left in its carry cell, after the
+//    previous slot's `carried` event.
+//  - The decodes into device memory (CODEC with a decode, UNWRAP, PLACED_DECODE): src is page-locked host memory, copied
+//    up a stage at a time on the copy engine, weighed by src_len; the decoders write dst (device memory) in place.  A
+//    CODEC decode writes at dst_off; an UNWRAP reads the headers from the staged bytes on the device (run_unwrap), since
+//    work still queued on `caller` may write them.  The packed forms (placed: PLACED_DECODE, an UNWRAP without dst_off)
+//    measure, scan and place their stage behind the previous one's from the same carry cells (place), then decode behind
+//    the stage's "fits" flag; their absolute offsets are copied to out_off, the last stage's running total to out_off[n].
+//    The stage's results are copied to out_len (device or page-locked memory).
 // Calls are chained through async_done; the call's metadata block is taken again once the caller's stream has passed it.
-int run_async(lz4b200_ctx* c, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
+int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
               const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
               int64_t dst_total_cap, cudaStream_t caller)
 {
-    const bool enc = is_encode(op);
+    const bool enc = is_encode(op), placed = kind == Stage::PLACED_DECODE || (kind == Stage::UNWRAP && !dst_off);
     struct Plan { int32_t b0, b1; size_t at; StageSpan sp; };
     std::vector<Plan> plan;
     size_t bytes = 0;
@@ -805,11 +839,11 @@ int run_async(lz4b200_ctx* c, Op op, const uint8_t* src, const int64_t* src_off,
         Plan& p = plan[k];
         const int32_t m = p.b1 - p.b0;
         p.sp = fill_stage(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, src_off, src_len, dst_off, dst_cap, enc, !enc, false,
-                          false, nullptr);
+                          placed, nullptr);
         size_t* nd = need[k % NASYNC];
         nd[0] = std::max(nd[0], (size_t)(enc ? p.sp.dsum : p.sp.shi - p.sp.slo) + 64);
-        nd[1] = std::max(nd[1], (size_t)m * META_BYTES);
-        if (enc) { nd[2] = std::max(nd[2], sizeof(int64_t) * (size_t)(m + 1)); nd[3] = std::max(nd[3], compact_tmp_bytes(m)); }
+        nd[1] = std::max(nd[1], async_meta_bytes(m));
+        if (enc || placed) { nd[2] = std::max(nd[2], sizeof(int64_t) * (size_t)(m + 1)); nd[3] = std::max(nd[3], compact_tmp_bytes(m)); }
     }
     // growth: an earlier call may still be using the buffers
     bool grow = false;
@@ -841,15 +875,52 @@ int run_async(lz4b200_ctx* c, Op op, const uint8_t* src, const int64_t* src_off,
             CU(cudaMemcpyAsync(sl.meta.p, h.so, (size_t)((uint8_t*)h.aux - (uint8_t*)h.so), cudaMemcpyHostToDevice, sl.stream));
             const size_t sbytes = (size_t)(p.sp.shi - p.sp.slo);
             if (!enc && sbytes) CU(cudaMemcpyAsync(sl.io.p, src + p.sp.slo, sbytes, cudaMemcpyHostToDevice, sl.stream));
-            const BatchArgs a{enc ? src : (const uint8_t*)sl.io.p, d.so, d.sl, enc ? (uint8_t*)sl.io.p : dst, d.dof, d.dc, d.out, m};
-            int rc = run_device(c, a, op, sl.stream, stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1),
-                                stage_hc_large(op, src_len, p.b0, p.b1));
+            // (a packed Unwrap's prep reads no capacity: the placement writes the decode's into d.dc)
+            const BatchArgs a{enc ? src : (const uint8_t*)sl.io.p, d.so, d.sl, enc ? (uint8_t*)sl.io.p : dst, d.dof,
+                              kind == Stage::UNWRAP && placed ? nullptr : d.dc, d.out, m};
+            const WrapScratch w = wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m);
+            int* fits = async_fits(sl.meta.p, m);
+            int64_t* offs = (int64_t*)sl.offs.p;
+            // a packed stage's sizes scanned and placed behind the previous stage's (lz4_packed.cuh); the next one follows
+            auto place_stage = [&](int32_t room) {
+                cudaError_t e = place(c, d.out, offs, m, sl.scan, dst_total_cap, room, d.dc, fits, sl.stream,
+                                      k > 0 ? c->aslot[prev].carried : nullptr, k > 0 ? carry + prev : nullptr, d.dof, carry + s);
+                return e == cudaSuccess ? cudaEventRecord(sl.carried, sl.stream) : e;
+            };
+            int rc = LZ4B200_OK;
+            switch (kind) {
+            case Stage::CODEC:
+                rc = run_device(c, a, op, sl.stream, stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), stage_hc_large(op, src_len, p.b0, p.b1));
+                break;
+            case Stage::WRAP_ENCODE:
+                rc = run_wrap(c, a, w, op, sl.stream, stage_hc_large(op, src_len, p.b0, p.b1));
+                break;
+            case Stage::UNWRAP: {
+                const UnwrapPlacement pl{[&] { return place_stage(0); }, d.dc, fits};
+                rc = run_unwrap(c, a, w, sl.stream, Capture{}, placed ? &pl : nullptr);
+                break;
+            }
+            case Stage::PLACED_DECODE: {
+                // measure -> scan -> placement, behind the previous stage's -> decode behind the stage's flag (run_host's)
+                BatchArgs sizes = a; sizes.dst_cap = nullptr;
+                cudaError_t e = launch_measure(sizes, false, c->dev, sl.stream, &c->launches);
+                if (e == cudaSuccess) e = place_stage(PACKED_ROOM_UNKNOWN);
+                if (e == cudaSuccess) e = launch_decode(a, false, c->pinned_lanes(), c->counter(), c->dev, sl.stream, &c->launches, fits);
+                rc = launched(e, "packed measure / placement / decode launch");
+                break;
+            }
+            default:
+                return fail(LZ4B200_E_ARG, "run_async: no asynchronous form of this stage");
+            }
             if (rc) return rc;
             if (!enc) {
                 CU(cudaMemcpyAsync(out_len + p.b0, d.out, sizeof(int32_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
+                if (placed) {
+                    CU(cudaMemcpyAsync(out_off + p.b0, d.dof, sizeof(int64_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
+                    if (p.b1 == n) CU(cudaMemcpyAsync(out_off + n, carry + s, sizeof(int64_t), cudaMemcpyDefault, sl.stream));
+                }
                 continue;
             }
-            int64_t* offs = (int64_t*)sl.offs.p;
             cudaError_t e = launch_compact(nullptr, nullptr, d.out, nullptr, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
             if (e == cudaSuccess && k > 0) e = cudaStreamWaitEvent(sl.stream, c->aslot[prev].carried, 0);
             if (e == cudaSuccess)
@@ -873,6 +944,48 @@ int run_async(lz4b200_ctx* c, Op op, const uint8_t* src, const int64_t* src_off,
     rc = stages();
     const int jr = join();
     return rc ? rc : jr;
+}
+
+// The asynchronous packed encodes from device memory into page-locked host memory (the codec's blocks, Wrap packets),
+// after their argument checks: the capture refusal and the kinds of memory, then run_async.  n == 0 writes out_off[0] = 0
+// on the stream.
+int landed_async(lz4b200_ctx* c, Stage kind, Op op, const void* src, const int64_t* src_off, const int32_t* src_len,
+                 const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
+                 void* stream, const char* what)
+{
+    CallGuard g(c); if (g.rc) return g.rc;
+    int rc = refuse_capture_async(stream, what); if (rc) return rc;
+    void *off_at = nullptr, *dst_at = nullptr, *len_at = nullptr;
+    rc = device_address(c, out_off, true, "out_off", &off_at); if (rc) return rc;
+    if (n == 0) { CU(cudaMemsetAsync(off_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
+    rc = check_side(c, src, true, "src"); if (rc) return rc;
+    rc = device_address(c, dst, false, "dst", &dst_at); if (rc) return rc;
+    rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc;
+    return run_async(c, kind, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst_at, nullptr, dst_cap, (int32_t*)len_at, n,
+                     (int64_t*)off_at, dst_total_cap, (cudaStream_t)stream);
+}
+
+// The asynchronous decodes from page-locked host memory into device memory (the codec's blocks, Unwrap packets; packed
+// when out_off is given), after their argument checks: the capture refusal and the kinds of memory, then run_async.  A
+// packed call with n == 0 writes out_off[0] = 0 on the stream.
+int staged_async(lz4b200_ctx* c, Stage kind, Op op, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                 const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
+                 int64_t dst_total_cap, void* stream, const char* what)
+{
+    CallGuard g(c); if (g.rc) return g.rc;
+    int rc = refuse_capture_async(stream, what); if (rc) return rc;
+    void* at = nullptr;
+    if (out_off) {
+        rc = device_address(c, out_off, true, "out_off", &at); if (rc) return rc;
+        if (n == 0) { CU(cudaMemsetAsync(at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
+    }
+    if (n == 0) return LZ4B200_OK;
+    rc = device_address(c, src, false, "src", &at); if (rc) return rc;
+    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
+    rc = device_address(c, out_len, true, "out_len", &at); if (rc) return rc;
+    // (the stages copy out_len and out_off at the caller's addresses, which the copy engines take for either kind)
+    return run_async(c, kind, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, out_off,
+                     dst_total_cap, (cudaStream_t)stream);
 }
 
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
@@ -1244,16 +1357,8 @@ int lz4b200_encode_batch_packed_from_device_async(lz4b200_ctx* c, const void* sr
     if (n > 0 && (!src || !src_off || !src_len || !dst_cap || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
     for (int32_t i = 0; i < n; i++)
         if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
-    CallGuard g(c); if (g.rc) return g.rc;
-    int rc = refuse_capture_async(stream, "lz4b200_encode_batch_packed_from_device_async"); if (rc) return rc;
-    void *off_at = nullptr, *dst_at = nullptr, *len_at = nullptr;
-    rc = device_address(c, out_off, true, "out_off", &off_at); if (rc) return rc;
-    if (n == 0) { CU(cudaMemsetAsync(off_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
-    rc = check_side(c, src, true, "src"); if (rc) return rc;
-    rc = device_address(c, dst, false, "dst", &dst_at); if (rc) return rc;
-    rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc;
-    return run_async(c, encode_op(mode == LZ4B200_MODE_HC), (const uint8_t*)src, src_off, src_len, (uint8_t*)dst_at, nullptr, dst_cap,
-                     (int32_t*)len_at, n, (int64_t*)off_at, dst_total_cap, (cudaStream_t)stream);
+    return landed_async(c, Stage::CODEC, encode_op(mode == LZ4B200_MODE_HC), src, src_off, src_len, dst_cap, dst, dst_total_cap,
+                        out_off, out_len, n, stream, "lz4b200_encode_batch_packed_from_device_async");
 }
 
 int lz4b200_decode_batch_to_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
@@ -1265,16 +1370,63 @@ int lz4b200_decode_batch_to_device_async(lz4b200_ctx* c, const void* src, const 
     if (n > 0 && (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
     for (int32_t i = 0; i < n; i++)
         if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
-    CallGuard g(c); if (g.rc) return g.rc;
-    int rc = refuse_capture_async(stream, "lz4b200_decode_batch_to_device_async"); if (rc) return rc;
-    if (n == 0) return LZ4B200_OK;
-    void* at = nullptr;
-    rc = device_address(c, src, false, "src", &at); if (rc) return rc;
-    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
-    rc = device_address(c, out_len, true, "out_len", &at); if (rc) return rc;
-    // (the stages copy out_len at the caller's address, which the copy engines take for either kind)
-    return run_async(c, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst,
-                     dst_off, dst_cap, out_len, n, nullptr, 0, (cudaStream_t)stream);
+    return staged_async(c, Stage::CODEC, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, src, src_off, src_len, dst, dst_off,
+                        dst_cap, out_len, n, nullptr, 0, stream, "lz4b200_decode_batch_to_device_async");
+}
+
+int lz4b200_decode_batch_packed_to_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                                void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
+                                                void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n > 0 && (!src || !src_off || !src_len || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    for (int32_t i = 0; i < n; i++)
+        if (src_len[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
+    return staged_async(c, Stage::PLACED_DECODE, Op::DECODE_UNKNOWN, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
+                        dst_total_cap, stream, "lz4b200_decode_batch_packed_to_device_async");
+}
+
+int lz4b200_wrap_batch_packed_from_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                                int high_compression, void* dst, int64_t dst_total_cap, int64_t* out_off,
+                                                int32_t* out_len, int32_t n, void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n > 0 && (!src || !src_off || !src_len || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    // the dense slots hold whole packets: capacity src_len + 8 (wrap_packets)
+    std::vector<int32_t> pcap((size_t)n);
+    for (int32_t i = 0; i < n; i++) {
+        if (src_len[i] < 0 || src_len[i] > INT32_MAX - WRAP_HEADER) return fail(LZ4B200_E_ARG, "input length: negative, or a packet above INT32_MAX bytes");
+        pcap[i] = src_len[i] + WRAP_HEADER;
+    }
+    return landed_async(c, Stage::WRAP_ENCODE, encode_op(high_compression != 0), src, src_off, src_len, pcap.data(), dst,
+                        dst_total_cap, out_off, out_len, n, stream, "lz4b200_wrap_batch_packed_from_device_async");
+}
+
+int lz4b200_unwrap_batch_to_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
+                                         const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
+    if (n > 0 && (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    for (int32_t i = 0; i < n; i++)
+        if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative packet length");
+    return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, nullptr, 0,
+                        stream, "lz4b200_unwrap_batch_to_device_async");
+}
+
+int lz4b200_unwrap_batch_packed_to_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
+                                                void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
+                                                void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n > 0 && (!src || !src_off || !src_len || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    for (int32_t i = 0; i < n; i++)
+        if (src_len[i] < 0) return fail(LZ4B200_E_ARG, "negative packet length");
+    return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
+                        dst_total_cap, stream, "lz4b200_unwrap_batch_packed_to_device_async");
 }
 
 // ---- LZ4Stream (lz4_stream.cuh): the host pipeline, the frames written on the device ----------------------------------
@@ -1396,13 +1548,8 @@ int lz4b200_unwrap_batch_device(lz4b200_ctx* c, const void* src, const int64_t* 
     if (n == 0) return LZ4B200_OK;
     if (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     int rc = call.enter(need_of(c, n, WRAP, 1)); if (rc) return rc;
-    const WrapScratch w = wrap_scratch_at(c->wrap_tmp.p, n);
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n};
-    rc = launched(launch_unwrap_prep(a, w, call.st, &c->launches), "unwrap prep launch"); if (rc) return rc;
-    // the compressed packets, known size (LZ4Codec.cs:595); stored and rejected ones are neutral entries
-    const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, dst_off, w.cap, w.res, n};
-    rc = run_device(c, dec, Op::DECODE_KNOWN, call.st, 0, -1, call.cap); if (rc) return rc;
-    rc = launched(launch_unwrap_finish(a, w, nullptr, call.st, &c->launches), "unwrap finish launch"); if (rc) return rc;
+    rc = run_unwrap(c, a, wrap_scratch_at(c->wrap_tmp.p, n), call.st, call.cap); if (rc) return rc;
     return call.done();
 }
 
@@ -1417,18 +1564,12 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (n == 0) { CU(cudaMemsetAsync(out_off, 0, sizeof(int64_t), call.st)); return LZ4B200_OK; }     // out_off[0] = total = 0
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     int rc = call.enter(need_of(c, n, SCAN | CAPS | WRAP, 1)); if (rc) return rc;
-    const WrapScratch w = wrap_scratch_at(c->wrap_tmp.p, n);
     int32_t* caps = (int32_t*)c->packed_caps.p;
     int* fits = (int*)(caps + n);
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, nullptr, out_len, n};
-    cudaError_t e = launch_unwrap_prep(a, w, call.st, &c->launches);
-    if (e == cudaSuccess) e = place(c, out_len, out_off, n, c->compact_tmp, dst_total_cap, 0, caps, fits, call.st);
-    if (e == cudaSuccess) {
-        const BatchArgs dec{(const uint8_t*)src, w.off, w.len, (uint8_t*)dst, out_off, caps, w.res, n};
-        e = launch_decode(dec, true, c->pinned_lanes(), c->counter(call.cap), c->dev, call.st, &c->launches, fits);
-    }
-    if (e == cudaSuccess) e = launch_unwrap_finish(a, w, fits, call.st, &c->launches);
-    if (e != cudaSuccess) return cuda_fail(e, "packed unwrap launch");
+    const UnwrapPlacement pl{[&] { return place(c, out_len, out_off, n, c->compact_tmp, dst_total_cap, 0, caps, fits, call.st); },
+                             caps, fits};
+    rc = run_unwrap(c, a, wrap_scratch_at(c->wrap_tmp.p, n), call.st, call.cap, &pl); if (rc) return rc;
     return call.done();
 }
 
