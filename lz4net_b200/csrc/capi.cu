@@ -7,11 +7,13 @@
 // (MEM_DEVICE_TO_HOST, MEM_HOST_TO_DEVICE and the packed encode from device memory) and the LZ4Stream and Wrap / Unwrap
 // calls between device and host memory go through it too, skipping the copy of whichever side is already on the device;
 // so does the packed unknown-size decode from host into device memory, whose output offset is carried across the stages
-// on the device (lz4_packed.cuh).  What a stage runs is named by its caller (Stage); the codec operation by Op.
+// on the device (Placement, lz4_packed.cuh).  What a stage runs is named by its caller (Stage) and mapped to its sequence
+// in one place (run_stage); the codec operation is named by Op.
 // The asynchronous calls between device memory and page-locked host memory (run_async: the packed encode and Wrap into it,
-// the decode, packed decode and Unwrap from it) cut their stages by the same plan, enqueue them on streams and buffers of
-// their own and return without waiting; the packed encodes' stages land in host memory from a kernel (lz4_land.cuh), since
-// where a stage lands is known only on the device, and the Unwraps read their headers on the device (run_unwrap).
+// the decode, packed decode and Unwrap from it, checked by landed_async and staged_async) cut their stages by the same
+// plan, run the same stage sequences on streams and buffers of their own and return without waiting; the packed encodes'
+// stages land in host memory from a kernel (lz4_land.cuh), since where a stage lands is known only on the device, and the
+// Unwraps read their headers on the device (run_unwrap).
 // The device-memory calls enter through one path (DeviceCall): each states what it takes from the context (Need), which
 // admits it to a CUDA graph capture or grows an eager call's scratch; lz4b200_reserve grows to the same needs.
 // The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
@@ -150,18 +152,40 @@ void par_memcpy(void* dst, const void* src, size_t n)
 {
     par_ranges(n, STAGE_PARALLEL_MIN, [&](size_t lo, size_t hi) { std::memcpy((uint8_t*)dst + lo, (const uint8_t*)src + lo, hi - lo); });
 }
-bool is_pageable(const void* p)
+// What CUDA says p is: its kind of memory (cudaMemoryTypeUnregistered for pageable memory, or when CUDA cannot tell), its
+// device and its device address.
+cudaPointerAttributes pointer_attributes(const void* p)
 {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return true; }
-    return a.type == cudaMemoryTypeUnregistered;
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+    return a;
+}
+bool is_pageable(const void* p) { return pointer_attributes(p).type == cudaMemoryTypeUnregistered; }
+
+// A stream of the pipeline and the buffers of the stage on it.  `done`: the slot's last work of the call is enqueued;
+// `carried`: the stage's placement or landing step, which leaves the running total in the slot's carry cell, is enqueued
+// (the packed forms); meta, offs, scan: the stage's device metadata, scan offsets and scan scratch.
+struct SlotBase {
+    cudaStream_t stream = nullptr;
+    cudaEvent_t done = nullptr, carried = nullptr;
+    DevBuf meta, offs, scan;
+};
+cudaError_t create_slot(SlotBase& s)
+{
+    cudaError_t e = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.carried, cudaEventDisableTiming);
+    return e;
+}
+void destroy_slot(SlotBase& s)
+{
+    if (s.done) cudaEventDestroy(s.done);
+    if (s.carried) cudaEventDestroy(s.carried);
+    if (s.stream) cudaStreamDestroy(s.stream);
 }
 
-struct Slot {
-    cudaStream_t stream = nullptr;
-    cudaEvent_t done = nullptr;
-    cudaEvent_t carried = nullptr;         // the packed decode into device memory: the stage's placement step is enqueued
-    DevBuf src, dst, meta, packed, offs, scan;
+struct Slot : SlotBase {
+    DevBuf src, dst, packed;
     PinBuf hmeta, hsrc, hout;              // pinned: chunk metadata, staged pageable sources, staged outputs
 };
 
@@ -169,11 +193,8 @@ struct Slot {
 // the slots above before it returns, and an asynchronous stage may still be in flight then.  Two, so that one stage's
 // transfer overlaps the next one's kernels.
 constexpr int NASYNC = 2;
-struct AsyncSlot {
-    cudaStream_t stream = nullptr;
-    cudaEvent_t done = nullptr;            // the slot's last stage of the call is enqueued (the caller's stream joins it)
-    cudaEvent_t carried = nullptr;         // the encode: the stage's landing step, which leaves the running total, is enqueued
-    DevBuf io, meta, offs, scan;           // io: the encode's dense output slots, or the decode's staged source
+struct AsyncSlot : SlotBase {
+    DevBuf io;                             // the encode's dense output slots, or the decode's staged source
 };
 // The page-locked metadata of one asynchronous call, which the device reads after the call has returned: taken again once
 // `done`, recorded behind the call, has fired.
@@ -295,12 +316,14 @@ int capture_of(cudaStream_t st, Capture* cap)
     return LZ4B200_OK;
 }
 
-// The calls that synchronise refuse a capturing stream before any CUDA work, which leaves the caller's capture valid.
-int refuse_capture(void* stream, const char* what)
+// The calls that synchronise with the host, and the asynchronous calls, whose metadata is host data a graph would have to
+// keep alive, refuse a capturing stream before any CUDA work, which leaves the caller's capture valid.
+int refuse_capture(void* stream, const char* what, bool synchronises = true)
 {
     Capture cap;
     int rc = capture_of((cudaStream_t)stream, &cap); if (rc) return rc;
-    return cap.on ? fail(LZ4B200_E_ARG, std::string(what) + " synchronises with the host: it cannot be enqueued on a capturing stream")
+    return cap.on ? fail(LZ4B200_E_ARG, std::string(what) + (synchronises ? " synchronises with the host: it" : "") +
+                                            " cannot be enqueued on a capturing stream")
                   : LZ4B200_OK;
 }
 
@@ -375,6 +398,14 @@ struct DeviceCall : CallGuard {
 
 int launched(cudaError_t e, const char* what) { return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, what); }
 
+// The lengths of a batch of blocks or packets (unit) whose arrays are on the host: src_len and, when given, dst_cap.
+int check_lengths(const int32_t* src_len, const int32_t* dst_cap, int32_t n, const char* unit)
+{
+    for (int32_t i = 0; i < n; i++)
+        if (src_len[i] < 0 || (dst_cap && dst_cap[i] < 0)) return fail(LZ4B200_E_ARG, std::string("negative ") + unit + " length");
+    return LZ4B200_OK;
+}
+
 // Decode group size from the ratio compressed/raw of a batch (tools/sweep.py): incompressible data is long literal runs
 // (whole warps, 128-bit copies), nearly-empty streams are long matches, everything between is sequence-dense (the
 // denser, the smaller the group: 8 lanes around ratio 0.58, 4 lanes around 0.37; both output-staged).
@@ -425,19 +456,39 @@ int run_wrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, Op op, cu
     return launched(launch_wrap_finish(a, w, st, &c->launches), "wrap finish launch");
 }
 
-// What the packed Unwraps do between the prep and the decode: `place` enqueues the placement of the sizes the prep left in
-// out_len, which writes the decode's capacities (caps) and the "fits" flag that both the decode and the finish run behind.
-struct UnwrapPlacement { std::function<cudaError_t()> place; const int32_t* caps; const int* fits; };
+// The placement of a packed decode (lz4_packed.cuh): the sizes scanned into `off` (scan: the scan's scratch), then each
+// block's capacity (its size + room) into caps, and the "fits" flag against total_cap.  A pipeline stage places behind the
+// previous one: it waits on `after`, starts from the running total in `base` (null for the first stage), leaves its
+// absolute offsets in abs_off and the running total in `total`, and records `placed` once placed.  A batch placed in one
+// piece leaves those null.
+struct Placement {
+    int64_t* off; void* scan; size_t scan_bytes;
+    int64_t total_cap; int32_t room; int32_t* caps; int* fits;
+    cudaEvent_t after = nullptr; const int64_t* base = nullptr; int64_t* abs_off = nullptr; int64_t* total = nullptr;
+    cudaEvent_t placed = nullptr;
+};
+
+cudaError_t place(lz4b200_ctx* c, const int32_t* size, int32_t n, const Placement& p, cudaStream_t st)
+{
+    cudaError_t e = launch_compact(nullptr, nullptr, size, nullptr, p.off, n, p.scan, p.scan_bytes, c->dev, st, &c->launches);
+    if (e == cudaSuccess && p.after) e = cudaStreamWaitEvent(st, p.after, 0);
+    if (e == cudaSuccess)
+        e = launch_packed_prep(size, p.off, n, p.total_cap, p.room, p.caps, p.fits, st, &c->launches, p.base, p.abs_off, p.total);
+    if (e == cudaSuccess && p.placed) e = cudaEventRecord(p.placed, st);
+    return e;
+}
 
 // An Unwrap of the packets of a (src / src_off / src_len; outputs at dst + dst_off, capacities dst_cap, null = no limit):
 // prep (each header, read on the device: a decode entry for a compressed packet, a neutral one for a stored or rejected
-// packet) -> [the placement of the packed forms] -> the known-size decode -> finish (the stored copies, out_len = bytes
-// restored or the packet's status).  The counterpart of run_wrap, for the device calls and the asynchronous stages alike.
+// packet) -> [the packed forms: the placement of the sizes the prep left in out_len, which writes the decode's capacities
+// and the "fits" flag that both the decode and the finish run behind] -> the known-size decode -> finish (the stored
+// copies, out_len = bytes restored or the packet's status).  The counterpart of run_wrap, for the device calls and the
+// asynchronous stages alike.
 int run_unwrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, cudaStream_t st, const Capture& cap = {},
-               const UnwrapPlacement* placed = nullptr)
+               const Placement* placed = nullptr)
 {
     int rc = launched(launch_unwrap_prep(a, w, st, &c->launches), "unwrap prep launch"); if (rc) return rc;
-    if (placed) { rc = launched(placed->place(), "unwrap placement launch"); if (rc) return rc; }
+    if (placed) { rc = launched(place(c, a.out_len, a.n_blocks, *placed, st), "unwrap placement launch"); if (rc) return rc; }
     // the compressed packets, known size (LZ4Codec.cs:595); stored and rejected ones are neutral entries
     const BatchArgs dec{a.src, w.off, w.len, a.dst, a.dst_off, placed ? placed->caps : w.cap, w.res, a.n_blocks};
     const int* fits = placed ? placed->fits : nullptr;
@@ -446,16 +497,37 @@ int run_unwrap(lz4b200_ctx* c, const BatchArgs& a, const WrapScratch& w, cudaStr
     return launched(launch_unwrap_finish(a, w, fits, st, &c->launches), "unwrap finish launch");
 }
 
-// The placement of the packed decodes (lz4_packed.cuh): n sizes scanned into the offsets `off`, then each block's capacity
-// (its size + room) and the "fits" flag.  A pipeline stage places behind the previous one (waits on `after`, starts from
-// `base`: null for the first stage) and leaves its absolute offsets and the running total (lz4_packed.cuh).
-cudaError_t place(lz4b200_ctx* c, const int32_t* size, int64_t* off, int32_t n, const DevBuf& scan, int64_t total_cap,
-                  int32_t room, int32_t* caps, int* fits, cudaStream_t st, cudaEvent_t after = nullptr,
-                  const int64_t* base = nullptr, int64_t* abs_off = nullptr, int64_t* total = nullptr)
+// The packed unknown-size decode of a, whose dst_off and dst_cap are the placement's abs_off (or off) and caps: measure
+// (no capacity) -> place the sizes, with the room of an unknown-size decode -> the decode behind the "fits" flag, whose
+// decoders leave at once when the total does not fit, so out_len keeps the measured sizes and dst is untouched.
+int run_placed_decode(lz4b200_ctx* c, const BatchArgs& a, Placement p, cudaStream_t st, const Capture& cap = {})
 {
-    cudaError_t e = launch_compact(nullptr, nullptr, size, nullptr, off, n, scan.p, scan.cap, c->dev, st, &c->launches);
-    if (e == cudaSuccess && after) e = cudaStreamWaitEvent(st, after, 0);
-    return e == cudaSuccess ? launch_packed_prep(size, off, n, total_cap, room, caps, fits, st, &c->launches, base, abs_off, total) : e;
+    p.room = PACKED_ROOM_UNKNOWN;
+    BatchArgs sizes = a; sizes.dst_cap = nullptr;
+    cudaError_t e = launch_measure(sizes, false, c->dev, st, &c->launches);
+    if (e == cudaSuccess) e = place(c, a.out_len, a.n_blocks, p, st);
+    if (e == cudaSuccess) e = launch_decode(a, false, c->pinned_lanes(), c->counter(cap), c->dev, st, &c->launches, p.fits);
+    return launched(e, "packed measure / placement / decode launch");
+}
+
+// What a stage of run_host or run_async runs on its blocks a (lanes, hc_large: its decoder and HC arena, stage_lanes and
+// stage_hc_large): w is the stage's packet view (WRAP_ENCODE, UNWRAP), placed its placement (PLACED_DECODE, a packed
+// UNWRAP) and stored a FRAMED_DECODE's stored lengths.
+int run_stage(lz4b200_ctx* c, Stage kind, Op op, const BatchArgs& a, int lanes, int32_t hc_large, const WrapScratch& w,
+              const Placement* placed, const int32_t* stored, cudaStream_t st)
+{
+    switch (kind) {
+    case Stage::CODEC:
+    case Stage::STREAM_ENCODE: return run_device(c, a, op, st, lanes, hc_large);
+    case Stage::WRAP_ENCODE: return run_wrap(c, a, w, op, st, hc_large);
+    case Stage::FRAMED_DECODE: {
+        int rc = run_device(c, a, op, st, lanes); if (rc) return rc;
+        return launched(launch_stream_stored(a, stored, st, &c->launches), "stored copy launch");
+    }
+    case Stage::PLACED_DECODE: return run_placed_decode(c, a, *placed, st);
+    case Stage::UNWRAP: return run_unwrap(c, a, w, st, {}, placed);
+    }
+    return fail(LZ4B200_E_ARG, "unknown stage kind");
 }
 
 // ---- the stage plan of the host pipeline, shared by run_host and the asynchronous calls (run_async) ------------------
@@ -506,10 +578,11 @@ StageSpan fill_stage(const Meta& h, int32_t b0, int32_t b1, const int64_t* src_o
     return sp;
 }
 
-// The decoder of a decode stage, from its compression ratio (0: the context's pinned choice, or not a decode).
+// The decoder of a decode stage, from its compression ratio (0: the context's pinned choice, or not a decode, or a placed
+// stage, whose decoded sizes are known on the device only: dst_cap == nullptr).
 int stage_lanes(const lz4b200_ctx* c, Op op, const int32_t* src_len, const int32_t* dst_cap, int32_t b0, int32_t b1)
 {
-    if (!is_decode(op) || !c->decode_lanes_auto) return 0;
+    if (!is_decode(op) || !c->decode_lanes_auto || !dst_cap) return 0;
     double cs = 0, rs = 0;
     for (int32_t i = b0; i < b1; i++) { cs += src_len[i]; rs += dst_cap[i]; }
     return lanes_for_ratio(rs > 0 ? cs / rs : 1.0, b1 - b0, c->dev);
@@ -555,8 +628,7 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
              const uint8_t* stored = nullptr)
 {
     const bool measure = is_measure(op), framed = kind == Stage::FRAMED_DECODE, placed = kind == Stage::PLACED_DECODE;
-    for (int32_t i = 0; i < n; i++)
-        if (src_len[i] < 0 || (dst_cap && dst_cap[i] < 0)) return fail(LZ4B200_E_ARG, "negative block length");
+    int rc = check_lengths(src_len, dst_cap, n, "block"); if (rc) return rc;
     const bool src_pageable = !src_dev && is_pageable(src), dst_pageable = !measure && !dst_dev && is_pageable(dst);
     enum Mode { NONE, PER_BLOCK, RUNS, SCATTER, APPEND };
     struct Pending { int32_t b0, b1; Mode mode; };
@@ -640,7 +712,7 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
     while (b0 < n) {
         const int32_t b1 = stage_end(c, src_len, measure || dst_dev ? nullptr : dst_cap, b0, n, !src_dev);
         const int s = k % NSLOT; k++;
-        int rc = retire(s); if (rc) return rc;
+        rc = retire(s); if (rc) return rc;
         Slot& sl = c->slot[s];
         const int32_t m = b1 - b0;
         const Mode mode = measure || dst_dev ? NONE : !dst_off ? APPEND : m <= 8 ? PER_BLOCK : op == Op::DECODE_KNOWN ? RUNS : SCATTER;
@@ -662,41 +734,22 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
             CU(cudaMemcpyAsync(sl.src.p, from, sbytes, cudaMemcpyHostToDevice, sl.stream));
         }
         const BatchArgs a{src_dev ? src : (const uint8_t*)sl.src.p, d.so, d.sl, dst_dev ? dst : (uint8_t*)sl.dst.p, d.dof, d.dc, d.out, m};
-        // (a placed stage's decoded size is known on the device only)
-        const int lanes = placed ? 0 : stage_lanes(c, op, src_len, dst_cap, b0, b1);
-        const int32_t hc_large = stage_hc_large(op, src_len, b0, b1);
-        switch (kind) {
-        case Stage::CODEC:
-        case Stage::STREAM_ENCODE:
-            rc = run_device(c, a, op, sl.stream, lanes, hc_large);
-            break;
-        case Stage::WRAP_ENCODE:
-            rc = run_wrap(c, a, wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), op, sl.stream, hc_large);
-            break;
-        case Stage::FRAMED_DECODE:
-            rc = run_device(c, a, op, sl.stream, lanes);
-            if (!rc) rc = launched(launch_stream_stored(a, d.aux, sl.stream, &c->launches), "stored copy launch");
-            break;
-        case Stage::PLACED_DECODE: {
-            // measure -> scan -> placement, behind the previous stage's -> decode behind the stage's flag
+        Placement pl{};
+        if (placed) {
+            // behind the previous stage's placement; the stage's "fits" flag lives behind its arrays (Meta)
             CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
             const int prev = (s + NSLOT - 1) % NSLOT;
-            int* fits = (int*)d.off;
-            BatchArgs sizes = a; sizes.dst_cap = nullptr;
-            cudaError_t e = launch_measure(sizes, false, c->dev, sl.stream, &c->launches);
-            if (e == cudaSuccess) e = place(c, d.out, (int64_t*)sl.offs.p, m, sl.scan, dst_total_cap, PACKED_ROOM_UNKNOWN, d.dc, fits,
-                                            sl.stream, b0 > 0 ? c->slot[prev].carried : nullptr, b0 > 0 ? c->carry + prev : nullptr,
-                                            d.dof, c->carry + s);
-            if (e != cudaSuccess) return cuda_fail(e, "packed measure / placement launch");
-            CU(cudaEventRecord(sl.carried, sl.stream));
-            e = launch_decode(a, false, c->pinned_lanes(), c->counter(), c->dev, sl.stream, &c->launches, fits);
-            if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
+            pl = Placement{(int64_t*)sl.offs.p, sl.scan.p, sl.scan.cap, dst_total_cap, 0, d.dc, (int*)d.off,
+                           b0 > 0 ? c->slot[prev].carried : nullptr, b0 > 0 ? c->carry + prev : nullptr, d.dof, c->carry + s, sl.carried};
+        }
+        rc = run_stage(c, kind, op, a, stage_lanes(c, op, src_len, dst_cap, b0, b1), stage_hc_large(op, src_len, b0, b1),
+                       wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), placed ? &pl : nullptr, d.aux,
+                       sl.stream);
+        if (rc) return rc;
+        if (placed) {
             CU(cudaMemcpyAsync(h.dof, d.dof, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, sl.stream));
             CU(cudaMemcpyAsync(h.off, c->carry + s, sizeof(int64_t), cudaMemcpyDeviceToHost, sl.stream));
-            break;
         }
-        }
-        if (rc) return rc;
         if (mode >= SCATTER) {
             // the outputs back to back: compacted, or an LZ4Stream encode's frames (sizes -> scan -> headers + payloads)
             const bool frames = kind == Stage::STREAM_ENCODE;
@@ -729,7 +782,7 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
         pend[s] = Pending{b0, b1, mode}; busy[s] = true;
         b0 = b1;
     }
-    for (int i = 0; i < NSLOT; i++) { int rc = retire((k + i) % NSLOT); if (rc) return rc; }
+    for (int i = 0; i < NSLOT; i++) { rc = retire((k + i) % NSLOT); if (rc) return rc; }
     if (out_off) out_off[n] = written;
     return LZ4B200_OK;
 }
@@ -738,8 +791,7 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
 // side that must be host memory is not device memory (pageable, page-locked or managed host memory all copy).
 int check_side(const lz4b200_ctx* c, const void* p, bool device, const char* what)
 {
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+    const cudaPointerAttributes a = pointer_attributes(p);
     const bool on_device = a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
     if (device && !(on_device && a.device == c->device))
         return fail(LZ4B200_E_ARG, std::string(what) + " must be device memory of the context's GPU");
@@ -753,8 +805,7 @@ int check_side(const lz4b200_ctx* c, const void* p, bool device, const char* wha
 // lz4b200_host_register'd range), or, when `device_ok`, device memory of the context's GPU.
 int device_address(const lz4b200_ctx* c, const void* p, bool device_ok, const char* what, void** at)
 {
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+    const cudaPointerAttributes a = pointer_attributes(p);
     if (a.type == cudaMemoryTypeHost && a.devicePointer) { *at = a.devicePointer; return LZ4B200_OK; }
     if (device_ok && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == c->device) {
         *at = const_cast<void*>(p);
@@ -762,15 +813,6 @@ int device_address(const lz4b200_ctx* c, const void* p, bool device_ok, const ch
     }
     return fail(LZ4B200_E_ARG, std::string(what) + (device_ok ? " must be device memory of the context's GPU or page-locked host memory"
                                                               : " must be page-locked host memory the device can address"));
-}
-
-// The asynchronous calls refuse a capturing stream before any CUDA work: their metadata is host data a graph would have
-// to keep alive.
-int refuse_capture_async(void* stream, const char* what)
-{
-    Capture cap;
-    int rc = capture_of((cudaStream_t)stream, &cap); if (rc) return rc;
-    return cap.on ? fail(LZ4B200_E_ARG, std::string(what) + " cannot be enqueued on a capturing stream") : LZ4B200_OK;
 }
 
 // A page-locked metadata block of at least `bytes` whose last call the device has passed (cudaEventQuery, never waited
@@ -804,7 +846,7 @@ int take_meta(lz4b200_ctx* c, size_t bytes, MetaBlock** out)
 
 // The stages of an asynchronous call, cut and described as run_host cuts and describes them (stage_end, fill_stage,
 // stage_lanes, stage_hc_large), enqueued on the context's NASYNC streams in turn, forked from `caller` and joined back to
-// it; nothing is waited on unless a buffer must grow.  What a stage runs is its kind's sequence in run_host:
+// it; nothing is waited on unless a buffer must grow.  What a stage runs is its kind's sequence (run_stage), as in run_host:
 //  - The packed encodes (enc: CODEC with an encode, WRAP_ENCODE): src is device memory, dst the device address of
 //    page-locked host memory, out_off / out_len device addresses.  A stage encodes (or wraps, run_wrap: capacity src_len + 8
 //    per packet, the stage weighed by it) into its dense slots (AsyncSlot::io), scans the lengths, and lands
@@ -814,8 +856,9 @@ int take_meta(lz4b200_ctx* c, size_t bytes, MetaBlock** out)
 //    up a stage at a time on the copy engine, weighed by src_len; the decoders write dst (device memory) in place.  A
 //    CODEC decode writes at dst_off; an UNWRAP reads the headers from the staged bytes on the device (run_unwrap), since
 //    work still queued on `caller` may write them.  The packed forms (placed: PLACED_DECODE, an UNWRAP without dst_off)
-//    measure, scan and place their stage behind the previous one's from the same carry cells (place), then decode behind
-//    the stage's "fits" flag; their absolute offsets are copied to out_off, the last stage's running total to out_off[n].
+//    measure (PLACED_DECODE) or prep (UNWRAP), scan and place their stage behind the previous one's from the same carry
+//    cells (place), then decode behind the stage's "fits" flag; their absolute offsets are copied to out_off, the last
+//    stage's running total to out_off[n].
 //    The stage's results are copied to out_len (device or page-locked memory).
 // Calls are chained through async_done; the call's metadata block is taken again once the caller's stream has passed it.
 int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
@@ -834,28 +877,28 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
     }
     MetaBlock* blk = nullptr;
     int rc = take_meta(c, bytes, &blk); if (rc) return rc;
-    size_t need[NASYNC][4] = {};                                              // io, meta, offs, scan
+    struct Sizes { size_t io = 0, meta = 0, offs = 0, scan = 0; } need[NASYNC];      // each slot's buffers, for its largest stage
     for (size_t k = 0; k < plan.size(); k++) {
         Plan& p = plan[k];
         const int32_t m = p.b1 - p.b0;
         p.sp = fill_stage(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, src_off, src_len, dst_off, dst_cap, enc, !enc, false,
                           placed, nullptr);
-        size_t* nd = need[k % NASYNC];
-        nd[0] = std::max(nd[0], (size_t)(enc ? p.sp.dsum : p.sp.shi - p.sp.slo) + 64);
-        nd[1] = std::max(nd[1], async_meta_bytes(m));
-        if (enc || placed) { nd[2] = std::max(nd[2], sizeof(int64_t) * (size_t)(m + 1)); nd[3] = std::max(nd[3], compact_tmp_bytes(m)); }
+        Sizes& nd = need[k % NASYNC];
+        nd.io = std::max(nd.io, (size_t)(enc ? p.sp.dsum : p.sp.shi - p.sp.slo) + 64);
+        nd.meta = std::max(nd.meta, async_meta_bytes(m));
+        if (enc || placed) { nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(m + 1)); nd.scan = std::max(nd.scan, compact_tmp_bytes(m)); }
     }
     // growth: an earlier call may still be using the buffers
     bool grow = false;
     for (int s = 0; s < NASYNC; s++) {
         const AsyncSlot& sl = c->aslot[s];
-        grow |= need[s][0] > sl.io.cap || need[s][1] > sl.meta.cap || need[s][2] > sl.offs.cap || need[s][3] > sl.scan.cap;
+        grow |= need[s].io > sl.io.cap || need[s].meta > sl.meta.cap || need[s].offs > sl.offs.cap || need[s].scan > sl.scan.cap;
     }
     if (grow) {
         CU(cudaDeviceSynchronize());
         for (int s = 0; s < NASYNC; s++) {
             AsyncSlot& sl = c->aslot[s];
-            CU(sl.io.reserve(need[s][0])); CU(sl.meta.reserve(need[s][1])); CU(sl.offs.reserve(need[s][2])); CU(sl.scan.reserve(need[s][3]));
+            CU(sl.io.reserve(need[s].io)); CU(sl.meta.reserve(need[s].meta)); CU(sl.offs.reserve(need[s].offs)); CU(sl.scan.reserve(need[s].scan));
         }
     }
     const int used = (int)std::min<size_t>(plan.size(), NASYNC);
@@ -878,40 +921,13 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
             // (a packed Unwrap's prep reads no capacity: the placement writes the decode's into d.dc)
             const BatchArgs a{enc ? src : (const uint8_t*)sl.io.p, d.so, d.sl, enc ? (uint8_t*)sl.io.p : dst, d.dof,
                               kind == Stage::UNWRAP && placed ? nullptr : d.dc, d.out, m};
-            const WrapScratch w = wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m);
-            int* fits = async_fits(sl.meta.p, m);
             int64_t* offs = (int64_t*)sl.offs.p;
-            // a packed stage's sizes scanned and placed behind the previous stage's (lz4_packed.cuh); the next one follows
-            auto place_stage = [&](int32_t room) {
-                cudaError_t e = place(c, d.out, offs, m, sl.scan, dst_total_cap, room, d.dc, fits, sl.stream,
-                                      k > 0 ? c->aslot[prev].carried : nullptr, k > 0 ? carry + prev : nullptr, d.dof, carry + s);
-                return e == cudaSuccess ? cudaEventRecord(sl.carried, sl.stream) : e;
-            };
-            int rc = LZ4B200_OK;
-            switch (kind) {
-            case Stage::CODEC:
-                rc = run_device(c, a, op, sl.stream, stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), stage_hc_large(op, src_len, p.b0, p.b1));
-                break;
-            case Stage::WRAP_ENCODE:
-                rc = run_wrap(c, a, w, op, sl.stream, stage_hc_large(op, src_len, p.b0, p.b1));
-                break;
-            case Stage::UNWRAP: {
-                const UnwrapPlacement pl{[&] { return place_stage(0); }, d.dc, fits};
-                rc = run_unwrap(c, a, w, sl.stream, Capture{}, placed ? &pl : nullptr);
-                break;
-            }
-            case Stage::PLACED_DECODE: {
-                // measure -> scan -> placement, behind the previous stage's -> decode behind the stage's flag (run_host's)
-                BatchArgs sizes = a; sizes.dst_cap = nullptr;
-                cudaError_t e = launch_measure(sizes, false, c->dev, sl.stream, &c->launches);
-                if (e == cudaSuccess) e = place_stage(PACKED_ROOM_UNKNOWN);
-                if (e == cudaSuccess) e = launch_decode(a, false, c->pinned_lanes(), c->counter(), c->dev, sl.stream, &c->launches, fits);
-                rc = launched(e, "packed measure / placement / decode launch");
-                break;
-            }
-            default:
-                return fail(LZ4B200_E_ARG, "run_async: no asynchronous form of this stage");
-            }
+            // a packed stage places behind the previous stage's placement (lz4_packed.cuh); the next one follows
+            const Placement pl{offs, sl.scan.p, sl.scan.cap, dst_total_cap, 0, d.dc, async_fits(sl.meta.p, m),
+                               k > 0 ? c->aslot[prev].carried : nullptr, k > 0 ? carry + prev : nullptr, d.dof, carry + s, sl.carried};
+            int rc = run_stage(c, kind, op, a, stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), stage_hc_large(op, src_len, p.b0, p.b1),
+                               wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), placed ? &pl : nullptr,
+                               nullptr, sl.stream);
             if (rc) return rc;
             if (!enc) {
                 CU(cudaMemcpyAsync(out_len + p.b0, d.out, sizeof(int32_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
@@ -946,36 +962,65 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
     return rc ? rc : jr;
 }
 
-// The asynchronous packed encodes from device memory into page-locked host memory (the codec's blocks, Wrap packets),
-// after their argument checks: the capture refusal and the kinds of memory, then run_async.  n == 0 writes out_off[0] = 0
-// on the stream.
-int landed_async(lz4b200_ctx* c, Stage kind, Op op, const void* src, const int64_t* src_off, const int32_t* src_len,
+// The capacities of n Wrap packets, src_len[i] + 8 (the largest a packet gets), into caps; an input whose packet would not
+// fit an int32 is refused.  Packets that go into the caller's slots (slot_cap) must each fit their slot.
+int wrap_caps(const int32_t* src_len, const int32_t* slot_cap, int32_t n, std::vector<int32_t>& caps)
+{
+    caps.resize((size_t)n);
+    for (int32_t i = 0; i < n; i++) {
+        if (src_len[i] < 0 || src_len[i] > INT32_MAX - WRAP_HEADER) return fail(LZ4B200_E_ARG, "input length: negative, or a packet above INT32_MAX bytes");
+        if (slot_cap && (int64_t)slot_cap[i] < (int64_t)src_len[i] + WRAP_HEADER) return fail(LZ4B200_E_ARG, "dst_cap[i] < src_len[i] + 8");
+        caps[i] = src_len[i] + WRAP_HEADER;
+    }
+    return LZ4B200_OK;
+}
+
+// The asynchronous packed encodes from device memory into page-locked host memory (the codec's blocks; Wrap packets,
+// kind WRAP_ENCODE, whose capacities are their own): the argument checks, the capture refusal and the kinds of memory,
+// then run_async.  n == 0 writes out_off[0] = 0 on the stream.
+int landed_async(lz4b200_ctx* c, Stage kind, int mode, const void* src, const int64_t* src_off, const int32_t* src_len,
                  const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
                  void* stream, const char* what)
 {
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
+    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    const bool wrap = kind == Stage::WRAP_ENCODE;
+    if (n > 0 && (!src || !src_off || !src_len || (!wrap && !dst_cap) || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    // a Wrap's dense slots hold whole packets
+    std::vector<int32_t> pcap;
+    int rc = wrap ? wrap_caps(src_len, nullptr, n, pcap) : check_lengths(src_len, dst_cap, n, "block"); if (rc) return rc;
+    if (wrap) dst_cap = pcap.data();
     CallGuard g(c); if (g.rc) return g.rc;
-    int rc = refuse_capture_async(stream, what); if (rc) return rc;
+    rc = refuse_capture(stream, what, false); if (rc) return rc;
     void *off_at = nullptr, *dst_at = nullptr, *len_at = nullptr;
     rc = device_address(c, out_off, true, "out_off", &off_at); if (rc) return rc;
     if (n == 0) { CU(cudaMemsetAsync(off_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
     rc = check_side(c, src, true, "src"); if (rc) return rc;
     rc = device_address(c, dst, false, "dst", &dst_at); if (rc) return rc;
     rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc;
-    return run_async(c, kind, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst_at, nullptr, dst_cap, (int32_t*)len_at, n,
-                     (int64_t*)off_at, dst_total_cap, (cudaStream_t)stream);
+    return run_async(c, kind, encode_op(mode == LZ4B200_MODE_HC), (const uint8_t*)src, src_off, src_len, (uint8_t*)dst_at, nullptr,
+                     dst_cap, (int32_t*)len_at, n, (int64_t*)off_at, dst_total_cap, (cudaStream_t)stream);
 }
 
-// The asynchronous decodes from page-locked host memory into device memory (the codec's blocks, Unwrap packets; packed
-// when out_off is given), after their argument checks: the capture refusal and the kinds of memory, then run_async.  A
-// packed call with n == 0 writes out_off[0] = 0 on the stream.
-int staged_async(lz4b200_ctx* c, Stage kind, Op op, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
-                 const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
+// The asynchronous decodes from page-locked host memory into device memory (the codec's blocks; Unwrap packets, kind
+// UNWRAP), into the caller's slots or packed (out_off, dst_total_cap; no dst_off, dst_cap): the argument checks, the
+// capture refusal and the kinds of memory, then run_async.  A packed call with n == 0 writes out_off[0] = 0 on the stream.
+int staged_async(lz4b200_ctx* c, Stage kind, Op op, bool packed, const void* src, const int64_t* src_off, const int32_t* src_len,
+                 void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
                  int64_t dst_total_cap, void* stream, const char* what)
 {
+    const char* unit = kind == Stage::UNWRAP ? "packet" : "block";
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (packed && (n < 0 || !out_off || dst_total_cap < 0)) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n < 0) return fail(LZ4B200_E_ARG, std::string("negative ") + unit + " count");
+    if (n > 0 && (!src || !src_off || !src_len || !dst || (!packed && (!dst_off || !dst_cap)) || !out_len))
+        return fail(LZ4B200_E_ARG, "null argument");
+    int rc = check_lengths(src_len, dst_cap, n, unit); if (rc) return rc;
     CallGuard g(c); if (g.rc) return g.rc;
-    int rc = refuse_capture_async(stream, what); if (rc) return rc;
+    rc = refuse_capture(stream, what, false); if (rc) return rc;
     void* at = nullptr;
-    if (out_off) {
+    if (packed) {
         rc = device_address(c, out_off, true, "out_off", &at); if (rc) return rc;
         if (n == 0) { CU(cudaMemsetAsync(at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
     }
@@ -1020,6 +1065,19 @@ int batch(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t
     }
     return run_host(c, Stage::CODEC, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, out_off,
                     dst_total_cap, src_dev, dst_dev, (cudaStream_t)stream);
+}
+
+// The packed encode into host memory, from host memory (MEM_HOST) or device memory (MEM_DEVICE_TO_HOST): n == 0 writes
+// out_off[0] = 0.
+int encode_packed(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, const int32_t* dst_cap, void* dst,
+                  int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n, int mode, int mem, void* stream)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
+    if (n < 0 || !out_off) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
+    return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, encode_op(mode == LZ4B200_MODE_HC), mem, stream, out_off,
+                 dst_total_cap);
 }
 
 // The single-block entry points are re-entrant like the reference's (SURVEY 8b "Threading"): every calling thread gets
@@ -1141,15 +1199,11 @@ int wrap_packets(lz4b200_ctx* c, const void* src, const int64_t* src_off, const 
     if (n == 0) { if (out_off) out_off[0] = 0; return LZ4B200_OK; }
     if (!src || !src_off || !src_len || !dst || !out_len || (dst_off ? !dst_cap : !out_off)) return fail(LZ4B200_E_ARG, "null argument");
     // the slots' dense layout holds packets, whatever room the caller's slots have
-    std::vector<int32_t> pcap((size_t)n);
-    for (int32_t i = 0; i < n; i++) {
-        if (src_len[i] < 0 || src_len[i] > INT32_MAX - WRAP_HEADER) return fail(LZ4B200_E_ARG, "input length: negative, or a packet above INT32_MAX bytes");
-        if (dst_off && (int64_t)dst_cap[i] < (int64_t)src_len[i] + WRAP_HEADER) return fail(LZ4B200_E_ARG, "dst_cap[i] < src_len[i] + 8");
-        pcap[i] = src_len[i] + WRAP_HEADER;
-    }
+    std::vector<int32_t> pcap;
+    int rc = wrap_caps(src_len, dst_off ? dst_cap : nullptr, n, pcap); if (rc) return rc;
     CallGuard g(c); if (g.rc) return g.rc;
     if (src_dev) {
-        int rc = refuse_capture(stream, "a Wrap from device memory"); if (rc) return rc;
+        rc = refuse_capture(stream, "a Wrap from device memory"); if (rc) return rc;
         rc = check_side(c, src, true, "src"); if (rc) return rc;
         rc = check_side(c, dst, false, "dst"); if (rc) return rc;
     }
@@ -1264,16 +1318,8 @@ int lz4b200_create(lz4b200_ctx** out, int device)
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->inner, cudaEventDisableTiming);
     }
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->entry, cudaEventDisableTiming);
-    for (int i = 0; i < NSLOT && e == cudaSuccess; i++) {
-        e = cudaStreamCreateWithFlags(&c->slot[i].stream, cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->slot[i].done, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->slot[i].carried, cudaEventDisableTiming);
-    }
-    for (int i = 0; i < NASYNC && e == cudaSuccess; i++) {
-        e = cudaStreamCreateWithFlags(&c->aslot[i].stream, cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->aslot[i].done, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->aslot[i].carried, cudaEventDisableTiming);
-    }
+    for (Slot& s : c->slot) if (e == cudaSuccess) e = create_slot(s);
+    for (AsyncSlot& s : c->aslot) if (e == cudaSuccess) e = create_slot(s);
     if (e != cudaSuccess) { int rc = cuda_fail(e, "context creation"); lz4b200_destroy(c); return rc; }
     *out = c;
     return LZ4B200_OK;
@@ -1284,16 +1330,8 @@ void lz4b200_destroy(lz4b200_ctx* c)
     if (!c) return;
     DeviceGuard g(c->device);
     cudaDeviceSynchronize();
-    for (Slot& s : c->slot) {
-        if (s.done) cudaEventDestroy(s.done);
-        if (s.carried) cudaEventDestroy(s.carried);
-        if (s.stream) cudaStreamDestroy(s.stream);
-    }
-    for (AsyncSlot& s : c->aslot) {
-        if (s.done) cudaEventDestroy(s.done);
-        if (s.carried) cudaEventDestroy(s.carried);
-        if (s.stream) cudaStreamDestroy(s.stream);
-    }
+    for (Slot& s : c->slot) destroy_slot(s);
+    for (AsyncSlot& s : c->aslot) destroy_slot(s);
     for (auto& b : c->meta_pool) if (b->done) cudaEventDestroy(b->done);
     for (Chain* ch : {&c->hc_done, &c->compact_done, &c->async_done}) {
         if (ch->done) cudaEventDestroy(ch->done);
@@ -1326,24 +1364,15 @@ int lz4b200_encode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
                                 const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len,
                                 int32_t n, int mode)
 {
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
-    if (n < 0 || !out_off) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
-    return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, encode_op(mode == LZ4B200_MODE_HC), LZ4B200_MEM_HOST,
-                 nullptr, out_off, dst_total_cap);
+    return encode_packed(c, src, src_off, src_len, dst_cap, dst, dst_total_cap, out_off, out_len, n, mode, LZ4B200_MEM_HOST, nullptr);
 }
 
 int lz4b200_encode_batch_packed_from_device(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
                                             const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off,
                                             int32_t* out_len, int32_t n, int mode, void* stream)
 {
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
-    if (n < 0 || !out_off) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n == 0) { out_off[0] = 0; return LZ4B200_OK; }
-    return batch(c, src, src_off, src_len, dst, nullptr, dst_cap, out_len, n, encode_op(mode == LZ4B200_MODE_HC),
-                 LZ4B200_MEM_DEVICE_TO_HOST, stream, out_off, dst_total_cap);
+    return encode_packed(c, src, src_off, src_len, dst_cap, dst, dst_total_cap, out_off, out_len, n, mode, LZ4B200_MEM_DEVICE_TO_HOST,
+                         stream);
 }
 
 // ---- between device memory and page-locked host memory without blocking: run_async -----------------------------------
@@ -1351,26 +1380,15 @@ int lz4b200_encode_batch_packed_from_device_async(lz4b200_ctx* c, const void* sr
                                                   const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off,
                                                   int32_t* out_len, int32_t n, int mode, void* stream)
 {
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
-    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n > 0 && (!src || !src_off || !src_len || !dst_cap || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-    for (int32_t i = 0; i < n; i++)
-        if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
-    return landed_async(c, Stage::CODEC, encode_op(mode == LZ4B200_MODE_HC), src, src_off, src_len, dst_cap, dst, dst_total_cap,
-                        out_off, out_len, n, stream, "lz4b200_encode_batch_packed_from_device_async");
+    return landed_async(c, Stage::CODEC, mode, src, src_off, src_len, dst_cap, dst, dst_total_cap, out_off, out_len, n, stream,
+                        "lz4b200_encode_batch_packed_from_device_async");
 }
 
 int lz4b200_decode_batch_to_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
                                          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int known_len,
                                          void* stream)
 {
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (n < 0) return fail(LZ4B200_E_ARG, "negative block count");
-    if (n > 0 && (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-    for (int32_t i = 0; i < n; i++)
-        if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
-    return staged_async(c, Stage::CODEC, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, src, src_off, src_len, dst, dst_off,
+    return staged_async(c, Stage::CODEC, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, false, src, src_off, src_len, dst, dst_off,
                         dst_cap, out_len, n, nullptr, 0, stream, "lz4b200_decode_batch_to_device_async");
 }
 
@@ -1378,41 +1396,22 @@ int lz4b200_decode_batch_packed_to_device_async(lz4b200_ctx* c, const void* src,
                                                 void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
                                                 void* stream)
 {
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n > 0 && (!src || !src_off || !src_len || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-    for (int32_t i = 0; i < n; i++)
-        if (src_len[i] < 0) return fail(LZ4B200_E_ARG, "negative block length");
-    return staged_async(c, Stage::PLACED_DECODE, Op::DECODE_UNKNOWN, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
-                        dst_total_cap, stream, "lz4b200_decode_batch_packed_to_device_async");
+    return staged_async(c, Stage::PLACED_DECODE, Op::DECODE_UNKNOWN, true, src, src_off, src_len, dst, nullptr, nullptr, out_len, n,
+                        out_off, dst_total_cap, stream, "lz4b200_decode_batch_packed_to_device_async");
 }
 
 int lz4b200_wrap_batch_packed_from_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
                                                 int high_compression, void* dst, int64_t dst_total_cap, int64_t* out_off,
                                                 int32_t* out_len, int32_t n, void* stream)
 {
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n > 0 && (!src || !src_off || !src_len || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-    // the dense slots hold whole packets: capacity src_len + 8 (wrap_packets)
-    std::vector<int32_t> pcap((size_t)n);
-    for (int32_t i = 0; i < n; i++) {
-        if (src_len[i] < 0 || src_len[i] > INT32_MAX - WRAP_HEADER) return fail(LZ4B200_E_ARG, "input length: negative, or a packet above INT32_MAX bytes");
-        pcap[i] = src_len[i] + WRAP_HEADER;
-    }
-    return landed_async(c, Stage::WRAP_ENCODE, encode_op(high_compression != 0), src, src_off, src_len, pcap.data(), dst,
-                        dst_total_cap, out_off, out_len, n, stream, "lz4b200_wrap_batch_packed_from_device_async");
+    return landed_async(c, Stage::WRAP_ENCODE, high_compression ? LZ4B200_MODE_HC : LZ4B200_MODE_FAST, src, src_off, src_len, nullptr,
+                        dst, dst_total_cap, out_off, out_len, n, stream, "lz4b200_wrap_batch_packed_from_device_async");
 }
 
 int lz4b200_unwrap_batch_to_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
                                          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
 {
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (n < 0) return fail(LZ4B200_E_ARG, "negative packet count");
-    if (n > 0 && (!src || !src_off || !src_len || !dst || !dst_off || !dst_cap || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-    for (int32_t i = 0; i < n; i++)
-        if (src_len[i] < 0 || dst_cap[i] < 0) return fail(LZ4B200_E_ARG, "negative packet length");
-    return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, nullptr, 0,
+    return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, false, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, nullptr, 0,
                         stream, "lz4b200_unwrap_batch_to_device_async");
 }
 
@@ -1420,12 +1419,7 @@ int lz4b200_unwrap_batch_packed_to_device_async(lz4b200_ctx* c, const void* src,
                                                 void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
                                                 void* stream)
 {
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n > 0 && (!src || !src_off || !src_len || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-    for (int32_t i = 0; i < n; i++)
-        if (src_len[i] < 0) return fail(LZ4B200_E_ARG, "negative packet length");
-    return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
+    return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, true, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
                         dst_total_cap, stream, "lz4b200_unwrap_batch_packed_to_device_async");
 }
 
@@ -1469,8 +1463,7 @@ int lz4b200_measure_batch(lz4b200_ctx* c, const void* src, const int64_t* src_of
                  mem, stream);
 }
 
-// measure -> scan -> capacities + "fits" -> decode, all enqueued on `stream`: the decoders leave at once (pick gate)
-// when the total does not fit, so out_len keeps the measured sizes and dst is untouched.
+// run_placed_decode, all enqueued on `stream`, placed in one piece by the call scratch.
 int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len,
                                 void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n, void* stream)
 {
@@ -1481,15 +1474,9 @@ int lz4b200_decode_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     int rc = call.enter(need_of(c, n, SCAN | CAPS, 1)); if (rc) return rc;
     int32_t* caps = (int32_t*)c->packed_caps.p;
-    int* fits = (int*)(caps + n);
-    const BatchArgs m{(const uint8_t*)src, src_off, src_len, nullptr, nullptr, nullptr, out_len, n};
-    cudaError_t e = launch_measure(m, false, c->dev, call.st, &c->launches);
-    if (e == cudaSuccess) e = place(c, out_len, out_off, n, c->compact_tmp, dst_total_cap, PACKED_ROOM_UNKNOWN, caps, fits, call.st);
-    if (e == cudaSuccess) {
-        const BatchArgs d{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, caps, out_len, n};
-        e = launch_decode(d, false, c->pinned_lanes(), c->counter(call.cap), c->dev, call.st, &c->launches, fits);
-    }
-    if (e != cudaSuccess) return cuda_fail(e, "packed decode launch");
+    const Placement pl{out_off, c->compact_tmp.p, c->compact_tmp.cap, dst_total_cap, 0, caps, (int*)(caps + n)};
+    const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, caps, out_len, n};
+    rc = run_placed_decode(c, a, pl, call.st, call.cap); if (rc) return rc;
     return call.done();
 }
 
@@ -1565,10 +1552,8 @@ int lz4b200_unwrap_batch_packed(lz4b200_ctx* c, const void* src, const int64_t* 
     if (!src || !src_off || !src_len || !dst || !out_len) return fail(LZ4B200_E_ARG, "null argument");
     int rc = call.enter(need_of(c, n, SCAN | CAPS | WRAP, 1)); if (rc) return rc;
     int32_t* caps = (int32_t*)c->packed_caps.p;
-    int* fits = (int*)(caps + n);
+    const Placement pl{out_off, c->compact_tmp.p, c->compact_tmp.cap, dst_total_cap, 0, caps, (int*)(caps + n)};
     const BatchArgs a{(const uint8_t*)src, src_off, src_len, (uint8_t*)dst, out_off, nullptr, out_len, n};
-    const UnwrapPlacement pl{[&] { return place(c, out_len, out_off, n, c->compact_tmp, dst_total_cap, 0, caps, fits, call.st); },
-                             caps, fits};
     rc = run_unwrap(c, a, wrap_scratch_at(c->wrap_tmp.p, n), call.st, call.cap, &pl); if (rc) return rc;
     return call.done();
 }

@@ -4,7 +4,8 @@ The launch counts (`lz4b200_launch_count` before and after a call) pin what ever
 encoders, decoders and measure pass in every kind of memory a call accepts, host batches of one block and of more than
 eight (every landing mode of the host pipeline), every pinned `decode_lanes` value and the automatic pick, the LZ4Stream
 and Wrap / Unwrap calls in their host, device, mixed and packed forms, and the packed decode into device memory over
-several pipeline stages.  A change to the host code that adds, drops or reorders a step shows up here.
+several pipeline stages; and the six asynchronous calls between device memory and page-locked host memory in one stage and
+in several.  A change to the host code that adds, drops or reorders a step shows up here.
 
 The device calls share the context's scan scratch, capacities and packet view whatever stream they are on.  Enqueued on
 two streams with no synchronise in between, a call that grows that scratch and one that does not must both give their
@@ -21,7 +22,8 @@ pytestmark = pytest.mark.gpu
 LANES = (1, 4, 8, 16, 32, 104, 108, 116, 132)
 MEMS = {"host": 0, "device": 1, "device_to_host": 2, "host_to_device": 3}
 
-# Recorded on an H100 80GB HBM3; the same before and after the host pipeline named its operations and stage kinds.
+# Recorded on an H100 80GB HBM3; the same before and after the host pipeline named its operations and stage kinds, and
+# (the asynchronous rows) before and after the pipeline's stage kinds were dispatched in one place.
 EXPECTED = {
     'encode/fast/host/1': 1, 'encode/hc/host/1': 2, 'decode/known/host/1': 1, 'decode/unknown/host/1': 1,
     'encode/fast/device/1': 1, 'encode/hc/device/1': 3, 'decode/known/device/1': 5, 'decode/unknown/device/1': 5,
@@ -66,6 +68,14 @@ EXPECTED = {
     'decode_batch_packed/lanes116': 7, 'decode/known/device/lanes132': 1, 'decode/unknown/device/lanes132': 1,
     'decode_batch_packed/lanes132': 7, 'decode_packed/host_to_device/auto': 30,
     'decode_packed/host_to_device/lanes16': 21,
+    'encode_packed_async/fast/1stage': 5, 'wrap_packed_async/fast/1stage': 7, 'encode_packed_async/hc/1stage': 7,
+    'wrap_packed_async/hc/1stage': 9, 'decode_async/known/1stage': 1, 'decode_async/unknown/1stage': 1,
+    'decode_packed_async/1stage': 10, 'unwrap_async/fast/1stage': 7, 'unwrap_packed_async/fast/1stage': 11,
+    'unwrap_async/hc/1stage': 7, 'unwrap_packed_async/hc/1stage': 11, 'encode_packed_async/fast/stages': 20,
+    'wrap_packed_async/fast/stages': 28, 'encode_packed_async/hc/stages': 28, 'wrap_packed_async/hc/stages': 36,
+    'decode_async/known/stages': 3, 'decode_async/unknown/stages': 3, 'decode_packed_async/stages': 30,
+    'unwrap_async/fast/stages': 21, 'unwrap_packed_async/fast/stages': 33, 'unwrap_async/hc/stages': 14,
+    'unwrap_packed_async/hc/stages': 22,
 }
 
 
@@ -305,6 +315,73 @@ def _placed_calls(ctx, count):
         ctx.set_option("decode_lanes_auto", 1)
 
 
+def _async_calls(ctx, count):
+    """The six asynchronous calls between device memory and page-locked host memory, each in one stage (the default
+    host_chunk_mb) and over several 1 MiB stages, in fast and HC where the call takes a mode."""
+    import torch
+    from lz4net_b200 import native
+    lib, h, st = native.lib(), ctx.handle, torch.cuda.current_stream().cuda_stream
+    raws = [cases.content(("E0", "E50", "ETEXT")[i % 3], 300000, seed=500 + i).tobytes() for i in range(12)]
+    n, want = len(raws), b"".join(raws)
+    rbuf, rso, rsl = _src(raws)
+    d_raw = _dev(rbuf)
+    ecap = np.array([oracle.bound(len(d)) for d in raws], np.int32)
+    rcap = rsl.copy()
+    rdo, rtotal = _layout(rcap, 0, 0)
+    pin = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory()            # noqa: E731
+    outs = lambda: (torch.zeros(n + 1, dtype=torch.int64, device="cuda"),             # noqa: E731
+                    torch.zeros(n, dtype=torch.int32, device="cuda"))
+    cbuf, cso, csl = _src([oracle.encode(d)[1] for d in raws])
+    comp = pin(cbuf)
+    try:
+        for stages, mb in (("1stage", 128), ("stages", 1)):
+            ctx.set_option("host_chunk_mb", mb)
+            packets = {}
+            for hc in (False, True):
+                tag = "hc" if hc else "fast"
+                dst = pin(np.zeros(int(ecap.sum()) + 64, np.uint8))
+                off, out = outs()
+                count(f"encode_packed_async/{tag}/{stages}", lambda: native.check(
+                    lib.lz4b200_encode_batch_packed_from_device_async(
+                        h, d_raw.data_ptr(), rso.ctypes.data, rsl.ctypes.data, ecap.ctypes.data, dst.data_ptr(), dst.numel(),
+                        off.data_ptr(), out.data_ptr(), n, int(hc), st), "encode_packed_async"))
+                assert int(off[n]) <= dst.numel(), (stages, tag)
+                dst = pin(np.zeros(int(rsl.sum()) + 8 * n + 64, np.uint8))
+                off, out = outs()
+                count(f"wrap_packed_async/{tag}/{stages}", lambda: native.check(lib.lz4b200_wrap_batch_packed_from_device_async(
+                    h, d_raw.data_ptr(), rso.ctypes.data, rsl.ctypes.data, int(hc), dst.data_ptr(), dst.numel(), off.data_ptr(),
+                    out.data_ptr(), n, st), "wrap_packed_async"))
+                packets[hc] = (dst, off.cpu().numpy(), out.cpu().numpy())
+            for known in (True, False):
+                d_dst, (_, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
+                count(f"decode_async/{'known' if known else 'unknown'}/{stages}", lambda: native.check(
+                    lib.lz4b200_decode_batch_to_device_async(
+                        h, comp.data_ptr(), cso.ctypes.data, csl.ctypes.data, d_dst.data_ptr(), rdo.ctypes.data, rcap.ctypes.data,
+                        out.data_ptr(), n, int(known), st), "decode_async"))
+                assert d_dst.cpu().numpy().tobytes() == want, (stages, known)
+            d_dst, (off, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
+            count(f"decode_packed_async/{stages}", lambda: native.check(lib.lz4b200_decode_batch_packed_to_device_async(
+                h, comp.data_ptr(), cso.ctypes.data, csl.ctypes.data, d_dst.data_ptr(), rtotal, off.data_ptr(), out.data_ptr(),
+                n, st), "decode_packed_async"))
+            assert d_dst.cpu().numpy().tobytes() == want and int(off[n]) == rtotal, stages
+            for hc, (pk, poff, plen) in packets.items():
+                tag = "hc" if hc else "fast"
+                pso = np.ascontiguousarray(poff[:n])
+                d_dst, (_, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
+                count(f"unwrap_async/{tag}/{stages}", lambda: native.check(lib.lz4b200_unwrap_batch_to_device_async(
+                    h, pk.data_ptr(), pso.ctypes.data, plen.ctypes.data, d_dst.data_ptr(), rdo.ctypes.data, rcap.ctypes.data,
+                    out.data_ptr(), n, st), "unwrap_async"))
+                assert d_dst.cpu().numpy().tobytes() == want, (stages, tag)
+                d_dst, (off, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
+                count(f"unwrap_packed_async/{tag}/{stages}", lambda: native.check(
+                    lib.lz4b200_unwrap_batch_packed_to_device_async(
+                        h, pk.data_ptr(), pso.ctypes.data, plen.ctypes.data, d_dst.data_ptr(), rtotal, off.data_ptr(),
+                        out.data_ptr(), n, st), "unwrap_packed_async"))
+                assert d_dst.cpu().numpy().tobytes() == want and int(off[n]) == rtotal, (stages, tag)
+    finally:
+        ctx.set_option("host_chunk_mb", 128)
+
+
 def test_gpu_launch_counts_of_every_call_family(ctx):
     count = _Counter(ctx)
     for n in (1, 12):
@@ -312,6 +389,7 @@ def test_gpu_launch_counts_of_every_call_family(ctx):
         _framing_calls(ctx, count, n)
     _decoder_calls(ctx, count)
     _placed_calls(ctx, count)
+    _async_calls(ctx, count)
     assert count.counts == EXPECTED, "\n" + "\n".join(f"    {k!r}: {v}," for k, v in count.counts.items())
 
 
