@@ -273,8 +273,10 @@ int lz4b200_compact(lz4b200_ctx* ctx, const void* slots, const int64_t* slot_off
  * and decode to device memory, the LZ4Stream and the Wrap / Unwrap calls between device and host memory): on a capturing
  * stream it returns LZ4B200_E_ARG before any CUDA work, and the capture stays valid.  So do the asynchronous calls --
  * lz4b200_encode_batch_packed_from_device_async, decode_batch_to_device_async, decode_batch_packed_to_device_async,
- * wrap_batch_packed_from_device_async, unwrap_batch_to_device_async and unwrap_batch_packed_to_device_async -- which do not
- * synchronise but hand the device host metadata that a graph would have to keep alive.  lz4b200_peer_copy is not covered.
+ * wrap_batch_packed_from_device_async, unwrap_batch_to_device_async, unwrap_batch_packed_to_device_async,
+ * stream_encode_from_device_async and stream_decode_to_device_async -- which do not synchronise but share the context's
+ * stage buffers between eager calls and, all but the stream encode, hand the device host metadata that a graph would have
+ * to keep alive.  lz4b200_peer_copy is not covered.
  * The calls without a stream (host-memory batches, single-block functions, lz4b200_synchronize, lz4b200_reserve) use
  * the legacy default stream or synchronise the device: they must not be made while any thread of the process captures
  * in cudaStreamCaptureModeGlobal.
@@ -327,6 +329,36 @@ int64_t lz4b200_stream_encode_from_device(lz4b200_ctx* ctx, const void* src, int
  *   the range are unspecified. */
 int64_t lz4b200_stream_decode_to_device(lz4b200_ctx* ctx, const void* src, int64_t n, void* dst, int64_t dst_cap,
                                         void* stream);
+
+/* The same stream between device memory and PAGE-LOCKED host memory without blocking: the contract of the asynchronous
+ * calls above ("offload without blocking": ordering on `stream` and among the context's calls, lifetime, page-locked host
+ * side, refusal of a capturing stream, no wait on device work except once when the context's buffers or HC arena grow).
+ * out_size may be device memory of the context's GPU or page-locked host memory; it is written by the device.  Argument
+ * and memory checks return what the synchronous calls return wherever the host can decide them.  One pointer and one
+ * length describe the whole offload: the bytes can be written to a file or a socket afterwards and read by any LZ4Stream.
+ *
+ * stream_encode_from_device_async: src is n bytes of device memory of the context's GPU; dst is page-locked host memory,
+ *   dst_cap >= lz4b200_stream_bound(n, block_size), so the stream always fits.  *out_size and dst[0, *out_size) equal what
+ *   lz4b200_stream_encode_from_device returns and writes for the same arguments; nothing outside [dst, dst + *out_size) is
+ *   written.  block_size >= 1 and at most INT32_MAX - 11, as in the synchronous call.  n == 0 writes *out_size = 0 on the
+ *   stream.  The call's page-locked metadata is O(pipeline stages): a stage's chunk table is computed on the device.
+ * stream_decode_to_device_async: src is the n bytes of a whole stream in page-locked host memory; dst is device memory of
+ *   the context's GPU.  The HOST walks the chunk headers during the call, as the synchronous call does: a caller who can
+ *   pass n has the stream's bytes in place (an asynchronous encode reports its size only on the device), so src must hold
+ *   the whole stream when the call is made, and stay untouched until `stream` has passed the call.
+ *   - A malformed header returns LZ4B200_E_FORMAT, and dst_cap below the decoded size LZ4B200_E_ARG; either way nothing is
+ *     enqueued and neither dst nor out_size is written.
+ *   - Otherwise the device writes *out_size: the decoded size, or LZ4B200_E_FORMAT when a compressed chunk does not decode
+ *     from exactly its compLen bytes (where the synchronous call returns LZ4B200_E_FORMAT).  Nothing is written outside
+ *     [dst, dst + decoded size); after a chunk that fails, the bytes inside it are unspecified.
+ *   - n == 0, or a stream of empty chunks, writes *out_size = 0 on the stream.
+ *   The call's page-locked metadata is O(non-empty chunks): one entry each (payload offset, compLen, rawLen, stored flag,
+ *   output offset), held until `stream` has passed the call. */
+int lz4b200_stream_encode_from_device_async(lz4b200_ctx* ctx, const void* src, int64_t n, int32_t block_size,
+                                            int high_compression, void* dst, int64_t dst_cap, int64_t* out_size,
+                                            void* stream);
+int lz4b200_stream_decode_to_device_async(lz4b200_ctx* ctx, const void* src, int64_t n, void* dst, int64_t dst_cap,
+                                          int64_t* out_size, void* stream);
 
 /* LZ4Codec.Wrap / Unwrap packet (src/LZ4/LZ4Codec.cs:510-543,574-599): u32le rawLen, u32le storedLen, payload. */
 int lz4b200_wrap(lz4b200_ctx* ctx, const void* src, int32_t n, int high_compression, void* dst, int32_t dst_cap);

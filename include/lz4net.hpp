@@ -125,6 +125,21 @@ public:
                                                         stream) != LZ4B200_OK)
             throw std::runtime_error(lz4b200_last_error());
     }
+    // The same for an LZ4Stream (lz4b200_stream_encode_from_device_async, lz4b200_stream_decode_to_device_async): n bytes
+    // of device memory as one stream in page-locked host memory, and back.  out_size is written by the device: the
+    // stream's size, or the decoded size (LZ4B200_E_FORMAT when a chunk does not decode).  The decode walks the stream's
+    // headers during the call, so src holds the whole stream when it is made.
+    void stream_encode_to_host_async(const void* src, int64_t n, int32_t block_size, bool hc, void* dst, int64_t dst_cap,
+                                     int64_t* out_size, void* stream)
+    {
+        if (lz4b200_stream_encode_from_device_async(h_, src, n, block_size, hc ? 1 : 0, dst, dst_cap, out_size, stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
+    void stream_decode_from_host_async(const void* src, int64_t n, void* dst, int64_t dst_cap, int64_t* out_size, void* stream)
+    {
+        if (lz4b200_stream_decode_to_device_async(h_, src, n, dst, dst_cap, out_size, stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
 private:
     lz4b200_ctx* h_ = nullptr;
 };

@@ -32,7 +32,9 @@ encode_to_host_packed_async and decode_from_host_async move blocks between a dev
 without blocking the calling thread: they enqueue their work on a stream and return, so a thread that launches a model's
 kernels can offload to host RAM, or prefetch back, and keep launching.  decode_from_host_packed_async,
 wrap_to_host_packed_async, unwrap_to_device_async and unwrap_to_device_packed_async do the same for the packed decode and
-for Wrap packets, which carry their own sizes and never exceed input + 8 bytes.  They refuse a capturing stream.
+for Wrap packets, which carry their own sizes and never exceed input + 8 bytes.  stream_encode_to_host_async and
+stream_decode_to_device_async do it for an LZ4Stream: one byte string, one pointer and one length, that any LZ4Stream reads.
+They refuse a capturing stream.
 """
 from __future__ import annotations
 
@@ -288,6 +290,35 @@ def unwrap_to_device_packed_async(ctx: Context, packets: torch.Tensor, src_off, 
     native.check(native.lib().lz4b200_unwrap_batch_packed_to_device_async(
         ctx.handle, p, _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), out.nbytes, off, res, n, _stream_of(stream)),
         "unwrap_batch_packed_to_device_async")
+
+
+def stream_encode_to_host_async(ctx: Context, raw: torch.Tensor, dst: torch.Tensor, out_size: torch.Tensor,
+                                block_size: int = 1 << 20, hc: bool = False, stream=None):
+    """stream_encode_to_host without blocking (lz4b200_stream_encode_from_device_async): the LZ4Stream of raw's bytes, cut
+    into block_size chunks, is written at the start of dst, and its size to out_size[0].  dst is a page-locked CPU uint8
+    tensor of at least lz4b200_stream_bound bytes; out_size (int64[1]) a CUDA or page-locked CPU tensor, written by the
+    device.  Enqueued on `stream` (default: the current torch stream) behind the work already there; returns at once.  The
+    caller keeps raw, dst and out_size alive and untouched until the stream has passed the call."""
+    d, size = _pinned(dst, torch.uint8, 0, "dst"), _pinned(out_size, torch.int64, 1, "out_size", True)
+    r = _flat_bytes(raw)
+    native.check(native.lib().lz4b200_stream_encode_from_device_async(
+        ctx.handle, r.data_ptr(), r.numel(), block_size, int(hc), d, dst.numel(), size, _stream_of(stream)),
+        "stream_encode_from_device_async")
+
+
+def stream_decode_to_device_async(ctx: Context, wire: torch.Tensor, n: int, out: torch.Tensor, out_size: torch.Tensor,
+                                  stream=None):
+    """stream_decode_to_device without blocking (lz4b200_stream_decode_to_device_async): the LZ4Stream in the first n
+    bytes of wire is decoded into out's bytes, from its first byte.  wire is a page-locked CPU uint8 tensor that holds the
+    whole stream when the call is made: its headers are read during the call.  out_size (int64[1]) is a CUDA or
+    page-locked CPU tensor that the device sets to the decoded size, or to LZ4B200_E_FORMAT when a chunk does not decode.
+    A malformed header or an `out` too small raises Lz4B200Error (E_FORMAT, E_ARG) with nothing enqueued.  Enqueued on
+    `stream` (default: the current torch stream); returns at once.  The caller keeps wire, out and out_size alive and
+    untouched until the stream has passed the call."""
+    w, size = _pinned(wire, torch.uint8, n, "wire"), _pinned(out_size, torch.int64, 1, "out_size", True)
+    o = _flat_bytes(out)
+    native.check(native.lib().lz4b200_stream_decode_to_device_async(
+        ctx.handle, w, n, o.data_ptr(), o.numel(), size, _stream_of(stream)), "stream_decode_to_device_async")
 
 
 def wrap_to_host(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, out_len, hc: bool = False):

@@ -9,11 +9,12 @@
 // so does the packed unknown-size decode from host into device memory, whose output offset is carried across the stages
 // on the device (Placement, lz4_packed.cuh).  What a stage runs is named by its caller (Stage) and mapped to its sequence
 // in one place (run_stage); the codec operation is named by Op.
-// The asynchronous calls between device memory and page-locked host memory (run_async: the packed encode and Wrap into it,
-// the decode, packed decode and Unwrap from it, checked by landed_async and staged_async) cut their stages by the same
-// plan, run the same stage sequences on streams and buffers of their own and return without waiting; the packed encodes'
-// stages land in host memory from a kernel (lz4_land.cuh), since where a stage lands is known only on the device, and the
-// Unwraps read their headers on the device (run_unwrap).
+// The asynchronous calls between device memory and page-locked host memory (run_async: the packed encode, Wrap and
+// LZ4Stream encode into it, the decode, packed decode, Unwrap and LZ4Stream decode from it, checked by landed_async and
+// staged_async) cut their stages by the same plan, run the same stage sequences on streams and buffers of their own and
+// return without waiting; the packed encodes' stages land in host memory from a kernel (lz4_land.cuh), since where a stage
+// lands is known only on the device, the Unwraps read their headers on the device (run_unwrap), and the LZ4Stream encode
+// computes its chunk tables on the device.
 // The device-memory calls enter through one path (DeviceCall): each states what it takes from the context (Need), which
 // admits it to a CUDA graph capture or grows an eager call's scratch; lz4b200_reserve grows to the same needs.
 // The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
@@ -195,6 +196,7 @@ struct Slot : SlotBase {
 constexpr int NASYNC = 2;
 struct AsyncSlot : SlotBase {
     DevBuf io;                             // the encode's dense output slots, or the decode's staged source
+    DevBuf frames;                         // an LZ4Stream encode's frames, back to back, before they land
 };
 // The page-locked metadata of one asynchronous call, which the device reads after the call has returned: taken again once
 // `done`, recorded behind the call, has fired.
@@ -235,8 +237,9 @@ constexpr bool is_measure(Op op) { return op == Op::MEASURE_KNOWN || op == Op::M
 // What a stage of the host pipeline (run_host) runs on its chunk.
 enum class Stage {
     CODEC,            // the operation (run_device)
-    STREAM_ENCODE,    // the encode, then the chunks' LZ4Stream frames (lz4_stream.cuh) in place of the compaction: APPEND
-                      // lands the frames, out_off[i] = where frame i starts
+    STREAM_ENCODE,    // the encode, then the chunks' LZ4Stream frames (lz4_stream.cuh, write_frames) in place of the
+                      // compaction: APPEND lands the frames, out_off[i] = where frame i starts; asynchronously, the landing
+                      // kernel does, keeping only the total
     WRAP_ENCODE,      // prep -> the encode -> finish (run_wrap, lz4_wrap.cuh): dst_cap[i] = the packet's capacity,
                       // src_len[i] + 8; the slot then holds whole packets, which land like the blocks of an encode
     FRAMED_DECODE,    // the known-size decode of LZ4Stream chunks or Unwrap packets: stored[i] != 0 marks a stored one, whose
@@ -264,7 +267,8 @@ struct lz4b200_ctx {
     Chain async_done;                      // likewise the asynchronous calls' stage buffers, carry cells and streams (run_async)
     cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
     int64_t* carry = nullptr;              // the running output offset behind each slot's stage: NSLOT cells for the packed decode into device
-                                           // memory, then NASYNC for the asynchronous packed encode
+                                           // memory, then NASYNC for the asynchronous packed encode, then one more cell
+                                           // whose int is the asynchronous LZ4Stream decode's failure flag (stream_failed)
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
     bool decode_lanes_auto = true;         // host-memory batches: chosen per chunk from the compression ratio
     int encode_ctas_per_sm = 0;            // encoder warps (= blocks in flight) per SM: 0 = as many as shared memory holds tables for (14)
@@ -288,6 +292,7 @@ struct lz4b200_ctx {
         uint32_t* c = counters + next_counter; next_counter = (next_counter + 4) % NCOUNTER; return c;
     }
     int pinned_lanes() const { return decode_lanes_auto ? 0 : decode_lanes; }   // 0: the decoder is picked on the device
+    int* stream_failed() const { return (int*)(carry + NSLOT + NASYNC); }       // serialised through async_done
 };
 
 namespace {
@@ -530,6 +535,18 @@ int run_stage(lz4b200_ctx* c, Stage kind, Op op, const BatchArgs& a, int lanes, 
     return fail(LZ4B200_E_ARG, "unknown stage kind");
 }
 
+// The LZ4Stream frames of an encoded STREAM_ENCODE stage a, back to back: the frame sizes into frame_len, their scan into
+// offs (offs[m] = the stage's bytes), then each frame at frames + offs[i].  In place of the compaction, in run_host and
+// run_async alike.
+cudaError_t write_frames(lz4b200_ctx* c, const BatchArgs& a, bool hc, int32_t* frame_len, int64_t* offs, void* scan,
+                         size_t scan_bytes, uint8_t* frames, cudaStream_t st)
+{
+    cudaError_t e = launch_stream_frame_size(a, frame_len, st, &c->launches);
+    if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, frame_len, nullptr, offs, a.n_blocks, scan, scan_bytes, c->dev, st, &c->launches);
+    if (e == cudaSuccess) e = launch_stream_frame(a, hc, frames, offs, st, &c->launches);
+    return e;
+}
+
 // ---- the stage plan of the host pipeline, shared by run_host and the asynchronous calls (run_async) ------------------
 // A stage [b0, b1) is weighed by the bytes it stages: src_len[i] when count_src, plus dst_cap[i] when dst_cap is given
 // (not for a destination already on the device, nor for the measure pass).  Blocks join it while it stays within
@@ -757,14 +774,9 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
             CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
             uint8_t* packed = (uint8_t*)sl.packed.p;
             int64_t* offs = (int64_t*)sl.offs.p;
-            cudaError_t e;
-            if (frames) {
-                e = launch_stream_frame_size(a, d.aux, sl.stream, &c->launches);
-                if (e == cudaSuccess) e = launch_compact(nullptr, nullptr, d.aux, nullptr, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
-                if (e == cudaSuccess) e = launch_stream_frame(a, op == Op::ENCODE_HC, packed, offs, sl.stream, &c->launches);
-            } else {
-                e = launch_compact(a.dst, a.dst_off, a.out_len, packed, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
-            }
+            const cudaError_t e =
+                frames ? write_frames(c, a, op == Op::ENCODE_HC, d.aux, offs, sl.scan.p, sl.scan.cap, packed, sl.stream)
+                       : launch_compact(a.dst, a.dst_off, a.out_len, packed, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
             rc = launched(e, frames ? "stream frame launch" : "compact launch"); if (rc) return rc;
             CU(cudaMemcpyAsync(h.off, offs, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDeviceToHost, sl.stream));
         }
@@ -844,6 +856,16 @@ int take_meta(lz4b200_ctx* c, size_t bytes, MetaBlock** out)
     return LZ4B200_OK;
 }
 
+// The LZ4Stream calls' own part of an asynchronous call: the stream's length n and the encode's chunk size, from which its
+// stages and their chunk tables follow (STREAM_ENCODE); the decode's stored flags, one per entry, and its decoded size
+// (FRAMED_DECODE).
+struct StreamCall { int64_t n = 0; int32_t block_size = 0; const uint8_t* stored = nullptr; int64_t total = 0; };
+
+// The LZ4Stream calls run the pipeline over at most this many chunks at a time: it bounds the host metadata by chunk
+// count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.  An asynchronous
+// encode stage takes at most this many chunks, which bounds its device metadata the same way.
+constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
+
 // The stages of an asynchronous call, cut and described as run_host cuts and describes them (stage_end, fill_stage,
 // stage_lanes, stage_hc_large), enqueued on the context's NASYNC streams in turn, forked from `caller` and joined back to
 // it; nothing is waited on unless a buffer must grow.  What a stage runs is its kind's sequence (run_stage), as in run_host:
@@ -852,39 +874,65 @@ int take_meta(lz4b200_ctx* c, size_t bytes, MetaBlock** out)
 //    per packet, the stage weighed by it) into its dense slots (AsyncSlot::io), scans the lengths, and lands
 //    (lz4_land.cuh) behind the running total that the previous stage's landing step left in its carry cell, after the
 //    previous slot's `carried` event.
-//  - The decodes into device memory (CODEC with a decode, UNWRAP, PLACED_DECODE): src is page-locked host memory, copied
-//    up a stage at a time on the copy engine, weighed by src_len; the decoders write dst (device memory) in place.  A
-//    CODEC decode writes at dst_off; an UNWRAP reads the headers from the staged bytes on the device (run_unwrap), since
-//    work still queued on `caller` may write them.  The packed forms (placed: PLACED_DECODE, an UNWRAP without dst_off)
-//    measure (PLACED_DECODE) or prep (UNWRAP), scan and place their stage behind the previous one's from the same carry
-//    cells (place), then decode behind the stage's "fits" flag; their absolute offsets are copied to out_off, the last
-//    stage's running total to out_off[n].
-//    The stage's results are copied to out_len (device or page-locked memory).
+//  - The LZ4Stream encode (STREAM_ENCODE, sc: the stream's length and chunk size) lands the same way, but its stages are
+//    cut arithmetically, as many chunks as host_chunk_bytes of input holds (at least one, at most STREAM_RUN_CHUNKS), and
+//    hold no host metadata: a stage's chunk table is computed on the device (lz4_stream.cuh stream_cut_one).  The stage
+//    encodes its chunks (capacity = the chunk's length), writes their frames back to back (write_frames, into
+//    AsyncSlot::frames) and lands the frames as its blocks.  Only the running total is kept: the last stage's goes to
+//    out_off[0], the stream's size, on `caller` behind the join.
+//  - The decodes into device memory (CODEC with a decode, UNWRAP, PLACED_DECODE, FRAMED_DECODE): src is page-locked host
+//    memory, copied up a stage at a time on the copy engine, weighed by src_len; the decoders write dst (device memory) in
+//    place.  A CODEC decode writes at dst_off; an UNWRAP reads the headers from the staged bytes on the device (run_unwrap),
+//    since work still queued on `caller` may write them.  The packed forms (placed: PLACED_DECODE, an UNWRAP without
+//    dst_off) measure (PLACED_DECODE) or prep (UNWRAP), scan and place their stage behind the previous one's from the same
+//    carry cells (place), then decode behind the stage's "fits" flag; their absolute offsets are copied to out_off, the
+//    last stage's running total to out_off[n].
+//    The stage's results are copied to out_len (device or page-locked memory), except for an LZ4Stream decode
+//    (FRAMED_DECODE, sc: the stored flags and the decoded size), whose entries come from the host's header walk: its stages
+//    set the context's failure flag (stream_failed) when a compressed chunk does not decode from exactly its compLen bytes,
+//    and one thread on `caller` behind the join writes out_off[0] = the decoded size, or LZ4B200_E_FORMAT.  The flag is
+//    cleared behind the context's previous asynchronous call and read before the next one (async_done).
 // Calls are chained through async_done; the call's metadata block is taken again once the caller's stream has passed it.
 int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
               const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
-              int64_t dst_total_cap, cudaStream_t caller)
+              int64_t dst_total_cap, cudaStream_t caller, const StreamCall* sc = nullptr)
 {
     const bool enc = is_encode(op), placed = kind == Stage::PLACED_DECODE || (kind == Stage::UNWRAP && !dst_off);
-    struct Plan { int32_t b0, b1; size_t at; StageSpan sp; };
+    const bool cut = kind == Stage::STREAM_ENCODE, framed = kind == Stage::FRAMED_DECODE;
+    // blocks [b0, b1) of the batch, their host metadata at `at` in the call's block; an LZ4Stream encode stage's chunks are
+    // [first + b0, first + b1) of the stream, b0 = 0
+    struct Plan { int32_t b0, b1; size_t at; StageSpan sp; int64_t first; };
     std::vector<Plan> plan;
     size_t bytes = 0;
-    for (int32_t b0 = 0; b0 < n;) {
-        const int32_t b1 = stage_end(c, src_len, enc ? dst_cap : nullptr, b0, n, !enc);
-        plan.push_back(Plan{b0, b1, bytes, {}});
-        bytes += (meta_host_bytes(b1 - b0) + 15) & ~(size_t)15;
-        b0 = b1;
+    if (cut) {
+        const int64_t bs = sc->block_size, chunks = (sc->n + bs - 1) / bs;
+        const int64_t per = std::max<int64_t>(1, std::min<int64_t>((int64_t)c->host_chunk_bytes / bs, STREAM_RUN_CHUNKS));
+        for (int64_t k0 = 0; k0 < chunks; k0 += per) {
+            const int32_t m = (int32_t)std::min(per, chunks - k0);
+            StageSpan sp;
+            sp.dsum = std::min((int64_t)m * bs, sc->n - k0 * bs);
+            plan.push_back(Plan{0, m, 0, sp, k0});
+        }
+    } else {
+        for (int32_t b0 = 0; b0 < n;) {
+            const int32_t b1 = stage_end(c, src_len, enc ? dst_cap : nullptr, b0, n, !enc);
+            plan.push_back(Plan{b0, b1, bytes, {}, 0});
+            bytes += (meta_host_bytes(b1 - b0) + 15) & ~(size_t)15;
+            b0 = b1;
+        }
     }
     MetaBlock* blk = nullptr;
-    int rc = take_meta(c, bytes, &blk); if (rc) return rc;
-    struct Sizes { size_t io = 0, meta = 0, offs = 0, scan = 0; } need[NASYNC];      // each slot's buffers, for its largest stage
+    int rc = bytes ? take_meta(c, bytes, &blk) : LZ4B200_OK; if (rc) return rc;
+    struct Sizes { size_t io = 0, frames = 0, meta = 0, offs = 0, scan = 0; } need[NASYNC];      // each slot's buffers, for its largest stage
     for (size_t k = 0; k < plan.size(); k++) {
         Plan& p = plan[k];
         const int32_t m = p.b1 - p.b0;
-        p.sp = fill_stage(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, src_off, src_len, dst_off, dst_cap, enc, !enc, false,
-                          placed, nullptr);
+        if (!cut)
+            p.sp = fill_stage(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, src_off, src_len, dst_off, dst_cap, enc, !enc, false,
+                              placed, framed ? sc->stored : nullptr);
         Sizes& nd = need[k % NASYNC];
         nd.io = std::max(nd.io, (size_t)(enc ? p.sp.dsum : p.sp.shi - p.sp.slo) + 64);
+        if (cut) nd.frames = std::max(nd.frames, (size_t)p.sp.dsum + (size_t)m * STREAM_HEADER_MAX + 64);
         nd.meta = std::max(nd.meta, async_meta_bytes(m));
         if (enc || placed) { nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(m + 1)); nd.scan = std::max(nd.scan, compact_tmp_bytes(m)); }
     }
@@ -892,18 +940,26 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
     bool grow = false;
     for (int s = 0; s < NASYNC; s++) {
         const AsyncSlot& sl = c->aslot[s];
-        grow |= need[s].io > sl.io.cap || need[s].meta > sl.meta.cap || need[s].offs > sl.offs.cap || need[s].scan > sl.scan.cap;
+        grow |= need[s].io > sl.io.cap || need[s].frames > sl.frames.cap || need[s].meta > sl.meta.cap || need[s].offs > sl.offs.cap ||
+                need[s].scan > sl.scan.cap;
     }
     if (grow) {
         CU(cudaDeviceSynchronize());
         for (int s = 0; s < NASYNC; s++) {
             AsyncSlot& sl = c->aslot[s];
-            CU(sl.io.reserve(need[s].io)); CU(sl.meta.reserve(need[s].meta)); CU(sl.offs.reserve(need[s].offs)); CU(sl.scan.reserve(need[s].scan));
+            CU(sl.io.reserve(need[s].io)); CU(sl.frames.reserve(need[s].frames)); CU(sl.meta.reserve(need[s].meta));
+            CU(sl.offs.reserve(need[s].offs)); CU(sl.scan.reserve(need[s].scan));
         }
     }
     const int used = (int)std::min<size_t>(plan.size(), NASYNC);
     int64_t* carry = c->carry + NSLOT;
+    int* failed = c->stream_failed();
     auto stages = [&]() -> int {
+        if (framed) {
+            // the failure flag, cleared behind the context's previous asynchronous call (which may still read it)
+            CU(c->async_done.wait(caller, Capture{}));
+            CU(cudaMemsetAsync(failed, 0, sizeof(int), caller));
+        }
         CU(cudaEventRecord(c->entry, caller));
         for (int s = 0; s < used; s++) {
             CU(cudaStreamWaitEvent(c->aslot[s].stream, c->entry, 0));
@@ -914,8 +970,17 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
             const int s = (int)(k % NASYNC), prev = (s + NASYNC - 1) % NASYNC;
             AsyncSlot& sl = c->aslot[s];
             const int32_t m = p.b1 - p.b0;
-            const Meta h((uint8_t*)blk->buf.p + p.at, m), d(sl.meta.p, m);
-            CU(cudaMemcpyAsync(sl.meta.p, h.so, (size_t)((uint8_t*)h.aux - (uint8_t*)h.so), cudaMemcpyHostToDevice, sl.stream));
+            const Meta d(sl.meta.p, m);
+            if (cut) {
+                int rc = launched(launch_stream_cut(p.first, m, sc->block_size, sc->n, d.so, d.sl, d.dof, d.dc, sl.stream, &c->launches),
+                                  "stream chunk table launch");
+                if (rc) return rc;
+            } else {
+                // up: the four arrays the kernels read, and a framed decode's stored lengths
+                const Meta h((uint8_t*)blk->buf.p + p.at, m);
+                CU(cudaMemcpyAsync(sl.meta.p, h.so, (size_t)((uint8_t*)(framed ? h.out : h.aux) - (uint8_t*)h.so), cudaMemcpyHostToDevice,
+                                   sl.stream));
+            }
             const size_t sbytes = (size_t)(p.sp.shi - p.sp.slo);
             if (!enc && sbytes) CU(cudaMemcpyAsync(sl.io.p, src + p.sp.slo, sbytes, cudaMemcpyHostToDevice, sl.stream));
             // (a packed Unwrap's prep reads no capacity: the placement writes the decode's into d.dc)
@@ -925,10 +990,16 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
             // a packed stage places behind the previous stage's placement (lz4_packed.cuh); the next one follows
             const Placement pl{offs, sl.scan.p, sl.scan.cap, dst_total_cap, 0, d.dc, async_fits(sl.meta.p, m),
                                k > 0 ? c->aslot[prev].carried : nullptr, k > 0 ? carry + prev : nullptr, d.dof, carry + s, sl.carried};
-            int rc = run_stage(c, kind, op, a, stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), stage_hc_large(op, src_len, p.b0, p.b1),
+            const int32_t hc_large = cut ? (op == Op::ENCODE_HC && sc->block_size > 65536 ? m : 0) : stage_hc_large(op, src_len, p.b0, p.b1);
+            int rc = run_stage(c, kind, op, a, stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), hc_large,
                                wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), placed ? &pl : nullptr,
-                               nullptr, sl.stream);
+                               framed ? d.aux : nullptr, sl.stream);
             if (rc) return rc;
+            if (framed) {
+                rc = launched(launch_stream_status(d.sl, d.aux, d.out, m, failed, sl.stream, &c->launches), "stream status launch");
+                if (rc) return rc;
+                continue;
+            }
             if (!enc) {
                 CU(cudaMemcpyAsync(out_len + p.b0, d.out, sizeof(int32_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
                 if (placed) {
@@ -937,28 +1008,39 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
                 }
                 continue;
             }
-            cudaError_t e = launch_compact(nullptr, nullptr, d.out, nullptr, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
+            // what lands: the compacted blocks, or an LZ4Stream stage's frames (dense = the frames, at their scan, of their sizes)
+            const uint8_t* frames = (const uint8_t*)sl.frames.p;
+            cudaError_t e = cut ? write_frames(c, a, op == Op::ENCODE_HC, d.aux, offs, sl.scan.p, sl.scan.cap, (uint8_t*)frames, sl.stream)
+                                : launch_compact(nullptr, nullptr, d.out, nullptr, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
             if (e == cudaSuccess && k > 0) e = cudaStreamWaitEvent(sl.stream, c->aslot[prev].carried, 0);
             if (e == cudaSuccess)
-                e = launch_land((const uint8_t*)sl.io.p, d.dof, d.out, offs, m, p.sp.dsum, k > 0 ? carry + prev : nullptr, dst_total_cap,
-                                dst, out_off + p.b0, out_len + p.b0, carry + s, c->dev, sl.stream, &c->launches);
+                e = cut ? launch_land(frames, offs, d.aux, offs, m, p.sp.dsum + (int64_t)m * STREAM_HEADER_MAX, k > 0 ? carry + prev : nullptr,
+                                      dst_total_cap, dst, nullptr, nullptr, carry + s, c->dev, sl.stream, &c->launches)
+                        : launch_land((const uint8_t*)sl.io.p, d.dof, d.out, offs, m, p.sp.dsum, k > 0 ? carry + prev : nullptr,
+                                      dst_total_cap, dst, out_off + p.b0, out_len + p.b0, carry + s, c->dev, sl.stream, &c->launches);
             if (e != cudaSuccess) return cuda_fail(e, "scan / landing launch");
             CU(cudaEventRecord(sl.carried, sl.stream));
         }
         return LZ4B200_OK;
     };
-    // whatever was enqueued, the caller's stream joins it, and the chain and the metadata block are recorded behind it
-    auto join = [&]() -> int {
+    // whatever was enqueued, the caller's stream joins it, and the chain and the metadata block are recorded behind it; an
+    // LZ4Stream call whose stages are all in writes its size or status in between
+    auto join = [&](bool all_in) -> int {
         for (int s = 0; s < used; s++) {
             CU(cudaEventRecord(c->aslot[s].done, c->aslot[s].stream));
             CU(cudaStreamWaitEvent(caller, c->aslot[s].done, 0));
         }
+        int tail = LZ4B200_OK;
+        if (all_in && cut)
+            tail = launched(cudaMemcpyAsync(out_off, carry + (plan.size() - 1) % NASYNC, sizeof(int64_t), cudaMemcpyDefault, caller),
+                            "stream size copy");
+        if (all_in && framed) tail = launched(launch_stream_result(failed, sc->total, out_off, caller, &c->launches), "stream result launch");
         CU(c->async_done.record(caller, Capture{}));
-        CU(cudaEventRecord(blk->done, caller));
-        return LZ4B200_OK;
+        if (blk) CU(cudaEventRecord(blk->done, caller));
+        return tail;
     };
     rc = stages();
-    const int jr = join();
+    const int jr = join(rc == LZ4B200_OK);
     return rc ? rc : jr;
 }
 
@@ -976,61 +1058,104 @@ int wrap_caps(const int32_t* src_len, const int32_t* slot_cap, int32_t n, std::v
 }
 
 // The asynchronous packed encodes from device memory into page-locked host memory (the codec's blocks; Wrap packets,
-// kind WRAP_ENCODE, whose capacities are their own): the argument checks, the capture refusal and the kinds of memory,
-// then run_async.  n == 0 writes out_off[0] = 0 on the stream.
+// kind WRAP_ENCODE, whose capacities are their own; an LZ4Stream, kind STREAM_ENCODE with sc, whose arguments the caller
+// has checked (stream_encode_args) and whose size goes to out_off[0]): the argument checks, the capture refusal and the
+// kinds of memory, then run_async.  n == 0 (for a stream, sc->n == 0) writes out_off[0] = 0 on the stream.
 int landed_async(lz4b200_ctx* c, Stage kind, int mode, const void* src, const int64_t* src_off, const int32_t* src_len,
                  const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
-                 void* stream, const char* what)
+                 void* stream, const char* what, const StreamCall* sc = nullptr)
 {
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
-    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-    const bool wrap = kind == Stage::WRAP_ENCODE;
-    if (n > 0 && (!src || !src_off || !src_len || (!wrap && !dst_cap) || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-    // a Wrap's dense slots hold whole packets
     std::vector<int32_t> pcap;
-    int rc = wrap ? wrap_caps(src_len, nullptr, n, pcap) : check_lengths(src_len, dst_cap, n, "block"); if (rc) return rc;
-    if (wrap) dst_cap = pcap.data();
+    if (!sc) {
+        if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+        const bool wrap = kind == Stage::WRAP_ENCODE;
+        if (n > 0 && (!src || !src_off || !src_len || (!wrap && !dst_cap) || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+        // a Wrap's dense slots hold whole packets
+        int rc = wrap ? wrap_caps(src_len, nullptr, n, pcap) : check_lengths(src_len, dst_cap, n, "block"); if (rc) return rc;
+        if (wrap) dst_cap = pcap.data();
+    }
     CallGuard g(c); if (g.rc) return g.rc;
-    rc = refuse_capture(stream, what, false); if (rc) return rc;
+    int rc = refuse_capture(stream, what, false); if (rc) return rc;
     void *off_at = nullptr, *dst_at = nullptr, *len_at = nullptr;
-    rc = device_address(c, out_off, true, "out_off", &off_at); if (rc) return rc;
-    if (n == 0) { CU(cudaMemsetAsync(off_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
+    rc = device_address(c, out_off, true, sc ? "out_size" : "out_off", &off_at); if (rc) return rc;
+    if (sc ? sc->n == 0 : n == 0) { CU(cudaMemsetAsync(off_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
     rc = check_side(c, src, true, "src"); if (rc) return rc;
     rc = device_address(c, dst, false, "dst", &dst_at); if (rc) return rc;
-    rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc;
+    if (!sc) { rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc; }
     return run_async(c, kind, encode_op(mode == LZ4B200_MODE_HC), (const uint8_t*)src, src_off, src_len, (uint8_t*)dst_at, nullptr,
-                     dst_cap, (int32_t*)len_at, n, (int64_t*)off_at, dst_total_cap, (cudaStream_t)stream);
+                     dst_cap, (int32_t*)len_at, n, (int64_t*)off_at, dst_total_cap, (cudaStream_t)stream, sc);
+}
+
+// The decode entries of an LZ4Stream of n bytes at s, from its header walk (stream_walk): one per non-empty chunk, with
+// its payload offset, compLen, output offset, rawLen and stored flag -- the header's flag: a compressed chunk may have
+// compLen == rawLen (LZ4Stream.cs:288).  Returns the decoded size or LZ4B200_E_FORMAT.
+struct StreamEntries { std::vector<int64_t> so, dof; std::vector<int32_t> len, raw; std::vector<uint8_t> stored; };
+int64_t stream_entries(const uint8_t* s, int64_t n, StreamEntries* e)
+{
+    std::vector<StreamChunk> chunks;
+    const int64_t total = stream_walk(s, n, &chunks);
+    if (total < 0) return total;
+    int64_t pos = 0;
+    for (const StreamChunk& k : chunks) {
+        if (k.raw > 0) {
+            e->so.push_back(k.payload); e->len.push_back(k.stored); e->dof.push_back(pos); e->raw.push_back(k.raw);
+            e->stored.push_back(!k.compressed);
+        }
+        pos += k.raw;
+    }
+    return total;
 }
 
 // The asynchronous decodes from page-locked host memory into device memory (the codec's blocks; Unwrap packets, kind
 // UNWRAP), into the caller's slots or packed (out_off, dst_total_cap; no dst_off, dst_cap): the argument checks, the
 // capture refusal and the kinds of memory, then run_async.  A packed call with n == 0 writes out_off[0] = 0 on the stream.
+// An LZ4Stream (stream_n >= 0: its length; kind FRAMED_DECODE, packed) has no arrays: the host walks its headers once src
+// is known to be page-locked, and its entries are the batch.  A malformed header is the call's LZ4B200_E_FORMAT, a decoded
+// size above dst_total_cap its LZ4B200_E_ARG, both before any device work; the decoded size, or the status the device
+// finds, goes to out_off[0], and 0 when the stream decodes to nothing.
 int staged_async(lz4b200_ctx* c, Stage kind, Op op, bool packed, const void* src, const int64_t* src_off, const int32_t* src_len,
                  void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
-                 int64_t dst_total_cap, void* stream, const char* what)
+                 int64_t dst_total_cap, void* stream, const char* what, int64_t stream_n = -1)
 {
     const char* unit = kind == Stage::UNWRAP ? "packet" : "block";
+    const bool lz4s = stream_n >= 0;
     if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (packed && (n < 0 || !out_off || dst_total_cap < 0)) return fail(LZ4B200_E_ARG, "bad argument");
-    if (n < 0) return fail(LZ4B200_E_ARG, std::string("negative ") + unit + " count");
-    if (n > 0 && (!src || !src_off || !src_len || !dst || (!packed && (!dst_off || !dst_cap)) || !out_len))
-        return fail(LZ4B200_E_ARG, "null argument");
-    int rc = check_lengths(src_len, dst_cap, n, unit); if (rc) return rc;
-    CallGuard g(c); if (g.rc) return g.rc;
-    rc = refuse_capture(stream, what, false); if (rc) return rc;
-    void* at = nullptr;
-    if (packed) {
-        rc = device_address(c, out_off, true, "out_off", &at); if (rc) return rc;
-        if (n == 0) { CU(cudaMemsetAsync(at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
+    if (!lz4s) {
+        if (packed && (n < 0 || !out_off || dst_total_cap < 0)) return fail(LZ4B200_E_ARG, "bad argument");
+        if (n < 0) return fail(LZ4B200_E_ARG, std::string("negative ") + unit + " count");
+        if (n > 0 && (!src || !src_off || !src_len || !dst || (!packed && (!dst_off || !dst_cap)) || !out_len))
+            return fail(LZ4B200_E_ARG, "null argument");
+        int rc = check_lengths(src_len, dst_cap, n, unit); if (rc) return rc;
     }
-    if (n == 0) return LZ4B200_OK;
+    CallGuard g(c); if (g.rc) return g.rc;
+    int rc = refuse_capture(stream, what, false); if (rc) return rc;
+    void *at = nullptr, *total_at = nullptr;
+    if (packed) {
+        rc = device_address(c, out_off, true, lz4s ? "out_size" : "out_off", &total_at); if (rc) return rc;
+        if (lz4s ? stream_n == 0 : n == 0) { CU(cudaMemsetAsync(total_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
+    }
+    if (n == 0 && !lz4s) return LZ4B200_OK;
     rc = device_address(c, src, false, "src", &at); if (rc) return rc;
+    StreamEntries e;
+    StreamCall sc;
+    if (lz4s) {
+        // src is final: a caller who knows the stream's length has its bytes in place
+        const int64_t total = stream_entries((const uint8_t*)src, stream_n, &e);
+        if (total < 0) return fail((int)total, "malformed LZ4Stream");
+        if (total > dst_total_cap || (total > 0 && !dst)) return fail(LZ4B200_E_ARG, "dst_cap < the decoded size");
+        if (total == 0) { CU(cudaMemsetAsync(total_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
+        if (e.so.size() > (size_t)INT32_MAX) return fail(LZ4B200_E_ARG, "more than INT32_MAX non-empty chunks");
+        n = (int32_t)e.so.size();
+        src_off = e.so.data(); src_len = e.len.data(); dst_off = e.dof.data(); dst_cap = e.raw.data(); out_off = (int64_t*)total_at;
+        sc = StreamCall{stream_n, 0, e.stored.data(), total};
+    }
     rc = check_side(c, dst, true, "dst"); if (rc) return rc;
-    rc = device_address(c, out_len, true, "out_len", &at); if (rc) return rc;
+    if (!lz4s) { rc = device_address(c, out_len, true, "out_len", &at); if (rc) return rc; }
     // (the stages copy out_len and out_off at the caller's addresses, which the copy engines take for either kind)
     return run_async(c, kind, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, out_off,
-                     dst_total_cap, (cudaStream_t)stream);
+                     dst_total_cap, (cudaStream_t)stream, lz4s ? &sc : nullptr);
 }
 
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
@@ -1110,9 +1235,14 @@ int single(const char* source, char* dest, int isize, int ocap, Op op)
     return out;
 }
 
-// The LZ4Stream calls run the pipeline over at most this many chunks at a time: it bounds the host metadata by chunk
-// count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.
-constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
+// The arguments of an LZ4Stream encode of n bytes in block_size chunks into dst_cap bytes, synchronous or not.
+int stream_encode_args(const lz4b200_ctx* c, const void* src, int64_t n, int32_t block_size, const void* dst, int64_t dst_cap)
+{
+    if (!c || n < 0 || block_size < 1 || (n > 0 && (!src || !dst))) return fail(LZ4B200_E_ARG, "bad argument");
+    if (std::min<int64_t>(block_size, n) > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "a chunk's frame must fit an int32");
+    if (dst_cap < lz4b200_stream_bound(n, block_size)) return fail(LZ4B200_E_ARG, "dst_cap < lz4b200_stream_bound(n, block_size)");
+    return LZ4B200_OK;
+}
 
 // The LZ4Stream of n bytes in host or device memory (src_dev), written into host memory: each run of chunks is encoded
 // (capacity = the chunk's length, LZ4Stream.cs:243-246) and its frames land back to back (STREAM_ENCODE, APPEND).  Returns
@@ -1120,9 +1250,7 @@ constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
 int64_t stream_encode(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_size, int high_compression, void* dst,
                       int64_t dst_cap, bool src_dev, void* stream)
 {
-    if (!c || n < 0 || block_size < 1 || (n > 0 && (!src || !dst))) return fail(LZ4B200_E_ARG, "bad argument");
-    if (std::min<int64_t>(block_size, n) > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "a chunk's frame must fit an int32");
-    if (dst_cap < lz4b200_stream_bound(n, block_size)) return fail(LZ4B200_E_ARG, "dst_cap < lz4b200_stream_bound(n, block_size)");
+    if (int rc = stream_encode_args(c, src, n, block_size, dst, dst_cap)) return rc;
     if (n == 0) return 0;
     CallGuard g(c); if (g.rc) return g.rc;
     if (src_dev) {
@@ -1159,30 +1287,24 @@ int64_t stream_decode(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int
         int rc = refuse_capture(stream, "lz4b200_stream_decode_to_device"); if (rc) return rc;
         rc = check_side(c, src, false, "src"); if (rc) return rc;
     }
-    std::vector<StreamChunk> chunks;
-    const int64_t total = stream_walk((const uint8_t*)src, n, &chunks);
+    StreamEntries e;
+    const int64_t total = stream_entries((const uint8_t*)src, n, &e);
     if (total < 0) return fail((int)total, "malformed LZ4Stream");
     if (total > dst_cap || (total > 0 && !dst)) return fail(LZ4B200_E_ARG, "dst_cap < the decoded size");
     if (total == 0) return 0;
     if (dst_dev) { int rc = check_side(c, dst, true, "dst"); if (rc) return rc; }
-    // one entry per non-empty chunk; the flag is the header's (a compressed chunk may have compLen == rawLen, LZ4Stream.cs:288)
-    std::vector<int64_t> so, dof; std::vector<int32_t> len, raw, res; std::vector<uint8_t> stored;
-    int64_t pos = 0;
-    for (const StreamChunk& k : chunks) {
-        if (k.raw > 0) { so.push_back(k.payload); len.push_back(k.stored); dof.push_back(pos); raw.push_back(k.raw); stored.push_back(!k.compressed); }
-        pos += k.raw;
-    }
-    const int64_t entries = (int64_t)so.size();
+    std::vector<int32_t> res;
+    const int64_t entries = (int64_t)e.so.size();
     for (int64_t e0 = 0; e0 < entries; e0 += STREAM_RUN_CHUNKS) {
         const int32_t m = (int32_t)std::min(STREAM_RUN_CHUNKS, entries - e0);
         res.assign(m, -1);
-        int rc = run_host(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, (const uint8_t*)src, so.data() + e0, len.data() + e0,
-                          (uint8_t*)dst, dof.data() + e0, raw.data() + e0, res.data(), m, nullptr, 0, false, dst_dev,
-                          (cudaStream_t)stream, stored.data() + e0);
+        int rc = run_host(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, (const uint8_t*)src, e.so.data() + e0, e.len.data() + e0,
+                          (uint8_t*)dst, e.dof.data() + e0, e.raw.data() + e0, res.data(), m, nullptr, 0, false, dst_dev,
+                          (cudaStream_t)stream, e.stored.data() + e0);
         if (rc) return rc;
         // a compressed chunk decodes from exactly its compLen bytes (LZ4Codec.Safe.cs:539-542)
         for (int32_t i = 0; i < m; i++)
-            if (!stored[e0 + i] && res[i] != len[e0 + i]) return fail(LZ4B200_E_FORMAT, "a chunk does not decode to its compressed length");
+            if (!e.stored[e0 + i] && res[i] != e.len[e0 + i]) return fail(LZ4B200_E_FORMAT, "a chunk does not decode to its compressed length");
     }
     return total;
 }
@@ -1312,7 +1434,7 @@ int lz4b200_create(lz4b200_ctx** out, int device)
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device); c->dev.smem_per_sm = v;
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device); c->dev.smem_optin = v;
     cudaError_t e = cudaMalloc(&c->counters, sizeof(uint32_t) * (NCOUNTER + 4 * NCAPTURED));
-    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * (NSLOT + NASYNC));
+    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * (NSLOT + NASYNC + 1));
     for (Chain* ch : {&c->hc_done, &c->compact_done, &c->async_done}) {
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->done, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->inner, cudaEventDisableTiming);
@@ -1421,6 +1543,27 @@ int lz4b200_unwrap_batch_packed_to_device_async(lz4b200_ctx* c, const void* src,
 {
     return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, true, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
                         dst_total_cap, stream, "lz4b200_unwrap_batch_packed_to_device_async");
+}
+
+// An LZ4Stream without blocking: the encode's chunk table is computed on the device and its frames land like the packed
+// encode's blocks (STREAM_ENCODE); the decode's headers are walked on the host during the call (FRAMED_DECODE).
+int lz4b200_stream_encode_from_device_async(lz4b200_ctx* c, const void* src, int64_t n, int32_t block_size, int high_compression,
+                                            void* dst, int64_t dst_cap, int64_t* out_size, void* stream)
+{
+    if (block_size > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "block_size: a chunk's frame must fit an int32");
+    if (int rc = stream_encode_args(c, src, n, block_size, dst, dst_cap)) return rc;
+    if (!out_size) return fail(LZ4B200_E_ARG, "bad argument");
+    const StreamCall sc{n, block_size};
+    return landed_async(c, Stage::STREAM_ENCODE, high_compression ? LZ4B200_MODE_HC : LZ4B200_MODE_FAST, src, nullptr, nullptr, nullptr,
+                        dst, dst_cap, out_size, nullptr, 0, stream, "lz4b200_stream_encode_from_device_async", &sc);
+}
+
+int lz4b200_stream_decode_to_device_async(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int64_t dst_cap, int64_t* out_size,
+                                          void* stream)
+{
+    if (!c || n < 0 || (n > 0 && !src) || !out_size) return fail(LZ4B200_E_ARG, "bad argument");
+    return staged_async(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, true, src, nullptr, nullptr, dst, nullptr, nullptr, nullptr, 0,
+                        out_size, dst_cap, stream, "lz4b200_stream_decode_to_device_async", n);
 }
 
 // ---- LZ4Stream (lz4_stream.cuh): the host pipeline, the frames written on the device ----------------------------------

@@ -54,7 +54,8 @@ size_t      compact_tmp_bytes(int32_t n_blocks);
 // One stage of the asynchronous packed encode into mapped host memory (land.cu, lz4_land.cuh): block i of the stage's
 // dense slots (dense + dof[i], len[i] bytes; off = the scan of len, m + 1 entries) lands at dst + base + off[i] when
 // base + off[m] <= total_cap, base = *base_in (null: 0).  out_off[0..m] = base + off, out_len[0..m) = len and
-// *total_out = base + off[m] are written either way.  dense_bytes bounds off[m] (the slots' size) and sizes the launch.
+// *total_out = base + off[m] are written either way; out_off and out_len may be null (an LZ4Stream encode's frames: only
+// the total is kept).  dense_bytes bounds off[m] (the slots' size) and sizes the launch.
 cudaError_t launch_land(const uint8_t* dense, const int64_t* dof, const int32_t* len, const int64_t* off, int32_t m,
                         int64_t dense_bytes, const int64_t* base_in, int64_t total_cap, uint8_t* dst, int64_t* out_off,
                         int32_t* out_len, int64_t* total_out, const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
@@ -77,6 +78,15 @@ cudaError_t launch_stream_frame(const BatchArgs& a, bool hc, uint8_t* frames, co
 // a = the decoded batch (src / src_off = the staged stream and the payload offsets, dst / dst_off = the output): copies
 // stored_len[i] bytes of payload i to its output; entries with stored_len[i] == 0 do nothing
 cudaError_t launch_stream_stored(const BatchArgs& a, const int32_t* stored_len, cudaStream_t stream, int64_t* launches);
+// The asynchronous LZ4Stream calls.  launch_stream_cut: the chunk table of an encode stage of m chunks from chunk `first`
+// of a stream of n bytes (stream_cut_one).  launch_stream_status: *failed = 1 when a compressed entry of a decode stage
+// (stored[i] == 0) did not read exactly comp_len[i] bytes (res[i]); it never clears it.  launch_stream_result, one thread:
+// *out_size = *failed ? LZ4B200_E_FORMAT : total.
+cudaError_t launch_stream_cut(int64_t first, int32_t m, int32_t block_size, int64_t n, int64_t* so, int32_t* len, int64_t* dof,
+                              int32_t* cap, cudaStream_t stream, int64_t* launches);
+cudaError_t launch_stream_status(const int32_t* comp_len, const int32_t* stored, const int32_t* res, int32_t m, int* failed,
+                                 cudaStream_t stream, int64_t* launches);
+cudaError_t launch_stream_result(const int* failed, int64_t total, int64_t* out_size, cudaStream_t stream, int64_t* launches);
 cudaError_t launch_synth(uint8_t* dst, int64_t n_blocks, int32_t block_size, int cls, uint64_t seed, int64_t first_block,
                          const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 

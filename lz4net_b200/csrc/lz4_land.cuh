@@ -32,14 +32,14 @@ SIMT_DEV int64_t land_units(const uint8_t* at, int64_t total)
 
 // Entry i of the stage's results, thread i of m + 1: out_off[i] = base + off[i] (out_off[m] = the new running total, which
 // the next stage writes again as its out_off[0]), out_len[i] = len[i]; thread m also leaves the running total for the
-// next stage in *total_out.
+// next stage in *total_out.  A null out_off or out_len is not written (an LZ4Stream encode keeps only the total).
 SIMT_DEV void land_place(int64_t i, const int32_t* len, const int64_t* off, int32_t m, int64_t base, int64_t* out_off,
                          int32_t* out_len, int64_t* total_out)
 {
     if (i > m) return;
-    out_off[i] = base + off[i];
-    if (i < m) out_len[i] = len[i];
-    else *total_out = base + off[m];
+    if (out_off) out_off[i] = base + off[i];
+    if (i == m) *total_out = base + off[m];
+    else if (out_len) out_len[i] = len[i];
 }
 
 // Unit u of the stage's bytes at `at` (= dst + base).

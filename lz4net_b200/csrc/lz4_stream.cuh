@@ -11,6 +11,8 @@
 //            stored chunk, from the source: the caller's device memory, or the pipeline's staged copy of host bytes)
 //   decode:  known-size decode of the compressed chunks (stored ones get the neutral entry, see lz4_wrap.cuh) -> stored
 //            copy (a warp per chunk: a stored chunk's payload to its place in the output; compressed chunks do nothing)
+// The asynchronous calls add two per-thread rules: the encode's chunk table, computed on the device (stream_cut_one), and
+// the decode's status, kept on the device (stream_chunk_failed).
 // This is the library's only writer of the format.
 #pragma once
 #include "lz4_copy.cuh"
@@ -75,5 +77,22 @@ SIMT_DEV void stream_stored_one(const uint8_t* payload, int32_t stored, uint8_t*
     const InputSrc s{payload};
     group_copy<32, false>(dst, s, (uint32_t)stored, lane, 0xFFFFFFFFu);
 }
+
+// The asynchronous encode (capi.cu run_async) holds no per-chunk host metadata: each stage's chunk table is computed on
+// the device.  Entry i of the stage whose first chunk is `first`, in a stream of n bytes cut into block_size chunks: the
+// chunk is bytes [so, so + len) of the source, encoded into the stage's dense slot at dof with capacity cap = len.  Only
+// a stream's last chunk is short, so slot i starts at i * block_size.
+SIMT_DEV void stream_cut_one(int64_t i, int64_t first, int32_t block_size, int64_t n, int64_t* so, int32_t* len, int64_t* dof,
+                             int32_t* cap)
+{
+    const int64_t at = (first + i) * block_size;
+    const int32_t l = (int32_t)(n - at < block_size ? n - at : block_size);
+    so[i] = at; len[i] = l; dof[i] = i * (int64_t)block_size; cap[i] = l;
+}
+
+// The decode's status rule: an entry fails when it is a compressed chunk (stored == 0: no stored payload) whose known-size
+// decode did not read exactly its compLen bytes (res, negative for a malformed block; LZ4Codec.Safe.cs:539-542).  Stored
+// chunks are copied, never decoded, and never fail.
+SIMT_DEV bool stream_chunk_failed(int32_t stored, int32_t comp_len, int32_t res) { return stored == 0 && res != comp_len; }
 
 }  // namespace lz4b200

@@ -1,4 +1,5 @@
 // stream.cu -- kernels + launchers of the LZ4Stream frame steps in device memory (see lz4_stream.cuh for the rules).
+#include "../../include/lz4b200.h"
 #include "kernels.h"
 #include "lz4_stream.cuh"
 
@@ -35,6 +36,51 @@ lz4_stream_stored_kernel(const uint8_t* src, const int64_t* src_off, const int32
     const int64_t i = (int64_t)blockIdx.x * COPY_WARPS + (threadIdx.x >> 5);
     if (i >= n) return;
     stream_stored_one(src + src_off[i], stored_len[i], dst + dst_off[i], (int)(threadIdx.x & 31));
+}
+
+__global__ void __launch_bounds__(SIZE_THREADS)
+lz4_stream_cut_kernel(int64_t first, int32_t m, int32_t block_size, int64_t n, int64_t* so, int32_t* len, int64_t* dof, int32_t* cap)
+{
+    const int64_t i = (int64_t)blockIdx.x * SIZE_THREADS + threadIdx.x;
+    if (i < m) stream_cut_one(i, first, block_size, n, so, len, dof, cap);
+}
+
+// Every failing entry stores 1; nothing stores 0, so the racing stores agree.
+__global__ void __launch_bounds__(SIZE_THREADS)
+lz4_stream_status_kernel(const int32_t* comp_len, const int32_t* stored, const int32_t* res, int32_t m, int* failed)
+{
+    const int64_t i = (int64_t)blockIdx.x * SIZE_THREADS + threadIdx.x;
+    if (i < m && stream_chunk_failed(stored[i], comp_len[i], res[i])) *failed = 1;
+}
+
+__global__ void lz4_stream_result_kernel(const int* failed, int64_t total, int64_t* out_size)
+{
+    *out_size = *failed ? (int64_t)LZ4B200_E_FORMAT : total;
+}
+
+cudaError_t launch_stream_cut(int64_t first, int32_t m, int32_t block_size, int64_t n, int64_t* so, int32_t* len, int64_t* dof,
+                              int32_t* cap, cudaStream_t stream, int64_t* launches)
+{
+    if (m <= 0) return cudaSuccess;
+    lz4_stream_cut_kernel<<<size_grid(m), SIZE_THREADS, 0, stream>>>(first, m, block_size, n, so, len, dof, cap);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_stream_status(const int32_t* comp_len, const int32_t* stored, const int32_t* res, int32_t m, int* failed,
+                                 cudaStream_t stream, int64_t* launches)
+{
+    if (m <= 0) return cudaSuccess;
+    lz4_stream_status_kernel<<<size_grid(m), SIZE_THREADS, 0, stream>>>(comp_len, stored, res, m, failed);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_stream_result(const int* failed, int64_t total, int64_t* out_size, cudaStream_t stream, int64_t* launches)
+{
+    lz4_stream_result_kernel<<<1, 1, 0, stream>>>(failed, total, out_size);
+    if (launches) ++*launches;
+    return cudaGetLastError();
 }
 
 cudaError_t launch_stream_frame_size(const BatchArgs& a, int32_t* frame_len, cudaStream_t stream, int64_t* launches)
