@@ -243,6 +243,37 @@ int lz4b200_unwrap_batch_packed_to_device_async(lz4b200_ctx* ctx, const void* sr
                                                 const int32_t* src_len, void* dst, int64_t dst_total_cap, int64_t* out_off,
                                                 int32_t* out_len, int32_t n, void* stream);
 
+/* Restoring from offsets that exist only on the device.  The packed asynchronous encode and Wrap write out_off on the
+ * device, so the calls above, which read src_off / src_len on the host during the call, would make the caller wait for the
+ * offload first.  The two calls below take src_off where the device reads it, when the call's work runs, so a whole
+ * offload -> restore round trip is enqueued with no host wait: pass the offload's out_off as src_off, and its own
+ * src_off / src_len as dst_off / dst_cap.
+ *   - src is page-locked host memory, of which src_cap bytes may be read: nothing outside [src, src + src_cap) is read,
+ *     whatever src_off holds, except the rest of an aligned 16-byte unit that overlaps the range (which lies in the same
+ *     page-locked page).  src_off has n + 1 int64 entries, in device memory of the context's GPU or in page-locked host
+ *     memory; block i spans [src_off[i], src_off[i+1]).  dst, dst_off, dst_cap and out_len are as in the host-offset form.
+ *   - Each block's span may be at most a bound the host knows, by which the call sizes its stage buffers: a decode's
+ *     lz4b200_compress_bound(dst_cap[i]); an Unwrap packet's dst_cap[i] + 8 (no packet that restores into dst_cap[i]
+ *     bytes is larger).
+ *   - A span is well-formed when 0 <= src_off[i] <= src_off[i+1] <= src_cap and its length is at most its bound.  Then
+ *     out_len[i] and the bytes written equal what the host-offset form gives with src_len[i] = src_off[i+1] - src_off[i].
+ *     Otherwise out_len[i] = LZ4B200_E_ARG, nothing of that block is read and nothing in its dst range is written.  This is
+ *     where the two forms differ: a span longer than its bound (a packet with trailing bytes, for one) is rejected here
+ *     but may be accepted by the host-offset form.
+ *   - src_off[n] > src_cap means the offload that wrote the offsets did not fit its destination, so which of its bytes
+ *     landed is unknown: every block is LZ4B200_E_ARG and dst is not written.  A destination sized by the offload's bound
+ *     never hits this: sum(dst_cap) at compress_bound for an encode, sum(src_len + 8) for a Wrap.
+ *   - The rest is the contract of the asynchronous calls above; the dst_off and dst_cap arrays are read during the call.
+ *
+ * decode_batch_to_device_at_async: lz4b200_decode_batch_to_device_async with the blocks' offsets read on the device.
+ * unwrap_batch_to_device_at_async: lz4b200_unwrap_batch_to_device_async with the packets' offsets read on the device. */
+int lz4b200_decode_batch_to_device_at_async(lz4b200_ctx* ctx, const void* src, int64_t src_cap, const int64_t* src_off,
+                                            void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len,
+                                            int32_t n_blocks, int known_len, void* stream);
+int lz4b200_unwrap_batch_to_device_at_async(lz4b200_ctx* ctx, const void* src, int64_t src_cap, const int64_t* src_off,
+                                            void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len,
+                                            int32_t n, void* stream);
+
 /* Compaction of fixed-stride encoder slots into one contiguous payload (device memory only): the batched form of
  * the Buffer.BlockCopy trim in LZ4Codec.Encode (src/LZ4/LZ4Codec.cs:357-364).  out_off[i] (int64, n_blocks+1
  * entries) = exclusive prefix sum of max(len[i],0); block i's bytes are copied to packed + out_off[i]. */
@@ -274,6 +305,7 @@ int lz4b200_compact(lz4b200_ctx* ctx, const void* slots, const int64_t* slot_off
  * stream it returns LZ4B200_E_ARG before any CUDA work, and the capture stays valid.  So do the asynchronous calls --
  * lz4b200_encode_batch_packed_from_device_async, decode_batch_to_device_async, decode_batch_packed_to_device_async,
  * wrap_batch_packed_from_device_async, unwrap_batch_to_device_async, unwrap_batch_packed_to_device_async,
+ * decode_batch_to_device_at_async, unwrap_batch_to_device_at_async,
  * stream_encode_from_device_async and stream_decode_to_device_async -- which do not synchronise but share the context's
  * stage buffers between eager calls and, all but the stream encode, hand the device host metadata that a graph would have
  * to keep alive.  lz4b200_peer_copy is not covered.

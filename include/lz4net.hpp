@@ -125,6 +125,22 @@ public:
                                                         stream) != LZ4B200_OK)
             throw std::runtime_error(lz4b200_last_error());
     }
+    // The decode and the Unwrap from offsets the device wrote (lz4b200_decode_batch_to_device_at_async,
+    // lz4b200_unwrap_batch_to_device_at_async): src_off (n + 1 entries, device or page-locked memory) is read on the device,
+    // so the out_off of a packed offload above can be passed straight in; only src_cap bytes of src are read.
+    void decode_from_host_at_async(const void* src, int64_t src_cap, const int64_t* src_off, void* dst, const int64_t* dst_off,
+                                   const int32_t* dst_cap, int32_t* out_len, int32_t n, bool known, void* stream)
+    {
+        if (lz4b200_decode_batch_to_device_at_async(h_, src, src_cap, src_off, dst, dst_off, dst_cap, out_len, n, known ? 1 : 0,
+                                                    stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
+    void unwrap_from_host_at_async(const void* src, int64_t src_cap, const int64_t* src_off, void* dst, const int64_t* dst_off,
+                                   const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
+    {
+        if (lz4b200_unwrap_batch_to_device_at_async(h_, src, src_cap, src_off, dst, dst_off, dst_cap, out_len, n, stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
     // The same for an LZ4Stream (lz4b200_stream_encode_from_device_async, lz4b200_stream_decode_to_device_async): n bytes
     // of device memory as one stream in page-locked host memory, and back.  out_size is written by the device: the
     // stream's size, or the decoded size (LZ4B200_E_FORMAT when a chunk does not decode).  The decode walks the stream's

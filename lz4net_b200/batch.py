@@ -32,7 +32,9 @@ encode_to_host_packed_async and decode_from_host_async move blocks between a dev
 without blocking the calling thread: they enqueue their work on a stream and return, so a thread that launches a model's
 kernels can offload to host RAM, or prefetch back, and keep launching.  decode_from_host_packed_async,
 wrap_to_host_packed_async, unwrap_to_device_async and unwrap_to_device_packed_async do the same for the packed decode and
-for Wrap packets, which carry their own sizes and never exceed input + 8 bytes.  stream_encode_to_host_async and
+for Wrap packets, which carry their own sizes and never exceed input + 8 bytes.  decode_from_host_at_async and
+unwrap_to_device_at_async bring such an offload back from the out_off the device wrote, with no synchronisation in
+between.  stream_encode_to_host_async and
 stream_decode_to_device_async do it for an LZ4Stream: one byte string, one pointer and one length, that any LZ4Stream reads.
 They refuse a capturing stream.
 """
@@ -290,6 +292,42 @@ def unwrap_to_device_packed_async(ctx: Context, packets: torch.Tensor, src_off, 
     native.check(native.lib().lz4b200_unwrap_batch_packed_to_device_async(
         ctx.handle, p, _h(src_off, np.int64), _h(src_len, np.int32, n), _d(out), out.nbytes, off, res, n, _stream_of(stream)),
         "unwrap_batch_packed_to_device_async")
+
+
+def _at_args(comp, src_cap, src_off, out_len, n, what):
+    """The page-locked source, its readable bytes and the device-read offsets of the *_at_async calls."""
+    c = _pinned(comp, torch.uint8, 0, what)
+    if not 0 <= src_cap <= comp.numel():
+        raise ValueError(f"src_cap: {src_cap} is not within the {comp.numel()} bytes of {what}")
+    return c, _pinned(src_off, torch.int64, n + 1, "src_off", True), _pinned(out_len, torch.int32, n, "out_len", True)
+
+
+def decode_from_host_at_async(ctx: Context, comp: torch.Tensor, src_cap: int, src_off: torch.Tensor, out: torch.Tensor, dst_off,
+                              dst_cap, out_len: torch.Tensor, known: bool = True, stream=None):
+    """decode_from_host_async whose block offsets are read on the device, when the call's work runs
+    (lz4b200_decode_batch_to_device_at_async): block i spans comp[src_off[i]:src_off[i+1]] and is decoded at
+    out + dst_off[i].  src_off (int64[n+1]) is a CUDA or page-locked CPU tensor -- the out_off an
+    encode_to_host_packed_async has just written, for one -- so the round trip needs no synchronisation in between.  Only
+    the first src_cap bytes of comp are read.  A span that is not within them, runs backwards or is longer than
+    compress_bound(dst_cap[i]) gets out_len[i] = LZ4B200_E_ARG and nothing written; so does every block when
+    src_off[n] > src_cap.  dst_off / dst_cap are numpy arrays, read during the call."""
+    n = len(dst_off)
+    c, off, res = _at_args(comp, src_cap, src_off, out_len, n, "comp")
+    native.check(native.lib().lz4b200_decode_batch_to_device_at_async(
+        ctx.handle, c, src_cap, off, _d(out), _h(dst_off, np.int64), _h(dst_cap, np.int32, n), res, n, int(known),
+        _stream_of(stream)), "decode_batch_to_device_at_async")
+
+
+def unwrap_to_device_at_async(ctx: Context, packets: torch.Tensor, src_cap: int, src_off: torch.Tensor, out: torch.Tensor, dst_off,
+                              dst_cap, out_len: torch.Tensor, stream=None):
+    """unwrap_to_device_async whose packet offsets are read on the device (lz4b200_unwrap_batch_to_device_at_async): the
+    out_off a wrap_to_host_packed_async has just written can be passed as src_off.  A packet span above dst_cap[i] + 8
+    bytes is LZ4B200_E_ARG; otherwise as decode_from_host_at_async."""
+    n = len(dst_off)
+    p, off, res = _at_args(packets, src_cap, src_off, out_len, n, "packets")
+    native.check(native.lib().lz4b200_unwrap_batch_to_device_at_async(
+        ctx.handle, p, src_cap, off, _d(out), _h(dst_off, np.int64), _h(dst_cap, np.int32, n), res, n, _stream_of(stream)),
+        "unwrap_batch_to_device_at_async")
 
 
 def stream_encode_to_host_async(ctx: Context, raw: torch.Tensor, dst: torch.Tensor, out_size: torch.Tensor,

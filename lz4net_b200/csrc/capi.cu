@@ -23,6 +23,7 @@
 #include "../../include/lz4b200.h"
 #include "framing.h"
 #include "kernels.h"
+#include "lz4_lift.cuh"
 #include "lz4_packed.cuh"
 #include "lz4_stream.cuh"
 #include "lz4_wrap.cuh"
@@ -861,6 +862,25 @@ int take_meta(lz4b200_ctx* c, size_t bytes, MetaBlock** out)
 // (FRAMED_DECODE).
 struct StreamCall { int64_t n = 0; int32_t block_size = 0; const uint8_t* stored = nullptr; int64_t total = 0; };
 
+// The decodes and Unwraps whose block offsets exist only on the device (lz4_lift.cuh): src's device address and the bytes
+// of it that may be read, src_off (n + 1 entries, device memory or page-locked), and each block's bound, by which the
+// stages are cut and their slots sized.
+struct LiftCall { const uint8_t* src = nullptr; int64_t src_cap = 0; const int64_t* src_off = nullptr; std::vector<int32_t> bound; };
+
+// A lift stage's metadata: dst_off / dst_cap as the caller gave them, each block's slot (so[i], and its prefix in off[0..m])
+// and its bound (aux); the spans are written on the device.  sp.shi = the stage's staging bytes.
+StageSpan fill_lift(const Meta& h, int32_t b0, int32_t b1, const int32_t* bound, const int64_t* dst_off, const int32_t* dst_cap)
+{
+    StageSpan sp;
+    for (int32_t i = 0; i < b1 - b0; i++) {
+        h.off[i] = h.so[i] = sp.shi;
+        h.dof[i] = dst_off[b0 + i]; h.sl[i] = 0; h.dc[i] = dst_cap[b0 + i]; h.aux[i] = bound[b0 + i];
+        sp.shi += lift_slot_bytes(bound[b0 + i]);
+    }
+    h.off[b1 - b0] = sp.shi;
+    return sp;
+}
+
 // The LZ4Stream calls run the pipeline over at most this many chunks at a time: it bounds the host metadata by chunk
 // count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.  An asynchronous
 // encode stage takes at most this many chunks, which bounds its device metadata the same way.
@@ -887,6 +907,9 @@ constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
 //    dst_off) measure (PLACED_DECODE) or prep (UNWRAP), scan and place their stage behind the previous one's from the same
 //    carry cells (place), then decode behind the stage's "fits" flag; their absolute offsets are copied to out_off, the
 //    last stage's running total to out_off[n].
+//    A decode or Unwrap from device-written offsets (lc) cuts its stages by the blocks' bounds, stages them with the lift
+//    kernel (lz4_lift.cuh) in place of the copy, and has its decoder picked on the device from the staged spans (the
+//    context's pinned choice, if any, still holds); after the decode, its rejected blocks' results become LZ4B200_E_ARG.
 //    The stage's results are copied to out_len (device or page-locked memory), except for an LZ4Stream decode
 //    (FRAMED_DECODE, sc: the stored flags and the decoded size), whose entries come from the host's header walk: its stages
 //    set the context's failure flag (stream_failed) when a compressed chunk does not decode from exactly its compLen bytes,
@@ -895,10 +918,10 @@ constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
 // Calls are chained through async_done; the call's metadata block is taken again once the caller's stream has passed it.
 int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
               const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
-              int64_t dst_total_cap, cudaStream_t caller, const StreamCall* sc = nullptr)
+              int64_t dst_total_cap, cudaStream_t caller, const StreamCall* sc = nullptr, const LiftCall* lc = nullptr)
 {
     const bool enc = is_encode(op), placed = kind == Stage::PLACED_DECODE || (kind == Stage::UNWRAP && !dst_off);
-    const bool cut = kind == Stage::STREAM_ENCODE, framed = kind == Stage::FRAMED_DECODE;
+    const bool cut = kind == Stage::STREAM_ENCODE, framed = kind == Stage::FRAMED_DECODE, lift = lc != nullptr;
     // blocks [b0, b1) of the batch, their host metadata at `at` in the call's block; an LZ4Stream encode stage's chunks are
     // [first + b0, first + b1) of the stream, b0 = 0
     struct Plan { int32_t b0, b1; size_t at; StageSpan sp; int64_t first; };
@@ -915,7 +938,7 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
         }
     } else {
         for (int32_t b0 = 0; b0 < n;) {
-            const int32_t b1 = stage_end(c, src_len, enc ? dst_cap : nullptr, b0, n, !enc);
+            const int32_t b1 = stage_end(c, lift ? lc->bound.data() : src_len, enc ? dst_cap : nullptr, b0, n, !enc);
             plan.push_back(Plan{b0, b1, bytes, {}, 0});
             bytes += (meta_host_bytes(b1 - b0) + 15) & ~(size_t)15;
             b0 = b1;
@@ -927,7 +950,8 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
     for (size_t k = 0; k < plan.size(); k++) {
         Plan& p = plan[k];
         const int32_t m = p.b1 - p.b0;
-        if (!cut)
+        if (lift) p.sp = fill_lift(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, lc->bound.data(), dst_off, dst_cap);
+        else if (!cut)
             p.sp = fill_stage(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, src_off, src_len, dst_off, dst_cap, enc, !enc, false,
                               placed, framed ? sc->stored : nullptr);
         Sizes& nd = need[k % NASYNC];
@@ -935,6 +959,7 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
         if (cut) nd.frames = std::max(nd.frames, (size_t)p.sp.dsum + (size_t)m * STREAM_HEADER_MAX + 64);
         nd.meta = std::max(nd.meta, async_meta_bytes(m));
         if (enc || placed) { nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(m + 1)); nd.scan = std::max(nd.scan, compact_tmp_bytes(m)); }
+        if (lift) nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(2 * m + 3));      // slot[0..m] | span[0..m+1]
     }
     // growth: an earlier call may still be using the buffers
     bool grow = false;
@@ -976,25 +1001,41 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
                                   "stream chunk table launch");
                 if (rc) return rc;
             } else {
-                // up: the four arrays the kernels read, and a framed decode's stored lengths
+                // up: the four arrays the kernels read, and a framed decode's stored lengths or a lift stage's bounds
                 const Meta h((uint8_t*)blk->buf.p + p.at, m);
-                CU(cudaMemcpyAsync(sl.meta.p, h.so, (size_t)((uint8_t*)(framed ? h.out : h.aux) - (uint8_t*)h.so), cudaMemcpyHostToDevice,
-                                   sl.stream));
+                CU(cudaMemcpyAsync(sl.meta.p, h.so, (size_t)((uint8_t*)(framed || lift ? h.out : h.aux) - (uint8_t*)h.so),
+                                   cudaMemcpyHostToDevice, sl.stream));
             }
             const size_t sbytes = (size_t)(p.sp.shi - p.sp.slo);
-            if (!enc && sbytes) CU(cudaMemcpyAsync(sl.io.p, src + p.sp.slo, sbytes, cudaMemcpyHostToDevice, sl.stream));
+            int64_t* offs = (int64_t*)sl.offs.p;
+            int64_t* span = offs + m + 1;
+            if (lift) {
+                // the slots, then the stage's offsets and src_off[n], wherever the caller's src_off lives
+                CU(cudaMemcpyAsync(offs, Meta((uint8_t*)blk->buf.p + p.at, m).off, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyHostToDevice,
+                                   sl.stream));
+                CU(cudaMemcpyAsync(span, lc->src_off + p.b0, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDefault, sl.stream));
+                CU(cudaMemcpyAsync(span + m + 1, lc->src_off + n, sizeof(int64_t), cudaMemcpyDefault, sl.stream));
+                int rc = launched(launch_lift(lc->src, lc->src_cap, offs, span, m, p.sp.shi, d.aux, d.so, d.sl, d.dc, (uint8_t*)sl.io.p,
+                                              c->dev, sl.stream, &c->launches), "lift launch");
+                if (rc) return rc;
+            } else if (!enc && sbytes) {
+                CU(cudaMemcpyAsync(sl.io.p, src + p.sp.slo, sbytes, cudaMemcpyHostToDevice, sl.stream));
+            }
             // (a packed Unwrap's prep reads no capacity: the placement writes the decode's into d.dc)
             const BatchArgs a{enc ? src : (const uint8_t*)sl.io.p, d.so, d.sl, enc ? (uint8_t*)sl.io.p : dst, d.dof,
                               kind == Stage::UNWRAP && placed ? nullptr : d.dc, d.out, m};
-            int64_t* offs = (int64_t*)sl.offs.p;
             // a packed stage places behind the previous stage's placement (lz4_packed.cuh); the next one follows
             const Placement pl{offs, sl.scan.p, sl.scan.cap, dst_total_cap, 0, d.dc, async_fits(sl.meta.p, m),
                                k > 0 ? c->aslot[prev].carried : nullptr, k > 0 ? carry + prev : nullptr, d.dof, carry + s, sl.carried};
             const int32_t hc_large = cut ? (op == Op::ENCODE_HC && sc->block_size > 65536 ? m : 0) : stage_hc_large(op, src_len, p.b0, p.b1);
-            int rc = run_stage(c, kind, op, a, stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), hc_large,
+            int rc = run_stage(c, kind, op, a, lift ? 0 : stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), hc_large,
                                wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), placed ? &pl : nullptr,
                                framed ? d.aux : nullptr, sl.stream);
             if (rc) return rc;
+            if (lift) {
+                rc = launched(launch_lift_status(lc->src_cap, span, m, d.aux, d.out, sl.stream, &c->launches), "lift status launch");
+                if (rc) return rc;
+            }
             if (framed) {
                 rc = launched(launch_stream_status(d.sl, d.aux, d.out, m, failed, sl.stream, &c->launches), "stream status launch");
                 if (rc) return rc;
@@ -1156,6 +1197,37 @@ int staged_async(lz4b200_ctx* c, Stage kind, Op op, bool packed, const void* src
     // (the stages copy out_len and out_off at the caller's addresses, which the copy engines take for either kind)
     return run_async(c, kind, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, out_off,
                      dst_total_cap, (cudaStream_t)stream, lz4s ? &sc : nullptr);
+}
+
+// The asynchronous decode and Unwrap from page-locked host memory whose offsets src_off (n + 1 entries, device memory or
+// page-locked) are read on the device: the argument checks, each block's bound (a decode's compress_bound(dst_cap[i]), an
+// Unwrap packet's dst_cap[i] + 8, at most INT32_MAX), the capture refusal and the kinds of memory, then run_async.
+int lifted_async(lz4b200_ctx* c, Stage kind, Op op, const void* src, int64_t src_cap, const int64_t* src_off, void* dst,
+                 const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream, const char* what)
+{
+    const bool unwrap = kind == Stage::UNWRAP;
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (n < 0 || src_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n > 0 && (!src || !src_off || !dst || !dst_off || !dst_cap || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    LiftCall lc;
+    lc.src_cap = src_cap; lc.src_off = src_off; lc.bound.resize((size_t)n);
+    for (int32_t i = 0; i < n; i++) {
+        if (dst_cap[i] < 0) return fail(LZ4B200_E_ARG, std::string("negative ") + (unwrap ? "packet" : "block") + " capacity");
+        lc.bound[i] = unwrap ? (int32_t)std::min<int64_t>((int64_t)dst_cap[i] + WRAP_HEADER, INT32_MAX)
+                             : (int32_t)std::min<int64_t>((int64_t)dst_cap[i] + dst_cap[i] / 255 + 16, INT32_MAX);
+    }
+    CallGuard g(c); if (g.rc) return g.rc;
+    int rc = refuse_capture(stream, what, false); if (rc) return rc;
+    if (n == 0) return LZ4B200_OK;
+    void *at = nullptr, *off_at = nullptr, *len_at = nullptr;
+    rc = device_address(c, src, false, "src", &at); if (rc) return rc;
+    rc = device_address(c, src_off, true, "src_off", &off_at); if (rc) return rc;
+    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
+    rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc;
+    lc.src = (const uint8_t*)at;
+    // (src_off and out_len are copied at the caller's addresses, which the copy engines take for either kind)
+    return run_async(c, kind, op, (const uint8_t*)src, nullptr, nullptr, (uint8_t*)dst, dst_off, dst_cap, out_len, n, nullptr, 0,
+                     (cudaStream_t)stream, nullptr, &lc);
 }
 
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
@@ -1543,6 +1615,23 @@ int lz4b200_unwrap_batch_packed_to_device_async(lz4b200_ctx* c, const void* src,
 {
     return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, true, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
                         dst_total_cap, stream, "lz4b200_unwrap_batch_packed_to_device_async");
+}
+
+// The decode and the Unwrap whose offsets the device wrote (an asynchronous packed encode's or Wrap's out_off), staged by
+// the lift kernel (lz4_lift.cuh).
+int lz4b200_decode_batch_to_device_at_async(lz4b200_ctx* c, const void* src, int64_t src_cap, const int64_t* src_off, void* dst,
+                                            const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int known_len,
+                                            void* stream)
+{
+    return lifted_async(c, Stage::CODEC, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, src, src_cap, src_off, dst, dst_off, dst_cap,
+                        out_len, n, stream, "lz4b200_decode_batch_to_device_at_async");
+}
+
+int lz4b200_unwrap_batch_to_device_at_async(lz4b200_ctx* c, const void* src, int64_t src_cap, const int64_t* src_off, void* dst,
+                                            const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
+{
+    return lifted_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, src, src_cap, src_off, dst, dst_off, dst_cap, out_len, n, stream,
+                        "lz4b200_unwrap_batch_to_device_at_async");
 }
 
 // An LZ4Stream without blocking: the encode's chunk table is computed on the device and its frames land like the packed

@@ -59,6 +59,16 @@ size_t      compact_tmp_bytes(int32_t n_blocks);
 cudaError_t launch_land(const uint8_t* dense, const int64_t* dof, const int32_t* len, const int64_t* off, int32_t m,
                         int64_t dense_bytes, const int64_t* base_in, int64_t total_cap, uint8_t* dst, int64_t* out_off,
                         int32_t* out_len, int64_t* total_out, const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
+// One stage of the asynchronous decode or Unwrap from device-written offsets (lift.cu, lz4_lift.cuh): src is the device
+// address of page-locked host memory, of which src_cap bytes may be read; slot[0..m] the blocks' slots in io (slot_bytes =
+// slot[m], which sizes the launch); span[0..m] the stage's src_off, span[m+1] the batch's src_off[n]; bound[i] the most
+// bytes block i may span.  Writes so / sl (and dc = 0 for a rejected block) and the spans' bytes into io.
+// launch_lift_status, after the decode: out[i] = LZ4B200_E_ARG for a rejected block.
+cudaError_t launch_lift(const uint8_t* src, int64_t src_cap, const int64_t* slot, const int64_t* span, int32_t m, int64_t slot_bytes,
+                        const int32_t* bound, int64_t* so, int32_t* sl, int32_t* dc, uint8_t* io, const DeviceInfo& dev,
+                        cudaStream_t stream, int64_t* launches);
+cudaError_t launch_lift_status(int64_t src_cap, const int64_t* span, int32_t m, const int32_t* bound, int32_t* out, cudaStream_t stream,
+                               int64_t* launches);
 // Wrap / Unwrap packets in device memory (wrap.cu, lz4_wrap.cuh).  The scratch holds the codec's view of the batch: payload
 // offsets, lengths and capacities per packet, and the codec's per-packet results.
 struct WrapScratch { int64_t* off; int32_t* len; int32_t* cap; int32_t* res; };
