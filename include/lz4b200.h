@@ -274,6 +274,36 @@ int lz4b200_unwrap_batch_to_device_at_async(lz4b200_ctx* ctx, const void* src, i
                                             void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len,
                                             int32_t n, void* stream);
 
+/* stream_decode_to_device_at_async: lz4b200_stream_decode_to_device_async (below) with the stream's size read on the device.
+ * stream_encode_from_device_async writes the stream's size only on the device, and the host-walk decode needs it on the
+ * host, so the caller would have to wait for the encode.  Here src_size (one int64, device memory of the context's GPU or
+ * page-locked host memory) is read on the device when the call's work runs, and the chunk headers are walked there too:
+ * pass the encode's out_size as src_size and enqueue the whole round trip with no host wait,
+ *     stream_encode_from_device_async(x, n, B, hc, buf, stream_bound(n, B), d_size, s)
+ *     stream_decode_to_device_at_async(buf, stream_bound(n, B), d_size, B, y, n, d_out, s)
+ *   - src is page-locked host memory of which src_cap bytes may be read; block_size is the largest rawLen a chunk may have
+ *     (the chunk size the stream was written with); dst is device memory of the context's GPU, dst_cap its bytes.  src may
+ *     be null when src_cap == 0, dst when dst_cap == 0.  Any other null pointer, src_cap < 0, dst_cap < 0 or block_size
+ *     outside [1, INT32_MAX - 11] returns LZ4B200_E_ARG and enqueues nothing.
+ *   - Let S = *src_size and K = ceil(dst_cap / block_size), the chunk count of a stream of dst_cap bytes at block_size.  S < 0
+ *     or S > src_cap: *out_size = LZ4B200_E_ARG, nothing of src is read and dst is not written.  Otherwise the chunks of
+ *     src[0, S) are walked in order with exactly the rules of the host walk; the first of these ends it: a malformed header
+ *     (LZ4B200_E_FORMAT), a chunk with rawLen > block_size, a (K+1)-th chunk (empty chunks count), or a chunk whose output
+ *     would end past dst_cap (each LZ4B200_E_ARG).  Else *out_size = LZ4B200_E_FORMAT when a compressed chunk does not
+ *     decode from exactly its compLen bytes, and otherwise the decoded size T, with dst[0, T) what
+ *     lz4b200_stream_decode_to_device writes for src[0, S).
+ *   - So for every well-formed stream whose chunks keep the three bounds, and for a malformed one whose chunks before the
+ *     first malformed header keep them, *out_size equals what lz4b200_stream_decode_to_device(src, S, dst, dst_cap)
+ *     returns.  The bounds are where the two differ, as the block calls' span bound above: the host sizes the stages'
+ *     buffers before the device has seen a header.
+ *   - Nothing outside [dst, dst + dst_cap) is written; after a failure the bytes inside it are unspecified.  Nothing outside
+ *     [src, src + S) is read, except the rest of an aligned 16-byte unit that overlaps it.
+ *   - The rest is the contract of the asynchronous calls.  The call holds no per-chunk host metadata; its device work
+ *     grows with K, since the host cuts the stages before the size is known. */
+int lz4b200_stream_decode_to_device_at_async(lz4b200_ctx* ctx, const void* src, int64_t src_cap, const int64_t* src_size,
+                                             int32_t block_size, void* dst, int64_t dst_cap, int64_t* out_size,
+                                             void* stream);
+
 /* Compaction of fixed-stride encoder slots into one contiguous payload (device memory only): the batched form of
  * the Buffer.BlockCopy trim in LZ4Codec.Encode (src/LZ4/LZ4Codec.cs:357-364).  out_off[i] (int64, n_blocks+1
  * entries) = exclusive prefix sum of max(len[i],0); block i's bytes are copied to packed + out_off[i]. */
@@ -306,9 +336,9 @@ int lz4b200_compact(lz4b200_ctx* ctx, const void* slots, const int64_t* slot_off
  * lz4b200_encode_batch_packed_from_device_async, decode_batch_to_device_async, decode_batch_packed_to_device_async,
  * wrap_batch_packed_from_device_async, unwrap_batch_to_device_async, unwrap_batch_packed_to_device_async,
  * decode_batch_to_device_at_async, unwrap_batch_to_device_at_async,
- * stream_encode_from_device_async and stream_decode_to_device_async -- which do not synchronise but share the context's
- * stage buffers between eager calls and, all but the stream encode, hand the device host metadata that a graph would have
- * to keep alive.  lz4b200_peer_copy is not covered.
+ * stream_encode_from_device_async, stream_decode_to_device_async and stream_decode_to_device_at_async -- which do not
+ * synchronise but share the context's stage buffers between eager calls and, all but the stream encode and the stream
+ * decode from a device-read size, hand the device host metadata that a graph would have to keep alive.  lz4b200_peer_copy is not covered.
  * The calls without a stream (host-memory batches, single-block functions, lz4b200_synchronize, lz4b200_reserve) use
  * the legacy default stream or synchronise the device: they must not be made while any thread of the process captures
  * in cudaStreamCaptureModeGlobal.

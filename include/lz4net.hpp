@@ -156,6 +156,15 @@ public:
         if (lz4b200_stream_decode_to_device_async(h_, src, n, dst, dst_cap, out_size, stream) != LZ4B200_OK)
             throw std::runtime_error(lz4b200_last_error());
     }
+    // The decode from the size the device wrote (lz4b200_stream_decode_to_device_at_async): src_size (device or page-locked
+    // memory) is read and the headers are walked on the device, so the out_size of stream_encode_to_host_async above can be
+    // passed straight in; only src_cap bytes of src are read, and block_size is the chunk size the stream was written with.
+    void stream_decode_from_host_at_async(const void* src, int64_t src_cap, const int64_t* src_size, int32_t block_size, void* dst,
+                                          int64_t dst_cap, int64_t* out_size, void* stream)
+    {
+        if (lz4b200_stream_decode_to_device_at_async(h_, src, src_cap, src_size, block_size, dst, dst_cap, out_size, stream) != LZ4B200_OK)
+            throw std::runtime_error(lz4b200_last_error());
+    }
 private:
     lz4b200_ctx* h_ = nullptr;
 };

@@ -35,8 +35,9 @@ wrap_to_host_packed_async, unwrap_to_device_async and unwrap_to_device_packed_as
 for Wrap packets, which carry their own sizes and never exceed input + 8 bytes.  decode_from_host_at_async and
 unwrap_to_device_at_async bring such an offload back from the out_off the device wrote, with no synchronisation in
 between.  stream_encode_to_host_async and
-stream_decode_to_device_async do it for an LZ4Stream: one byte string, one pointer and one length, that any LZ4Stream reads.
-They refuse a capturing stream.
+stream_decode_to_device_async do it for an LZ4Stream: one byte string, one pointer and one length, that any LZ4Stream reads;
+stream_decode_to_device_at_async brings such a stream back from the size the device wrote, with no synchronisation in
+between.  They refuse a capturing stream.
 """
 from __future__ import annotations
 
@@ -357,6 +358,25 @@ def stream_decode_to_device_async(ctx: Context, wire: torch.Tensor, n: int, out:
     o = _flat_bytes(out)
     native.check(native.lib().lz4b200_stream_decode_to_device_async(
         ctx.handle, w, n, o.data_ptr(), o.numel(), size, _stream_of(stream)), "stream_decode_to_device_async")
+
+
+def stream_decode_to_device_at_async(ctx: Context, wire: torch.Tensor, src_cap: int, src_size: torch.Tensor, out: torch.Tensor,
+                                     out_size: torch.Tensor, block_size: int = 1 << 20, stream=None):
+    """stream_decode_to_device_async whose stream size is read on the device, when the call's work runs
+    (lz4b200_stream_decode_to_device_at_async): src_size (int64[1]) is a CUDA or page-locked CPU tensor -- the out_size a
+    stream_encode_to_host_async has just written, for one -- so the round trip needs no synchronisation in between.  The
+    headers are walked on the device; only the first src_cap bytes of wire (page-locked) are read.  block_size is the chunk
+    size the stream was written with.  out_size (int64[1], CUDA or page-locked) is set to the decoded size, or to
+    LZ4B200_E_ARG (a size outside [0, src_cap], a chunk above block_size, more chunks or bytes than out holds) or
+    LZ4B200_E_FORMAT (a malformed header, a chunk that does not decode)."""
+    w = _pinned(wire, torch.uint8, 0, "wire")
+    if not 0 <= src_cap <= wire.numel():
+        raise ValueError(f"src_cap: {src_cap} is not within the {wire.numel()} bytes of wire")
+    size, res = _pinned(src_size, torch.int64, 1, "src_size", True), _pinned(out_size, torch.int64, 1, "out_size", True)
+    o = _flat_bytes(out)
+    native.check(native.lib().lz4b200_stream_decode_to_device_at_async(
+        ctx.handle, w, src_cap, size, block_size, o.data_ptr(), o.numel(), res, _stream_of(stream)),
+        "stream_decode_to_device_at_async")
 
 
 def wrap_to_host(ctx: Context, raw: torch.Tensor, src_off, src_len, dst: np.ndarray, dst_off, dst_cap, out_len, hc: bool = False):

@@ -269,7 +269,8 @@ struct lz4b200_ctx {
     cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
     int64_t* carry = nullptr;              // the running output offset behind each slot's stage: NSLOT cells for the packed decode into device
                                            // memory, then NASYNC for the asynchronous packed encode, then one more cell
-                                           // whose int is the asynchronous LZ4Stream decode's failure flag (stream_failed)
+                                           // whose int is the asynchronous LZ4Stream decode's failure flag (stream_failed),
+                                           // then STREAM_WALK_CELLS per asynchronous slot for the device header walk (walk_carry)
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
     bool decode_lanes_auto = true;         // host-memory batches: chosen per chunk from the compression ratio
     int encode_ctas_per_sm = 0;            // encoder warps (= blocks in flight) per SM: 0 = as many as shared memory holds tables for (14)
@@ -294,6 +295,7 @@ struct lz4b200_ctx {
     }
     int pinned_lanes() const { return decode_lanes_auto ? 0 : decode_lanes; }   // 0: the decoder is picked on the device
     int* stream_failed() const { return (int*)(carry + NSLOT + NASYNC); }       // serialised through async_done
+    int64_t* walk_carry(int s) const { return carry + NSLOT + NASYNC + 1 + STREAM_WALK_CELLS * s; }
 };
 
 namespace {
@@ -881,6 +883,17 @@ StageSpan fill_lift(const Meta& h, int32_t b0, int32_t b1, const int32_t* bound,
     return sp;
 }
 
+// The LZ4Stream decode from a size the device wrote (lz4_stream.cuh stream_walk_stage): src's device address, the bytes
+// of it that may be read, where S is, the chunk size, the output's capacity, and the stage plan, which is arithmetic: K =
+// ceil(dst_cap / block_size) chunk slots, `per` a stage, each stage's span at most stage_cap bytes.
+struct WalkCall {
+    const uint8_t* src = nullptr; int64_t src_cap = 0; const int64_t* src_size = nullptr;
+    int32_t block_size = 0; int64_t dst_cap = 0; int64_t chunks = 0, per = 0, stage_cap = 0;
+};
+// A walk stage's device scratch, in AsyncSlot::offs: the lift descriptor the walk writes (STREAM_WALK_LIFT_I64 int64, then
+// the int32 bound), then the lift's entry for its one block (so, then sl and dc).
+constexpr size_t WALK_OFFS_BYTES = sizeof(int64_t) * (STREAM_WALK_LIFT_I64 + 3);
+
 // The LZ4Stream calls run the pipeline over at most this many chunks at a time: it bounds the host metadata by chunk
 // count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.  An asynchronous
 // encode stage takes at most this many chunks, which bounds its device metadata the same way.
@@ -915,13 +928,19 @@ constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
 //    set the context's failure flag (stream_failed) when a compressed chunk does not decode from exactly its compLen bytes,
 //    and one thread on `caller` behind the join writes out_off[0] = the decoded size, or LZ4B200_E_FORMAT.  The flag is
 //    cleared behind the context's previous asynchronous call and read before the next one (async_done).
+//    An LZ4Stream decode from a size the device wrote (wc) has no host entries: its stages are cut arithmetically (WalkCall),
+//    and each stage's walk (lz4_stream.cuh stream_walk_stage, one warp, behind the previous stage's walk only: `carried`)
+//    writes its entries and its span, which the lift kernel stages as one block; the decode is then FRAMED_DECODE's, its
+//    decoder picked on the device.  One thread on `caller` behind the join writes out_off[0] from the last stage's walk
+//    carry cells and the failure flag (stream_walk_result).
 // Calls are chained through async_done; the call's metadata block is taken again once the caller's stream has passed it.
 int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
               const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
-              int64_t dst_total_cap, cudaStream_t caller, const StreamCall* sc = nullptr, const LiftCall* lc = nullptr)
+              int64_t dst_total_cap, cudaStream_t caller, const StreamCall* sc = nullptr, const LiftCall* lc = nullptr,
+              const WalkCall* wc = nullptr)
 {
     const bool enc = is_encode(op), placed = kind == Stage::PLACED_DECODE || (kind == Stage::UNWRAP && !dst_off);
-    const bool cut = kind == Stage::STREAM_ENCODE, framed = kind == Stage::FRAMED_DECODE, lift = lc != nullptr;
+    const bool cut = kind == Stage::STREAM_ENCODE, framed = kind == Stage::FRAMED_DECODE, lift = lc != nullptr, walk = wc != nullptr;
     // blocks [b0, b1) of the batch, their host metadata at `at` in the call's block; an LZ4Stream encode stage's chunks are
     // [first + b0, first + b1) of the stream, b0 = 0
     struct Plan { int32_t b0, b1; size_t at; StageSpan sp; int64_t first; };
@@ -935,6 +954,13 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
             StageSpan sp;
             sp.dsum = std::min((int64_t)m * bs, sc->n - k0 * bs);
             plan.push_back(Plan{0, m, 0, sp, k0});
+        }
+    } else if (walk) {
+        // at least one stage, which checks S (and, with no slots, that the stream is empty)
+        for (int64_t k0 = 0; k0 == 0 || k0 < wc->chunks; k0 += wc->per) {
+            StageSpan sp;
+            sp.shi = lift_slot_bytes((int32_t)wc->stage_cap);
+            plan.push_back(Plan{0, (int32_t)std::min(wc->per, wc->chunks - k0), 0, sp, k0});
         }
     } else {
         for (int32_t b0 = 0; b0 < n;) {
@@ -951,7 +977,7 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
         Plan& p = plan[k];
         const int32_t m = p.b1 - p.b0;
         if (lift) p.sp = fill_lift(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, lc->bound.data(), dst_off, dst_cap);
-        else if (!cut)
+        else if (!cut && !walk)
             p.sp = fill_stage(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, src_off, src_len, dst_off, dst_cap, enc, !enc, false,
                               placed, framed ? sc->stored : nullptr);
         Sizes& nd = need[k % NASYNC];
@@ -960,6 +986,7 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
         nd.meta = std::max(nd.meta, async_meta_bytes(m));
         if (enc || placed) { nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(m + 1)); nd.scan = std::max(nd.scan, compact_tmp_bytes(m)); }
         if (lift) nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(2 * m + 3));      // slot[0..m] | span[0..m+1]
+        if (walk) nd.offs = std::max(nd.offs, WALK_OFFS_BYTES);
     }
     // growth: an earlier call may still be using the buffers
     bool grow = false;
@@ -1000,6 +1027,22 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
                 int rc = launched(launch_stream_cut(p.first, m, sc->block_size, sc->n, d.so, d.sl, d.dof, d.dc, sl.stream, &c->launches),
                                   "stream chunk table launch");
                 if (rc) return rc;
+            } else if (walk) {
+                // behind the previous stage's walk only; the next stage's walk follows this one, not its lift or decode
+                if (k > 0) CU(cudaStreamWaitEvent(sl.stream, c->aslot[prev].carried, 0));
+                int64_t* desc = (int64_t*)sl.offs.p;
+                const StreamWalkStage w{wc->src, wc->src_cap, k == 0 ? wc->src_size : nullptr, k > 0 ? c->walk_carry(prev) : nullptr,
+                                        c->walk_carry(s), wc->block_size, wc->dst_cap, m, k + 1 == plan.size(), wc->stage_cap,
+                                        d.so, d.dof, d.sl, d.dc, d.aux, desc};
+                int rc = launched(launch_stream_walk(w, sl.stream, &c->launches), "stream walk launch"); if (rc) return rc;
+                CU(cudaEventRecord(sl.carried, sl.stream));
+                if (m == 0) continue;
+                // the stage's span, as the lift's one block
+                int32_t* lifted = (int32_t*)(desc + STREAM_WALK_LIFT_I64 + 2);
+                rc = launched(launch_lift(wc->src, wc->src_cap, desc, desc + 2, 1, p.sp.shi, (const int32_t*)(desc + STREAM_WALK_LIFT_I64),
+                                          desc + STREAM_WALK_LIFT_I64 + 1, lifted, lifted + 1, (uint8_t*)sl.io.p, c->dev, sl.stream,
+                                          &c->launches), "stream lift launch");
+                if (rc) return rc;
             } else {
                 // up: the four arrays the kernels read, and a framed decode's stored lengths or a lift stage's bounds
                 const Meta h((uint8_t*)blk->buf.p + p.at, m);
@@ -1018,7 +1061,7 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
                 int rc = launched(launch_lift(lc->src, lc->src_cap, offs, span, m, p.sp.shi, d.aux, d.so, d.sl, d.dc, (uint8_t*)sl.io.p,
                                               c->dev, sl.stream, &c->launches), "lift launch");
                 if (rc) return rc;
-            } else if (!enc && sbytes) {
+            } else if (!enc && !walk && sbytes) {
                 CU(cudaMemcpyAsync(sl.io.p, src + p.sp.slo, sbytes, cudaMemcpyHostToDevice, sl.stream));
             }
             // (a packed Unwrap's prep reads no capacity: the placement writes the decode's into d.dc)
@@ -1028,7 +1071,7 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
             const Placement pl{offs, sl.scan.p, sl.scan.cap, dst_total_cap, 0, d.dc, async_fits(sl.meta.p, m),
                                k > 0 ? c->aslot[prev].carried : nullptr, k > 0 ? carry + prev : nullptr, d.dof, carry + s, sl.carried};
             const int32_t hc_large = cut ? (op == Op::ENCODE_HC && sc->block_size > 65536 ? m : 0) : stage_hc_large(op, src_len, p.b0, p.b1);
-            int rc = run_stage(c, kind, op, a, lift ? 0 : stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), hc_large,
+            int rc = run_stage(c, kind, op, a, lift || walk ? 0 : stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), hc_large,
                                wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), placed ? &pl : nullptr,
                                framed ? d.aux : nullptr, sl.stream);
             if (rc) return rc;
@@ -1075,7 +1118,10 @@ int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64
         if (all_in && cut)
             tail = launched(cudaMemcpyAsync(out_off, carry + (plan.size() - 1) % NASYNC, sizeof(int64_t), cudaMemcpyDefault, caller),
                             "stream size copy");
-        if (all_in && framed) tail = launched(launch_stream_result(failed, sc->total, out_off, caller, &c->launches), "stream result launch");
+        if (all_in && framed)
+            tail = launched(walk ? launch_stream_walk_result(failed, c->walk_carry((int)((plan.size() - 1) % NASYNC)), out_off, caller, &c->launches)
+                                 : launch_stream_result(failed, sc->total, out_off, caller, &c->launches),
+                            "stream result launch");
         CU(c->async_done.record(caller, Capture{}));
         if (blk) CU(cudaEventRecord(blk->done, caller));
         return tail;
@@ -1228,6 +1274,36 @@ int lifted_async(lz4b200_ctx* c, Stage kind, Op op, const void* src, int64_t src
     // (src_off and out_len are copied at the caller's addresses, which the copy engines take for either kind)
     return run_async(c, kind, op, (const uint8_t*)src, nullptr, nullptr, (uint8_t*)dst, dst_off, dst_cap, out_len, n, nullptr, 0,
                      (cudaStream_t)stream, nullptr, &lc);
+}
+
+// The asynchronous LZ4Stream decode from page-locked host memory whose size S (*src_size, device memory or page-locked) is
+// read on the device: the argument checks, the stage plan (WalkCall), the capture refusal and the kinds of memory, then
+// run_async with the walk in place of the host's.  src may be null when src_cap == 0, dst when dst_cap == 0.
+int walked_async(lz4b200_ctx* c, const void* src, int64_t src_cap, const int64_t* src_size, int32_t block_size, void* dst,
+                 int64_t dst_cap, int64_t* out_size, void* stream, const char* what)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (src_cap < 0 || dst_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    if (block_size < 1 || block_size > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "block_size: a chunk's frame must fit an int32");
+    if (!src_size || !out_size || (src_cap > 0 && !src) || (dst_cap > 0 && !dst)) return fail(LZ4B200_E_ARG, "null argument");
+    WalkCall wc;
+    wc.src_cap = src_cap; wc.block_size = block_size; wc.dst_cap = dst_cap;
+    wc.chunks = dst_cap / block_size + (dst_cap % block_size != 0);
+    // the asynchronous encode's stages, as long as a stage's span (a header may take STREAM_WALK_HEADER_MAX bytes) fits an int32
+    const int64_t frame = (int64_t)block_size + STREAM_WALK_HEADER_MAX;
+    CallGuard g(c); if (g.rc) return g.rc;
+    wc.per = std::max<int64_t>(1, std::min<int64_t>({(int64_t)c->host_chunk_bytes / block_size, STREAM_RUN_CHUNKS, INT32_MAX / frame}));
+    // (the chunks' payloads add up to at most dst_cap bytes, which bounds a stage's span for a small output)
+    wc.stage_cap = std::min<int64_t>({wc.per * frame, wc.per * STREAM_WALK_HEADER_MAX + dst_cap, INT32_MAX});
+    int rc = refuse_capture(stream, what, false); if (rc) return rc;
+    void *at = nullptr, *size_at = nullptr, *out_at = nullptr;
+    if (src) { rc = device_address(c, src, false, "src", &at); if (rc) return rc; }
+    rc = device_address(c, src_size, true, "src_size", &size_at); if (rc) return rc;
+    if (dst) { rc = check_side(c, dst, true, "dst"); if (rc) return rc; }
+    rc = device_address(c, out_size, true, "out_size", &out_at); if (rc) return rc;
+    wc.src = (const uint8_t*)at; wc.src_size = (const int64_t*)size_at;
+    return run_async(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, wc.src, nullptr, nullptr, (uint8_t*)dst, nullptr, nullptr, nullptr, 0,
+                     (int64_t*)out_at, dst_cap, (cudaStream_t)stream, nullptr, nullptr, &wc);
 }
 
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
@@ -1506,7 +1582,7 @@ int lz4b200_create(lz4b200_ctx** out, int device)
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device); c->dev.smem_per_sm = v;
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device); c->dev.smem_optin = v;
     cudaError_t e = cudaMalloc(&c->counters, sizeof(uint32_t) * (NCOUNTER + 4 * NCAPTURED));
-    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * (NSLOT + NASYNC + 1));
+    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * (NSLOT + NASYNC + 1 + STREAM_WALK_CELLS * NASYNC));
     for (Chain* ch : {&c->hc_done, &c->compact_done, &c->async_done}) {
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->done, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->inner, cudaEventDisableTiming);
@@ -1653,6 +1729,14 @@ int lz4b200_stream_decode_to_device_async(lz4b200_ctx* c, const void* src, int64
     if (!c || n < 0 || (n > 0 && !src) || !out_size) return fail(LZ4B200_E_ARG, "bad argument");
     return staged_async(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, true, src, nullptr, nullptr, dst, nullptr, nullptr, nullptr, 0,
                         out_size, dst_cap, stream, "lz4b200_stream_decode_to_device_async", n);
+}
+
+// The LZ4Stream decode whose size the device wrote (an asynchronous encode's out_size): its headers are walked on the
+// device (lz4_stream.cuh stream_walk_stage) and each stage's span is staged by the lift kernel (lz4_lift.cuh).
+int lz4b200_stream_decode_to_device_at_async(lz4b200_ctx* c, const void* src, int64_t src_cap, const int64_t* src_size,
+                                             int32_t block_size, void* dst, int64_t dst_cap, int64_t* out_size, void* stream)
+{
+    return walked_async(c, src, src_cap, src_size, block_size, dst, dst_cap, out_size, stream, "lz4b200_stream_decode_to_device_at_async");
 }
 
 // ---- LZ4Stream (lz4_stream.cuh): the host pipeline, the frames written on the device ----------------------------------

@@ -97,6 +97,12 @@ cudaError_t launch_stream_cut(int64_t first, int32_t m, int32_t block_size, int6
 cudaError_t launch_stream_status(const int32_t* comp_len, const int32_t* stored, const int32_t* res, int32_t m, int* failed,
                                  cudaStream_t stream, int64_t* launches);
 cudaError_t launch_stream_result(const int* failed, int64_t total, int64_t* out_size, cudaStream_t stream, int64_t* launches);
+// The decode from a size the device wrote (lz4_stream.cuh stream_walk_stage): launch_stream_walk, one warp, walks one
+// stage's headers and writes its entries, lift descriptor and carry cells; launch_stream_walk_result, one thread: *out_size
+// from the last stage's carry cells and *failed (stream_walk_result).
+struct StreamWalkStage;
+cudaError_t launch_stream_walk(const StreamWalkStage& w, cudaStream_t stream, int64_t* launches);
+cudaError_t launch_stream_walk_result(const int* failed, const int64_t* carry, int64_t* out_size, cudaStream_t stream, int64_t* launches);
 cudaError_t launch_synth(uint8_t* dst, int64_t n_blocks, int32_t block_size, int cls, uint64_t seed, int64_t first_block,
                          const DeviceInfo& dev, cudaStream_t stream, int64_t* launches);
 

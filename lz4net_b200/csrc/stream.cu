@@ -58,6 +58,17 @@ __global__ void lz4_stream_result_kernel(const int* failed, int64_t total, int64
     *out_size = *failed ? (int64_t)LZ4B200_E_FORMAT : total;
 }
 
+// One warp walks a stage's headers: the walk is a chain of dependent reads of host memory.
+__global__ void __launch_bounds__(32) lz4_stream_walk_kernel(const StreamWalkStage w)
+{
+    stream_walk_stage(w, (int)threadIdx.x);
+}
+
+__global__ void lz4_stream_walk_result_kernel(const int* failed, const int64_t* carry, int64_t* out_size)
+{
+    *out_size = stream_walk_result(carry, *failed);
+}
+
 cudaError_t launch_stream_cut(int64_t first, int32_t m, int32_t block_size, int64_t n, int64_t* so, int32_t* len, int64_t* dof,
                               int32_t* cap, cudaStream_t stream, int64_t* launches)
 {
@@ -79,6 +90,20 @@ cudaError_t launch_stream_status(const int32_t* comp_len, const int32_t* stored,
 cudaError_t launch_stream_result(const int* failed, int64_t total, int64_t* out_size, cudaStream_t stream, int64_t* launches)
 {
     lz4_stream_result_kernel<<<1, 1, 0, stream>>>(failed, total, out_size);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_stream_walk(const StreamWalkStage& w, cudaStream_t stream, int64_t* launches)
+{
+    lz4_stream_walk_kernel<<<1, 32, 0, stream>>>(w);
+    if (launches) ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_stream_walk_result(const int* failed, const int64_t* carry, int64_t* out_size, cudaStream_t stream, int64_t* launches)
+{
+    lz4_stream_walk_result_kernel<<<1, 1, 0, stream>>>(failed, carry, out_size);
     if (launches) ++*launches;
     return cudaGetLastError();
 }

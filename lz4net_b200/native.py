@@ -37,6 +37,7 @@ SIGNATURES = {
     "lz4b200_unwrap_batch_packed_to_device_async": (_I, [_P, _P, _P, _P, _P, _L, _P, _P, C.c_int32, _P]),
     "lz4b200_decode_batch_to_device_at_async": (_I, [_P, _P, _L, _P, _P, _P, _P, _P, C.c_int32, _I, _P]),
     "lz4b200_unwrap_batch_to_device_at_async": (_I, [_P, _P, _L, _P, _P, _P, _P, _P, C.c_int32, _P]),
+    "lz4b200_stream_decode_to_device_at_async": (_I, [_P, _P, _L, _P, C.c_int32, _P, _L, _P, _P]),
     "lz4b200_compact": (_I, [_P, _P, _P, _P, _P, _P, C.c_int32, _P]),
     "lz4b200_reserve": (_I, [_P, C.c_int32, _I]),
     "lz4b200_measure_batch": (_I, [_P, _P, _P, _P, _P, _P, C.c_int32, _I, _I, _P]),
