@@ -9,12 +9,14 @@
 // so does the packed unknown-size decode from host into device memory, whose output offset is carried across the stages
 // on the device (Placement, lz4_packed.cuh).  What a stage runs is named by its caller (Stage) and mapped to its sequence
 // in one place (run_stage); the codec operation is named by Op.
-// The asynchronous calls between device memory and page-locked host memory (run_async: the packed encode, Wrap and
-// LZ4Stream encode into it, the decode, packed decode, Unwrap and LZ4Stream decode from it, checked by landed_async and
-// staged_async) cut their stages by the same plan, run the same stage sequences on streams and buffers of their own and
-// return without waiting; the packed encodes' stages land in host memory from a kernel (lz4_land.cuh), since where a stage
-// lands is known only on the device, the Unwraps read their headers on the device (run_unwrap), and the LZ4Stream encode
-// computes its chunk tables on the device.
+// The asynchronous calls between device memory and page-locked host memory (the packed encode, Wrap and LZ4Stream encode
+// into it, the decode, packed decode, Unwrap and LZ4Stream decode from it, and the decode, Unwrap and LZ4Stream decode
+// from offsets or a size the device wrote) are each one AsyncCall, which names where its stages' blocks come from
+// (Source); after its own argument checks each enters through enter_async, and run_async cuts its stages by the same plan
+// (or arithmetically, by chunks), runs the same stage sequences on streams and buffers of their own and returns without
+// waiting.  A stage is arrival (by source), its kind's sequence (run_stage) and departure (by kind): the packed encodes'
+// stages land in host memory from a kernel (lz4_land.cuh), since where a stage lands is known only on the device, the
+// Unwraps read their headers on the device (run_unwrap), and the LZ4Stream encode computes its chunk tables on the device.
 // The device-memory calls enter through one path (DeviceCall): each states what it takes from the context (Need), which
 // admits it to a CUDA graph capture or grows an eager call's scratch; lz4b200_reserve grows to the same needs.
 // The LZ4Stream frames and the Wrap headers are written on the device (lz4_stream.cuh, lz4_wrap.cuh) whichever side the
@@ -199,6 +201,10 @@ struct AsyncSlot : SlotBase {
     DevBuf io;                             // the encode's dense output slots, or the decode's staged source
     DevBuf frames;                         // an LZ4Stream encode's frames, back to back, before they land
 };
+// The context's device cells that carry state from one pipeline stage to the next: the running output offset behind each
+// slot's stage (run_host's packed decode into device memory, run_async's packed stages), the asynchronous LZ4Stream
+// decode's failure flag, each asynchronous slot's device header walk.  The asynchronous cells are serialised by async_done.
+struct Carry { int64_t host[NSLOT], async[NASYNC]; int failed; int64_t walk[NASYNC][STREAM_WALK_CELLS]; };
 // The page-locked metadata of one asynchronous call, which the device reads after the call has returned: taken again once
 // `done`, recorded behind the call, has fired.
 struct MetaBlock { PinBuf buf; cudaEvent_t done = nullptr; bool used = false; };
@@ -225,6 +231,10 @@ WrapScratch wrap_scratch_at(void* p, int32_t n)
 constexpr size_t META_BYTES = 32, WRAP_META_OFFSET = 32, WRAP_META_BYTES = WRAP_META_OFFSET + WRAP_SCRATCH_BYTES;
 // An asynchronous stage's device block (AsyncSlot::meta) holds every kind's: the arrays, a Wrap's or an Unwrap's
 // WrapScratch at WRAP_META_OFFSET * m, then a packed form's "fits" flag (async_fits).
+// The packet view (WrapScratch) of a stage of m blocks in its device block.
+WrapScratch packet_view(void* meta, int32_t m) { return wrap_scratch_at((uint8_t*)meta + WRAP_META_OFFSET * (size_t)m, m); }
+// The bytes of a stage's Meta h copied up: the four arrays the kernels read, and aux (stored lengths, lift bounds).
+size_t meta_up_bytes(const Meta& h, bool aux) { return (size_t)((uint8_t*)(aux ? h.out : h.aux) - (uint8_t*)h.so); }
 size_t async_meta_bytes(int32_t m) { return (size_t)m * WRAP_META_BYTES + sizeof(int64_t); }
 int* async_fits(void* meta, int32_t m) { return (int*)((uint8_t*)meta + (size_t)m * WRAP_META_BYTES); }
 
@@ -267,10 +277,7 @@ struct lz4b200_ctx {
     Chain compact_done;                    // likewise compact_tmp, packed_caps and wrap_tmp (DeviceCall)
     Chain async_done;                      // likewise the asynchronous calls' stage buffers, carry cells and streams (run_async)
     cudaEvent_t entry = nullptr;           // mixed-memory batches: recorded on the caller's stream, waited on by every slot
-    int64_t* carry = nullptr;              // the running output offset behind each slot's stage: NSLOT cells for the packed decode into device
-                                           // memory, then NASYNC for the asynchronous packed encode, then one more cell
-                                           // whose int is the asynchronous LZ4Stream decode's failure flag (stream_failed),
-                                           // then STREAM_WALK_CELLS per asynchronous slot for the device header walk (walk_carry)
+    Carry* carry = nullptr;                // device memory
     int decode_lanes = 16;                 // lanes per block for device-memory batches (+100 = output-staged variant)
     bool decode_lanes_auto = true;         // host-memory batches: chosen per chunk from the compression ratio
     int encode_ctas_per_sm = 0;            // encoder warps (= blocks in flight) per SM: 0 = as many as shared memory holds tables for (14)
@@ -294,8 +301,6 @@ struct lz4b200_ctx {
         uint32_t* c = counters + next_counter; next_counter = (next_counter + 4) % NCOUNTER; return c;
     }
     int pinned_lanes() const { return decode_lanes_auto ? 0 : decode_lanes; }   // 0: the decoder is picked on the device
-    int* stream_failed() const { return (int*)(carry + NSLOT + NASYNC); }       // serialised through async_done
-    int64_t* walk_carry(int s) const { return carry + NSLOT + NASYNC + 1 + STREAM_WALK_CELLS * s; }
 };
 
 namespace {
@@ -484,6 +489,14 @@ cudaError_t place(lz4b200_ctx* c, const int32_t* size, int32_t n, const Placemen
         e = launch_packed_prep(size, p.off, n, p.total_cap, p.room, p.caps, p.fits, st, &c->launches, p.base, p.abs_off, p.total);
     if (e == cudaSuccess && p.placed) e = cudaEventRecord(p.placed, st);
     return e;
+}
+
+// A pipeline stage's placement on slot sl (metadata d), behind the previous stage's (prev: its slot and the carry cell
+// `base` it leaves; none for the first stage); it leaves its running total in `total` and records sl's `carried`.
+Placement chained_placement(SlotBase& sl, const Meta& d, int* fits, int64_t total_cap, const SlotBase* prev, const int64_t* base, int64_t* total)
+{
+    return Placement{(int64_t*)sl.offs.p, sl.scan.p, sl.scan.cap, total_cap, 0, d.dc, fits, prev ? prev->carried : nullptr,
+                     prev ? base : nullptr, d.dof, total, sl.carried};
 }
 
 // An Unwrap of the packets of a (src / src_off / src_len; outputs at dst + dst_off, capacities dst_cap, null = no limit):
@@ -745,9 +758,7 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
         const size_t sbytes = (size_t)(sp.shi - slo);
         if (!src_dev) CU(sl.src.reserve(sbytes + 64));
         if (!dst_dev) CU(sl.dst.reserve((size_t)dsum + 64));
-        // up: the four arrays the kernels read, and a framed decode's stored lengths
-        const size_t up = (size_t)((uint8_t*)(framed ? h.out : h.aux) - (uint8_t*)h.so);
-        CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, up, cudaMemcpyHostToDevice, sl.stream));
+        CU(cudaMemcpyAsync(sl.meta.p, sl.hmeta.p, meta_up_bytes(h, framed), cudaMemcpyHostToDevice, sl.stream));
         if (sbytes) {
             const uint8_t* from = src + slo;
             if (src_pageable && m > 8) { CU(sl.hsrc.reserve(sbytes)); par_memcpy(sl.hsrc.p, from, sbytes); from = (const uint8_t*)sl.hsrc.p; }
@@ -759,16 +770,15 @@ int run_host(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_
             // behind the previous stage's placement; the stage's "fits" flag lives behind its arrays (Meta)
             CU(sl.offs.reserve(sizeof(int64_t) * (size_t)(m + 1))); CU(sl.scan.reserve(compact_tmp_bytes(m)));
             const int prev = (s + NSLOT - 1) % NSLOT;
-            pl = Placement{(int64_t*)sl.offs.p, sl.scan.p, sl.scan.cap, dst_total_cap, 0, d.dc, (int*)d.off,
-                           b0 > 0 ? c->slot[prev].carried : nullptr, b0 > 0 ? c->carry + prev : nullptr, d.dof, c->carry + s, sl.carried};
+            pl = chained_placement(sl, d, (int*)d.off, dst_total_cap, b0 > 0 ? &c->slot[prev] : nullptr, &c->carry->host[prev],
+                                   &c->carry->host[s]);
         }
         rc = run_stage(c, kind, op, a, stage_lanes(c, op, src_len, dst_cap, b0, b1), stage_hc_large(op, src_len, b0, b1),
-                       wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), placed ? &pl : nullptr, d.aux,
-                       sl.stream);
+                       packet_view(sl.meta.p, m), placed ? &pl : nullptr, d.aux, sl.stream);
         if (rc) return rc;
         if (placed) {
             CU(cudaMemcpyAsync(h.dof, d.dof, sizeof(int64_t) * (size_t)m, cudaMemcpyDeviceToHost, sl.stream));
-            CU(cudaMemcpyAsync(h.off, c->carry + s, sizeof(int64_t), cudaMemcpyDeviceToHost, sl.stream));
+            CU(cudaMemcpyAsync(h.off, &c->carry->host[s], sizeof(int64_t), cudaMemcpyDeviceToHost, sl.stream));
         }
         if (mode >= SCATTER) {
             // the outputs back to back: compacted, or an LZ4Stream encode's frames (sizes -> scan -> headers + payloads)
@@ -859,321 +869,10 @@ int take_meta(lz4b200_ctx* c, size_t bytes, MetaBlock** out)
     return LZ4B200_OK;
 }
 
-// The LZ4Stream calls' own part of an asynchronous call: the stream's length n and the encode's chunk size, from which its
-// stages and their chunk tables follow (STREAM_ENCODE); the decode's stored flags, one per entry, and its decoded size
-// (FRAMED_DECODE).
-struct StreamCall { int64_t n = 0; int32_t block_size = 0; const uint8_t* stored = nullptr; int64_t total = 0; };
-
-// The decodes and Unwraps whose block offsets exist only on the device (lz4_lift.cuh): src's device address and the bytes
-// of it that may be read, src_off (n + 1 entries, device memory or page-locked), and each block's bound, by which the
-// stages are cut and their slots sized.
-struct LiftCall { const uint8_t* src = nullptr; int64_t src_cap = 0; const int64_t* src_off = nullptr; std::vector<int32_t> bound; };
-
-// A lift stage's metadata: dst_off / dst_cap as the caller gave them, each block's slot (so[i], and its prefix in off[0..m])
-// and its bound (aux); the spans are written on the device.  sp.shi = the stage's staging bytes.
-StageSpan fill_lift(const Meta& h, int32_t b0, int32_t b1, const int32_t* bound, const int64_t* dst_off, const int32_t* dst_cap)
-{
-    StageSpan sp;
-    for (int32_t i = 0; i < b1 - b0; i++) {
-        h.off[i] = h.so[i] = sp.shi;
-        h.dof[i] = dst_off[b0 + i]; h.sl[i] = 0; h.dc[i] = dst_cap[b0 + i]; h.aux[i] = bound[b0 + i];
-        sp.shi += lift_slot_bytes(bound[b0 + i]);
-    }
-    h.off[b1 - b0] = sp.shi;
-    return sp;
-}
-
-// The LZ4Stream decode from a size the device wrote (lz4_stream.cuh stream_walk_stage): src's device address, the bytes
-// of it that may be read, where S is, the chunk size, the output's capacity, and the stage plan, which is arithmetic: K =
-// ceil(dst_cap / block_size) chunk slots, `per` a stage, each stage's span at most stage_cap bytes.
-struct WalkCall {
-    const uint8_t* src = nullptr; int64_t src_cap = 0; const int64_t* src_size = nullptr;
-    int32_t block_size = 0; int64_t dst_cap = 0; int64_t chunks = 0, per = 0, stage_cap = 0;
-};
-// A walk stage's device scratch, in AsyncSlot::offs: the lift descriptor the walk writes (STREAM_WALK_LIFT_I64 int64, then
-// the int32 bound), then the lift's entry for its one block (so, then sl and dc).
-constexpr size_t WALK_OFFS_BYTES = sizeof(int64_t) * (STREAM_WALK_LIFT_I64 + 3);
-
 // The LZ4Stream calls run the pipeline over at most this many chunks at a time: it bounds the host metadata by chunk
 // count (tiny blocks would otherwise need gigabytes of it), while a call covers many pipeline stages.  An asynchronous
 // encode stage takes at most this many chunks, which bounds its device metadata the same way.
 constexpr int64_t STREAM_RUN_CHUNKS = 1 << 20;
-
-// The stages of an asynchronous call, cut and described as run_host cuts and describes them (stage_end, fill_stage,
-// stage_lanes, stage_hc_large), enqueued on the context's NASYNC streams in turn, forked from `caller` and joined back to
-// it; nothing is waited on unless a buffer must grow.  What a stage runs is its kind's sequence (run_stage), as in run_host:
-//  - The packed encodes (enc: CODEC with an encode, WRAP_ENCODE): src is device memory, dst the device address of
-//    page-locked host memory, out_off / out_len device addresses.  A stage encodes (or wraps, run_wrap: capacity src_len + 8
-//    per packet, the stage weighed by it) into its dense slots (AsyncSlot::io), scans the lengths, and lands
-//    (lz4_land.cuh) behind the running total that the previous stage's landing step left in its carry cell, after the
-//    previous slot's `carried` event.
-//  - The LZ4Stream encode (STREAM_ENCODE, sc: the stream's length and chunk size) lands the same way, but its stages are
-//    cut arithmetically, as many chunks as host_chunk_bytes of input holds (at least one, at most STREAM_RUN_CHUNKS), and
-//    hold no host metadata: a stage's chunk table is computed on the device (lz4_stream.cuh stream_cut_one).  The stage
-//    encodes its chunks (capacity = the chunk's length), writes their frames back to back (write_frames, into
-//    AsyncSlot::frames) and lands the frames as its blocks.  Only the running total is kept: the last stage's goes to
-//    out_off[0], the stream's size, on `caller` behind the join.
-//  - The decodes into device memory (CODEC with a decode, UNWRAP, PLACED_DECODE, FRAMED_DECODE): src is page-locked host
-//    memory, copied up a stage at a time on the copy engine, weighed by src_len; the decoders write dst (device memory) in
-//    place.  A CODEC decode writes at dst_off; an UNWRAP reads the headers from the staged bytes on the device (run_unwrap),
-//    since work still queued on `caller` may write them.  The packed forms (placed: PLACED_DECODE, an UNWRAP without
-//    dst_off) measure (PLACED_DECODE) or prep (UNWRAP), scan and place their stage behind the previous one's from the same
-//    carry cells (place), then decode behind the stage's "fits" flag; their absolute offsets are copied to out_off, the
-//    last stage's running total to out_off[n].
-//    A decode or Unwrap from device-written offsets (lc) cuts its stages by the blocks' bounds, stages them with the lift
-//    kernel (lz4_lift.cuh) in place of the copy, and has its decoder picked on the device from the staged spans (the
-//    context's pinned choice, if any, still holds); after the decode, its rejected blocks' results become LZ4B200_E_ARG.
-//    The stage's results are copied to out_len (device or page-locked memory), except for an LZ4Stream decode
-//    (FRAMED_DECODE, sc: the stored flags and the decoded size), whose entries come from the host's header walk: its stages
-//    set the context's failure flag (stream_failed) when a compressed chunk does not decode from exactly its compLen bytes,
-//    and one thread on `caller` behind the join writes out_off[0] = the decoded size, or LZ4B200_E_FORMAT.  The flag is
-//    cleared behind the context's previous asynchronous call and read before the next one (async_done).
-//    An LZ4Stream decode from a size the device wrote (wc) has no host entries: its stages are cut arithmetically (WalkCall),
-//    and each stage's walk (lz4_stream.cuh stream_walk_stage, one warp, behind the previous stage's walk only: `carried`)
-//    writes its entries and its span, which the lift kernel stages as one block; the decode is then FRAMED_DECODE's, its
-//    decoder picked on the device.  One thread on `caller` behind the join writes out_off[0] from the last stage's walk
-//    carry cells and the failure flag (stream_walk_result).
-// Calls are chained through async_done; the call's metadata block is taken again once the caller's stream has passed it.
-int run_async(lz4b200_ctx* c, Stage kind, Op op, const uint8_t* src, const int64_t* src_off, const int32_t* src_len, uint8_t* dst,
-              const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
-              int64_t dst_total_cap, cudaStream_t caller, const StreamCall* sc = nullptr, const LiftCall* lc = nullptr,
-              const WalkCall* wc = nullptr)
-{
-    const bool enc = is_encode(op), placed = kind == Stage::PLACED_DECODE || (kind == Stage::UNWRAP && !dst_off);
-    const bool cut = kind == Stage::STREAM_ENCODE, framed = kind == Stage::FRAMED_DECODE, lift = lc != nullptr, walk = wc != nullptr;
-    // blocks [b0, b1) of the batch, their host metadata at `at` in the call's block; an LZ4Stream encode stage's chunks are
-    // [first + b0, first + b1) of the stream, b0 = 0
-    struct Plan { int32_t b0, b1; size_t at; StageSpan sp; int64_t first; };
-    std::vector<Plan> plan;
-    size_t bytes = 0;
-    if (cut) {
-        const int64_t bs = sc->block_size, chunks = (sc->n + bs - 1) / bs;
-        const int64_t per = std::max<int64_t>(1, std::min<int64_t>((int64_t)c->host_chunk_bytes / bs, STREAM_RUN_CHUNKS));
-        for (int64_t k0 = 0; k0 < chunks; k0 += per) {
-            const int32_t m = (int32_t)std::min(per, chunks - k0);
-            StageSpan sp;
-            sp.dsum = std::min((int64_t)m * bs, sc->n - k0 * bs);
-            plan.push_back(Plan{0, m, 0, sp, k0});
-        }
-    } else if (walk) {
-        // at least one stage, which checks S (and, with no slots, that the stream is empty)
-        for (int64_t k0 = 0; k0 == 0 || k0 < wc->chunks; k0 += wc->per) {
-            StageSpan sp;
-            sp.shi = lift_slot_bytes((int32_t)wc->stage_cap);
-            plan.push_back(Plan{0, (int32_t)std::min(wc->per, wc->chunks - k0), 0, sp, k0});
-        }
-    } else {
-        for (int32_t b0 = 0; b0 < n;) {
-            const int32_t b1 = stage_end(c, lift ? lc->bound.data() : src_len, enc ? dst_cap : nullptr, b0, n, !enc);
-            plan.push_back(Plan{b0, b1, bytes, {}, 0});
-            bytes += (meta_host_bytes(b1 - b0) + 15) & ~(size_t)15;
-            b0 = b1;
-        }
-    }
-    MetaBlock* blk = nullptr;
-    int rc = bytes ? take_meta(c, bytes, &blk) : LZ4B200_OK; if (rc) return rc;
-    struct Sizes { size_t io = 0, frames = 0, meta = 0, offs = 0, scan = 0; } need[NASYNC];      // each slot's buffers, for its largest stage
-    for (size_t k = 0; k < plan.size(); k++) {
-        Plan& p = plan[k];
-        const int32_t m = p.b1 - p.b0;
-        if (lift) p.sp = fill_lift(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, lc->bound.data(), dst_off, dst_cap);
-        else if (!cut && !walk)
-            p.sp = fill_stage(Meta((uint8_t*)blk->buf.p + p.at, m), p.b0, p.b1, src_off, src_len, dst_off, dst_cap, enc, !enc, false,
-                              placed, framed ? sc->stored : nullptr);
-        Sizes& nd = need[k % NASYNC];
-        nd.io = std::max(nd.io, (size_t)(enc ? p.sp.dsum : p.sp.shi - p.sp.slo) + 64);
-        if (cut) nd.frames = std::max(nd.frames, (size_t)p.sp.dsum + (size_t)m * STREAM_HEADER_MAX + 64);
-        nd.meta = std::max(nd.meta, async_meta_bytes(m));
-        if (enc || placed) { nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(m + 1)); nd.scan = std::max(nd.scan, compact_tmp_bytes(m)); }
-        if (lift) nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(2 * m + 3));      // slot[0..m] | span[0..m+1]
-        if (walk) nd.offs = std::max(nd.offs, WALK_OFFS_BYTES);
-    }
-    // growth: an earlier call may still be using the buffers
-    bool grow = false;
-    for (int s = 0; s < NASYNC; s++) {
-        const AsyncSlot& sl = c->aslot[s];
-        grow |= need[s].io > sl.io.cap || need[s].frames > sl.frames.cap || need[s].meta > sl.meta.cap || need[s].offs > sl.offs.cap ||
-                need[s].scan > sl.scan.cap;
-    }
-    if (grow) {
-        CU(cudaDeviceSynchronize());
-        for (int s = 0; s < NASYNC; s++) {
-            AsyncSlot& sl = c->aslot[s];
-            CU(sl.io.reserve(need[s].io)); CU(sl.frames.reserve(need[s].frames)); CU(sl.meta.reserve(need[s].meta));
-            CU(sl.offs.reserve(need[s].offs)); CU(sl.scan.reserve(need[s].scan));
-        }
-    }
-    const int used = (int)std::min<size_t>(plan.size(), NASYNC);
-    int64_t* carry = c->carry + NSLOT;
-    int* failed = c->stream_failed();
-    auto stages = [&]() -> int {
-        if (framed) {
-            // the failure flag, cleared behind the context's previous asynchronous call (which may still read it)
-            CU(c->async_done.wait(caller, Capture{}));
-            CU(cudaMemsetAsync(failed, 0, sizeof(int), caller));
-        }
-        CU(cudaEventRecord(c->entry, caller));
-        for (int s = 0; s < used; s++) {
-            CU(cudaStreamWaitEvent(c->aslot[s].stream, c->entry, 0));
-            CU(c->async_done.wait(c->aslot[s].stream, Capture{}));
-        }
-        for (size_t k = 0; k < plan.size(); k++) {
-            const Plan& p = plan[k];
-            const int s = (int)(k % NASYNC), prev = (s + NASYNC - 1) % NASYNC;
-            AsyncSlot& sl = c->aslot[s];
-            const int32_t m = p.b1 - p.b0;
-            const Meta d(sl.meta.p, m);
-            if (cut) {
-                int rc = launched(launch_stream_cut(p.first, m, sc->block_size, sc->n, d.so, d.sl, d.dof, d.dc, sl.stream, &c->launches),
-                                  "stream chunk table launch");
-                if (rc) return rc;
-            } else if (walk) {
-                // behind the previous stage's walk only; the next stage's walk follows this one, not its lift or decode
-                if (k > 0) CU(cudaStreamWaitEvent(sl.stream, c->aslot[prev].carried, 0));
-                int64_t* desc = (int64_t*)sl.offs.p;
-                const StreamWalkStage w{wc->src, wc->src_cap, k == 0 ? wc->src_size : nullptr, k > 0 ? c->walk_carry(prev) : nullptr,
-                                        c->walk_carry(s), wc->block_size, wc->dst_cap, m, k + 1 == plan.size(), wc->stage_cap,
-                                        d.so, d.dof, d.sl, d.dc, d.aux, desc};
-                int rc = launched(launch_stream_walk(w, sl.stream, &c->launches), "stream walk launch"); if (rc) return rc;
-                CU(cudaEventRecord(sl.carried, sl.stream));
-                if (m == 0) continue;
-                // the stage's span, as the lift's one block
-                int32_t* lifted = (int32_t*)(desc + STREAM_WALK_LIFT_I64 + 2);
-                rc = launched(launch_lift(wc->src, wc->src_cap, desc, desc + 2, 1, p.sp.shi, (const int32_t*)(desc + STREAM_WALK_LIFT_I64),
-                                          desc + STREAM_WALK_LIFT_I64 + 1, lifted, lifted + 1, (uint8_t*)sl.io.p, c->dev, sl.stream,
-                                          &c->launches), "stream lift launch");
-                if (rc) return rc;
-            } else {
-                // up: the four arrays the kernels read, and a framed decode's stored lengths or a lift stage's bounds
-                const Meta h((uint8_t*)blk->buf.p + p.at, m);
-                CU(cudaMemcpyAsync(sl.meta.p, h.so, (size_t)((uint8_t*)(framed || lift ? h.out : h.aux) - (uint8_t*)h.so),
-                                   cudaMemcpyHostToDevice, sl.stream));
-            }
-            const size_t sbytes = (size_t)(p.sp.shi - p.sp.slo);
-            int64_t* offs = (int64_t*)sl.offs.p;
-            int64_t* span = offs + m + 1;
-            if (lift) {
-                // the slots, then the stage's offsets and src_off[n], wherever the caller's src_off lives
-                CU(cudaMemcpyAsync(offs, Meta((uint8_t*)blk->buf.p + p.at, m).off, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyHostToDevice,
-                                   sl.stream));
-                CU(cudaMemcpyAsync(span, lc->src_off + p.b0, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDefault, sl.stream));
-                CU(cudaMemcpyAsync(span + m + 1, lc->src_off + n, sizeof(int64_t), cudaMemcpyDefault, sl.stream));
-                int rc = launched(launch_lift(lc->src, lc->src_cap, offs, span, m, p.sp.shi, d.aux, d.so, d.sl, d.dc, (uint8_t*)sl.io.p,
-                                              c->dev, sl.stream, &c->launches), "lift launch");
-                if (rc) return rc;
-            } else if (!enc && !walk && sbytes) {
-                CU(cudaMemcpyAsync(sl.io.p, src + p.sp.slo, sbytes, cudaMemcpyHostToDevice, sl.stream));
-            }
-            // (a packed Unwrap's prep reads no capacity: the placement writes the decode's into d.dc)
-            const BatchArgs a{enc ? src : (const uint8_t*)sl.io.p, d.so, d.sl, enc ? (uint8_t*)sl.io.p : dst, d.dof,
-                              kind == Stage::UNWRAP && placed ? nullptr : d.dc, d.out, m};
-            // a packed stage places behind the previous stage's placement (lz4_packed.cuh); the next one follows
-            const Placement pl{offs, sl.scan.p, sl.scan.cap, dst_total_cap, 0, d.dc, async_fits(sl.meta.p, m),
-                               k > 0 ? c->aslot[prev].carried : nullptr, k > 0 ? carry + prev : nullptr, d.dof, carry + s, sl.carried};
-            const int32_t hc_large = cut ? (op == Op::ENCODE_HC && sc->block_size > 65536 ? m : 0) : stage_hc_large(op, src_len, p.b0, p.b1);
-            int rc = run_stage(c, kind, op, a, lift || walk ? 0 : stage_lanes(c, op, src_len, dst_cap, p.b0, p.b1), hc_large,
-                               wrap_scratch_at((uint8_t*)sl.meta.p + WRAP_META_OFFSET * (size_t)m, m), placed ? &pl : nullptr,
-                               framed ? d.aux : nullptr, sl.stream);
-            if (rc) return rc;
-            if (lift) {
-                rc = launched(launch_lift_status(lc->src_cap, span, m, d.aux, d.out, sl.stream, &c->launches), "lift status launch");
-                if (rc) return rc;
-            }
-            if (framed) {
-                rc = launched(launch_stream_status(d.sl, d.aux, d.out, m, failed, sl.stream, &c->launches), "stream status launch");
-                if (rc) return rc;
-                continue;
-            }
-            if (!enc) {
-                CU(cudaMemcpyAsync(out_len + p.b0, d.out, sizeof(int32_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
-                if (placed) {
-                    CU(cudaMemcpyAsync(out_off + p.b0, d.dof, sizeof(int64_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
-                    if (p.b1 == n) CU(cudaMemcpyAsync(out_off + n, carry + s, sizeof(int64_t), cudaMemcpyDefault, sl.stream));
-                }
-                continue;
-            }
-            // what lands: the compacted blocks, or an LZ4Stream stage's frames (dense = the frames, at their scan, of their sizes)
-            const uint8_t* frames = (const uint8_t*)sl.frames.p;
-            cudaError_t e = cut ? write_frames(c, a, op == Op::ENCODE_HC, d.aux, offs, sl.scan.p, sl.scan.cap, (uint8_t*)frames, sl.stream)
-                                : launch_compact(nullptr, nullptr, d.out, nullptr, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches);
-            if (e == cudaSuccess && k > 0) e = cudaStreamWaitEvent(sl.stream, c->aslot[prev].carried, 0);
-            if (e == cudaSuccess)
-                e = cut ? launch_land(frames, offs, d.aux, offs, m, p.sp.dsum + (int64_t)m * STREAM_HEADER_MAX, k > 0 ? carry + prev : nullptr,
-                                      dst_total_cap, dst, nullptr, nullptr, carry + s, c->dev, sl.stream, &c->launches)
-                        : launch_land((const uint8_t*)sl.io.p, d.dof, d.out, offs, m, p.sp.dsum, k > 0 ? carry + prev : nullptr,
-                                      dst_total_cap, dst, out_off + p.b0, out_len + p.b0, carry + s, c->dev, sl.stream, &c->launches);
-            if (e != cudaSuccess) return cuda_fail(e, "scan / landing launch");
-            CU(cudaEventRecord(sl.carried, sl.stream));
-        }
-        return LZ4B200_OK;
-    };
-    // whatever was enqueued, the caller's stream joins it, and the chain and the metadata block are recorded behind it; an
-    // LZ4Stream call whose stages are all in writes its size or status in between
-    auto join = [&](bool all_in) -> int {
-        for (int s = 0; s < used; s++) {
-            CU(cudaEventRecord(c->aslot[s].done, c->aslot[s].stream));
-            CU(cudaStreamWaitEvent(caller, c->aslot[s].done, 0));
-        }
-        int tail = LZ4B200_OK;
-        if (all_in && cut)
-            tail = launched(cudaMemcpyAsync(out_off, carry + (plan.size() - 1) % NASYNC, sizeof(int64_t), cudaMemcpyDefault, caller),
-                            "stream size copy");
-        if (all_in && framed)
-            tail = launched(walk ? launch_stream_walk_result(failed, c->walk_carry((int)((plan.size() - 1) % NASYNC)), out_off, caller, &c->launches)
-                                 : launch_stream_result(failed, sc->total, out_off, caller, &c->launches),
-                            "stream result launch");
-        CU(c->async_done.record(caller, Capture{}));
-        if (blk) CU(cudaEventRecord(blk->done, caller));
-        return tail;
-    };
-    rc = stages();
-    const int jr = join(rc == LZ4B200_OK);
-    return rc ? rc : jr;
-}
-
-// The capacities of n Wrap packets, src_len[i] + 8 (the largest a packet gets), into caps; an input whose packet would not
-// fit an int32 is refused.  Packets that go into the caller's slots (slot_cap) must each fit their slot.
-int wrap_caps(const int32_t* src_len, const int32_t* slot_cap, int32_t n, std::vector<int32_t>& caps)
-{
-    caps.resize((size_t)n);
-    for (int32_t i = 0; i < n; i++) {
-        if (src_len[i] < 0 || src_len[i] > INT32_MAX - WRAP_HEADER) return fail(LZ4B200_E_ARG, "input length: negative, or a packet above INT32_MAX bytes");
-        if (slot_cap && (int64_t)slot_cap[i] < (int64_t)src_len[i] + WRAP_HEADER) return fail(LZ4B200_E_ARG, "dst_cap[i] < src_len[i] + 8");
-        caps[i] = src_len[i] + WRAP_HEADER;
-    }
-    return LZ4B200_OK;
-}
-
-// The asynchronous packed encodes from device memory into page-locked host memory (the codec's blocks; Wrap packets,
-// kind WRAP_ENCODE, whose capacities are their own; an LZ4Stream, kind STREAM_ENCODE with sc, whose arguments the caller
-// has checked (stream_encode_args) and whose size goes to out_off[0]): the argument checks, the capture refusal and the
-// kinds of memory, then run_async.  n == 0 (for a stream, sc->n == 0) writes out_off[0] = 0 on the stream.
-int landed_async(lz4b200_ctx* c, Stage kind, int mode, const void* src, const int64_t* src_off, const int32_t* src_len,
-                 const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
-                 void* stream, const char* what, const StreamCall* sc = nullptr)
-{
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
-    std::vector<int32_t> pcap;
-    if (!sc) {
-        if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
-        const bool wrap = kind == Stage::WRAP_ENCODE;
-        if (n > 0 && (!src || !src_off || !src_len || (!wrap && !dst_cap) || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-        // a Wrap's dense slots hold whole packets
-        int rc = wrap ? wrap_caps(src_len, nullptr, n, pcap) : check_lengths(src_len, dst_cap, n, "block"); if (rc) return rc;
-        if (wrap) dst_cap = pcap.data();
-    }
-    CallGuard g(c); if (g.rc) return g.rc;
-    int rc = refuse_capture(stream, what, false); if (rc) return rc;
-    void *off_at = nullptr, *dst_at = nullptr, *len_at = nullptr;
-    rc = device_address(c, out_off, true, sc ? "out_size" : "out_off", &off_at); if (rc) return rc;
-    if (sc ? sc->n == 0 : n == 0) { CU(cudaMemsetAsync(off_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
-    rc = check_side(c, src, true, "src"); if (rc) return rc;
-    rc = device_address(c, dst, false, "dst", &dst_at); if (rc) return rc;
-    if (!sc) { rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc; }
-    return run_async(c, kind, encode_op(mode == LZ4B200_MODE_HC), (const uint8_t*)src, src_off, src_len, (uint8_t*)dst_at, nullptr,
-                     dst_cap, (int32_t*)len_at, n, (int64_t*)off_at, dst_total_cap, (cudaStream_t)stream, sc);
-}
 
 // The decode entries of an LZ4Stream of n bytes at s, from its header walk (stream_walk): one per non-empty chunk, with
 // its payload offset, compLen, output offset, rawLen and stored flag -- the header's flag: a compressed chunk may have
@@ -1195,90 +894,404 @@ int64_t stream_entries(const uint8_t* s, int64_t n, StreamEntries* e)
     return total;
 }
 
-// The asynchronous decodes from page-locked host memory into device memory (the codec's blocks; Unwrap packets, kind
-// UNWRAP), into the caller's slots or packed (out_off, dst_total_cap; no dst_off, dst_cap): the argument checks, the
-// capture refusal and the kinds of memory, then run_async.  A packed call with n == 0 writes out_off[0] = 0 on the stream.
-// An LZ4Stream (stream_n >= 0: its length; kind FRAMED_DECODE, packed) has no arrays: the host walks its headers once src
-// is known to be page-locked, and its entries are the batch.  A malformed header is the call's LZ4B200_E_FORMAT, a decoded
-// size above dst_total_cap its LZ4B200_E_ARG, both before any device work; the decoded size, or the status the device
-// finds, goes to out_off[0], and 0 when the stream decodes to nothing.
-int staged_async(lz4b200_ctx* c, Stage kind, Op op, bool packed, const void* src, const int64_t* src_off, const int32_t* src_len,
-                 void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
-                 int64_t dst_total_cap, void* stream, const char* what, int64_t stream_n = -1)
+// Where the blocks of an asynchronous call's stages come from.
+enum class Source {
+    DEVICE,    // device memory, read in place, with host entries: the packed encodes
+    COPIED,    // page-locked host memory copied up a stage at a time, with host entries: the decodes
+    CUT,       // device memory, the entries cut on the device (stream_cut_one): the LZ4Stream encode
+    LIFTED,    // page-locked host memory lifted by offsets read on the device (lz4_lift.cuh): the _at decode and Unwrap
+    WALKED,    // page-locked host memory, its headers walked on the device (stream_walk_stage): the _at LZ4Stream decode
+};
+
+// One asynchronous call: what its stages run (kind, op), where their blocks come from, the caller's arrays, and the few
+// fields of the LZ4Stream and lifted calls, in that order.  out_off is an LZ4Stream call's out_size.
+struct AsyncCall {
+    Stage kind; Op op; Source from;
+    const uint8_t* src = nullptr; const int64_t* src_off = nullptr; const int32_t* src_len = nullptr;
+    uint8_t* dst = nullptr; const int64_t* dst_off = nullptr; const int32_t* dst_cap = nullptr;
+    int32_t* out_len = nullptr; int32_t n = 0; int64_t* out_off = nullptr; int64_t dst_total_cap = 0;
+    int64_t src_cap = 0;                   // LIFTED, WALKED: the bytes of src that may be read
+    const int64_t* src_size = nullptr;     // WALKED: where the stream's size S is
+    int64_t stream_len = 0;                // CUT, and COPIED into FRAMED_DECODE: the stream's length
+    int32_t block_size = 0;                // CUT, WALKED: the chunk size
+    std::vector<int32_t> bound;            // LIFTED: each block's bound, by which the stages are cut and their slots sized
+    const uint8_t* stored = nullptr;       // COPIED into FRAMED_DECODE: the entries' stored flags
+    int64_t total = 0;                     //   and the decoded size
+    // the packed decodes, whose stages place their blocks on the device (lz4_packed.cuh)
+    bool placed() const { return kind == Stage::PLACED_DECODE || (kind == Stage::UNWRAP && !dst_off); }
+};
+
+// A lift stage's metadata: dst_off / dst_cap as the caller gave them, each block's slot (so[i], and its prefix in off[0..m])
+// and its bound (aux); the spans are written on the device.  sp.shi = the stage's staging bytes.
+StageSpan fill_lift(const Meta& h, int32_t b0, int32_t b1, const int32_t* bound, const int64_t* dst_off, const int32_t* dst_cap)
 {
-    const char* unit = kind == Stage::UNWRAP ? "packet" : "block";
-    const bool lz4s = stream_n >= 0;
-    if (!c) return fail(LZ4B200_E_ARG, "null context");
-    if (!lz4s) {
-        if (packed && (n < 0 || !out_off || dst_total_cap < 0)) return fail(LZ4B200_E_ARG, "bad argument");
-        if (n < 0) return fail(LZ4B200_E_ARG, std::string("negative ") + unit + " count");
-        if (n > 0 && (!src || !src_off || !src_len || !dst || (!packed && (!dst_off || !dst_cap)) || !out_len))
-            return fail(LZ4B200_E_ARG, "null argument");
-        int rc = check_lengths(src_len, dst_cap, n, unit); if (rc) return rc;
+    StageSpan sp;
+    for (int32_t i = 0; i < b1 - b0; i++) {
+        h.off[i] = h.so[i] = sp.shi;
+        h.dof[i] = dst_off[b0 + i]; h.sl[i] = 0; h.dc[i] = dst_cap[b0 + i]; h.aux[i] = bound[b0 + i];
+        sp.shi += lift_slot_bytes(bound[b0 + i]);
     }
-    CallGuard g(c); if (g.rc) return g.rc;
-    int rc = refuse_capture(stream, what, false); if (rc) return rc;
-    void *at = nullptr, *total_at = nullptr;
-    if (packed) {
-        rc = device_address(c, out_off, true, lz4s ? "out_size" : "out_off", &total_at); if (rc) return rc;
-        if (lz4s ? stream_n == 0 : n == 0) { CU(cudaMemsetAsync(total_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
-    }
-    if (n == 0 && !lz4s) return LZ4B200_OK;
-    rc = device_address(c, src, false, "src", &at); if (rc) return rc;
-    StreamEntries e;
-    StreamCall sc;
-    if (lz4s) {
-        // src is final: a caller who knows the stream's length has its bytes in place
-        const int64_t total = stream_entries((const uint8_t*)src, stream_n, &e);
-        if (total < 0) return fail((int)total, "malformed LZ4Stream");
-        if (total > dst_total_cap || (total > 0 && !dst)) return fail(LZ4B200_E_ARG, "dst_cap < the decoded size");
-        if (total == 0) { CU(cudaMemsetAsync(total_at, 0, sizeof(int64_t), (cudaStream_t)stream)); return LZ4B200_OK; }
-        if (e.so.size() > (size_t)INT32_MAX) return fail(LZ4B200_E_ARG, "more than INT32_MAX non-empty chunks");
-        n = (int32_t)e.so.size();
-        src_off = e.so.data(); src_len = e.len.data(); dst_off = e.dof.data(); dst_cap = e.raw.data(); out_off = (int64_t*)total_at;
-        sc = StreamCall{stream_n, 0, e.stored.data(), total};
-    }
-    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
-    if (!lz4s) { rc = device_address(c, out_len, true, "out_len", &at); if (rc) return rc; }
-    // (the stages copy out_len and out_off at the caller's addresses, which the copy engines take for either kind)
-    return run_async(c, kind, op, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n, out_off,
-                     dst_total_cap, (cudaStream_t)stream, lz4s ? &sc : nullptr);
+    h.off[b1 - b0] = sp.shi;
+    return sp;
 }
 
-// The asynchronous decode and Unwrap from page-locked host memory whose offsets src_off (n + 1 entries, device memory or
-// page-locked) are read on the device: the argument checks, each block's bound (a decode's compress_bound(dst_cap[i]), an
-// Unwrap packet's dst_cap[i] + 8, at most INT32_MAX), the capture refusal and the kinds of memory, then run_async.
-int lifted_async(lz4b200_ctx* c, Stage kind, Op op, const void* src, int64_t src_cap, const int64_t* src_off, void* dst,
+// A walk stage's device scratch, in AsyncSlot::offs: the lift descriptor the walk writes (STREAM_WALK_LIFT_I64 int64, then
+// the int32 bound), then the lift's entry for its one block (so, then sl and dc).
+constexpr size_t WALK_OFFS_BYTES = sizeof(int64_t) * (STREAM_WALK_LIFT_I64 + 3);
+
+// An asynchronous stage: blocks [b0, b1), their host metadata at `at` in the call's block; or chunks [first, first + b1).
+struct Plan { int32_t b0, b1; size_t at; StageSpan sp; int64_t first; };
+
+// The stage plan by blocks (DEVICE, COPIED, LIFTED), cut as run_host cuts it (stage_end; a lifted one by the bounds),
+// each stage described in the call's metadata block (fill_stage, fill_lift).
+int plan_blocks(lz4b200_ctx* c, const AsyncCall& a, std::vector<Plan>& plan, MetaBlock** blk)
+{
+    const bool enc = is_encode(a.op), lifted = a.from == Source::LIFTED;
+    size_t bytes = 0;
+    for (int32_t b0 = 0; b0 < a.n;) {
+        const int32_t b1 = stage_end(c, lifted ? a.bound.data() : a.src_len, enc ? a.dst_cap : nullptr, b0, a.n, !enc);
+        plan.push_back(Plan{b0, b1, bytes, {}, 0});
+        bytes += (meta_host_bytes(b1 - b0) + 15) & ~(size_t)15;
+        b0 = b1;
+    }
+    int rc = take_meta(c, bytes, blk); if (rc) return rc;
+    for (Plan& p : plan) {
+        const Meta h((uint8_t*)(*blk)->buf.p + p.at, p.b1 - p.b0);
+        p.sp = lifted ? fill_lift(h, p.b0, p.b1, a.bound.data(), a.dst_off, a.dst_cap)
+                      : fill_stage(h, p.b0, p.b1, a.src_off, a.src_len, a.dst_off, a.dst_cap, enc, !enc, false, a.placed(), a.stored);
+    }
+    return LZ4B200_OK;
+}
+
+// The stage plan by chunks (CUT, WALKED): the stream's chunks of block_size bytes (the encode's input, the walk's output
+// capacity), `per` a stage (as many as host_chunk_bytes holds, 1 to STREAM_RUN_CHUNKS), at least one stage (a walk's first
+// checks S).  An encode stage's span is its input; a walk stage's, the bytes its lift stages: *span_cap.
+void plan_chunks(const lz4b200_ctx* c, const AsyncCall& a, std::vector<Plan>& plan, int64_t* span_cap)
+{
+    const bool walked = a.from == Source::WALKED;
+    const int64_t bs = a.block_size, len = walked ? a.dst_total_cap : a.stream_len, chunks = len / bs + (len % bs != 0);
+    // a walk stage's span (a header may take STREAM_WALK_HEADER_MAX bytes) must fit an int32: the walk's cap alone
+    const int64_t frame = bs + STREAM_WALK_HEADER_MAX, cap = walked ? INT32_MAX / frame : STREAM_RUN_CHUNKS;
+    const int64_t per = std::max<int64_t>(1, std::min<int64_t>({(int64_t)c->host_chunk_bytes / bs, STREAM_RUN_CHUNKS, cap}));
+    // (the chunks' payloads add up to at most dst_total_cap bytes, which bounds a walk stage's span for a small output)
+    if (walked) *span_cap = std::min<int64_t>({per * frame, per * STREAM_WALK_HEADER_MAX + a.dst_total_cap, INT32_MAX});
+    for (int64_t k0 = 0; k0 == 0 || k0 < chunks; k0 += per) {
+        const int32_t m = (int32_t)std::min(per, chunks - k0);
+        StageSpan sp;
+        if (walked) sp.shi = lift_slot_bytes((int32_t)*span_cap);
+        else sp.dsum = std::min((int64_t)m * bs, len - k0 * bs);
+        plan.push_back(Plan{0, m, 0, sp, k0});
+    }
+}
+
+// The stages of an asynchronous call, enqueued on the context's NASYNC streams in turn, forked from `caller` and joined
+// back to it; nothing is waited on unless a buffer must grow.  A stage runs as arrival (by source: its entries and bytes
+// on the device; a lifted or walked stage's decoder is then picked on the device), its kind's sequence (run_stage, as in
+// run_host: the encoders write AsyncSlot::io, the decoders dst in place) and departure (by kind): the packed encodes'
+// scan and landing (lz4_land.cuh), or the LZ4Stream encode's frames and their landing, behind the running total the
+// previous stage left in its carry cell; an LZ4Stream decode's failure flag (Carry::failed, cleared behind the previous
+// call); the other decodes' results, after a lifted stage's rejections, with a packed stage's absolute offsets (placed
+// behind the previous stage's from the same cells) and the last running total.  Behind the join, on `caller`, an
+// LZ4Stream call writes its size, or its decoded size or status (stream_result, stream_walk_result), to out_off[0].
+// Calls are chained through async_done; the call's metadata block is taken again once the caller's stream has passed it.
+int run_async(lz4b200_ctx* c, const AsyncCall& a, cudaStream_t caller)
+{
+    const bool enc = is_encode(a.op), placed = a.placed(), framed = a.kind == Stage::FRAMED_DECODE;
+    std::vector<Plan> plan;
+    MetaBlock* blk = nullptr;
+    int64_t span_cap = 0;
+    if (a.from == Source::CUT || a.from == Source::WALKED) plan_chunks(c, a, plan, &span_cap);
+    else if (int rc = plan_blocks(c, a, plan, &blk)) return rc;
+    struct Sizes { size_t io = 0, frames = 0, meta = 0, offs = 0, scan = 0; } need[NASYNC];      // each slot's buffers, for its largest stage
+    for (size_t k = 0; k < plan.size(); k++) {
+        const Plan& p = plan[k];
+        const int32_t m = p.b1 - p.b0;
+        Sizes& nd = need[k % NASYNC];
+        nd.io = std::max(nd.io, (size_t)(enc ? p.sp.dsum : p.sp.shi - p.sp.slo) + 64);
+        if (a.from == Source::CUT) nd.frames = std::max(nd.frames, (size_t)p.sp.dsum + (size_t)m * STREAM_HEADER_MAX + 64);
+        nd.meta = std::max(nd.meta, async_meta_bytes(m));
+        if (enc || placed) { nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(m + 1)); nd.scan = std::max(nd.scan, compact_tmp_bytes(m)); }
+        if (a.from == Source::LIFTED) nd.offs = std::max(nd.offs, sizeof(int64_t) * (size_t)(2 * m + 3));      // slot[0..m] | span[0..m+1]
+        if (a.from == Source::WALKED) nd.offs = std::max(nd.offs, WALK_OFFS_BYTES);
+    }
+    // growth: an earlier call may still be using the buffers
+    bool grow = false;
+    for (int s = 0; s < NASYNC; s++) {
+        const AsyncSlot& sl = c->aslot[s];
+        grow |= need[s].io > sl.io.cap || need[s].frames > sl.frames.cap || need[s].meta > sl.meta.cap || need[s].offs > sl.offs.cap ||
+                need[s].scan > sl.scan.cap;
+    }
+    if (grow) {
+        CU(cudaDeviceSynchronize());
+        for (int s = 0; s < NASYNC; s++) {
+            AsyncSlot& sl = c->aslot[s];
+            CU(sl.io.reserve(need[s].io)); CU(sl.frames.reserve(need[s].frames)); CU(sl.meta.reserve(need[s].meta));
+            CU(sl.offs.reserve(need[s].offs)); CU(sl.scan.reserve(need[s].scan));
+        }
+    }
+    const int used = (int)std::min<size_t>(plan.size(), NASYNC);
+    Carry* carry = c->carry;
+    auto stages = [&]() -> int {
+        if (framed) {
+            // the failure flag, cleared behind the context's previous asynchronous call (which may still read it)
+            CU(c->async_done.wait(caller, Capture{}));
+            CU(cudaMemsetAsync(&carry->failed, 0, sizeof(int), caller));
+        }
+        CU(cudaEventRecord(c->entry, caller));
+        for (int s = 0; s < used; s++) {
+            CU(cudaStreamWaitEvent(c->aslot[s].stream, c->entry, 0));
+            CU(c->async_done.wait(c->aslot[s].stream, Capture{}));
+        }
+        for (size_t k = 0; k < plan.size(); k++) {
+            const Plan& p = plan[k];
+            const int s = (int)(k % NASYNC), prev = (s + NASYNC - 1) % NASYNC;
+            AsyncSlot& sl = c->aslot[s];
+            const int32_t m = p.b1 - p.b0;
+            const Meta d(sl.meta.p, m);
+            int64_t* offs = (int64_t*)sl.offs.p;
+            int64_t* span = offs + m + 1;
+            auto up = [&](bool aux) { const Meta h((uint8_t*)blk->buf.p + p.at, m);
+                                      return cudaMemcpyAsync(sl.meta.p, h.so, meta_up_bytes(h, aux), cudaMemcpyHostToDevice, sl.stream); };
+            int rc = LZ4B200_OK;
+            switch (a.from) {
+            case Source::DEVICE: CU(up(false)); break;
+            case Source::COPIED:
+                CU(up(framed));
+                if (p.sp.shi != p.sp.slo)
+                    CU(cudaMemcpyAsync(sl.io.p, a.src + p.sp.slo, (size_t)(p.sp.shi - p.sp.slo), cudaMemcpyHostToDevice, sl.stream));
+                break;
+            case Source::CUT:
+                rc = launched(launch_stream_cut(p.first, m, a.block_size, a.stream_len, d.so, d.sl, d.dof, d.dc, sl.stream, &c->launches),
+                              "stream chunk table launch");
+                break;
+            case Source::LIFTED:
+                CU(up(true));
+                // the slots, then the stage's offsets and src_off[n], wherever the caller's src_off lives
+                CU(cudaMemcpyAsync(offs, Meta((uint8_t*)blk->buf.p + p.at, m).off, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyHostToDevice,
+                                   sl.stream));
+                CU(cudaMemcpyAsync(span, a.src_off + p.b0, sizeof(int64_t) * (size_t)(m + 1), cudaMemcpyDefault, sl.stream));
+                CU(cudaMemcpyAsync(span + m + 1, a.src_off + a.n, sizeof(int64_t), cudaMemcpyDefault, sl.stream));
+                rc = launched(launch_lift(a.src, a.src_cap, offs, span, m, p.sp.shi, d.aux, d.so, d.sl, d.dc, (uint8_t*)sl.io.p, c->dev,
+                                          sl.stream, &c->launches), "lift launch");
+                break;
+            case Source::WALKED: {
+                // behind the previous stage's walk only; the next stage's walk follows this one, not its lift or decode
+                if (k > 0) CU(cudaStreamWaitEvent(sl.stream, c->aslot[prev].carried, 0));
+                const StreamWalkStage w{a.src, a.src_cap, k == 0 ? a.src_size : nullptr, k > 0 ? carry->walk[prev] : nullptr,
+                                        carry->walk[s], a.block_size, a.dst_total_cap, m, k + 1 == plan.size(), span_cap,
+                                        d.so, d.dof, d.sl, d.dc, d.aux, offs};
+                rc = launched(launch_stream_walk(w, sl.stream, &c->launches), "stream walk launch"); if (rc) return rc;
+                CU(cudaEventRecord(sl.carried, sl.stream));
+                if (m == 0) continue;
+                // the stage's span, as the lift's one block
+                int32_t* lifted = (int32_t*)(offs + STREAM_WALK_LIFT_I64 + 2);
+                rc = launched(launch_lift(a.src, a.src_cap, offs, offs + 2, 1, p.sp.shi, (const int32_t*)(offs + STREAM_WALK_LIFT_I64),
+                                          offs + STREAM_WALK_LIFT_I64 + 1, lifted, lifted + 1, (uint8_t*)sl.io.p, c->dev, sl.stream,
+                                          &c->launches), "stream lift launch");
+                break;
+            }
+            }
+            if (rc) return rc;
+            // (a packed Unwrap's prep reads no capacity: the placement writes the decode's into d.dc)
+            const BatchArgs b{enc ? a.src : (const uint8_t*)sl.io.p, d.so, d.sl, enc ? (uint8_t*)sl.io.p : a.dst, d.dof,
+                              a.kind == Stage::UNWRAP && placed ? nullptr : d.dc, d.out, m};
+            // a packed stage places behind the previous stage's placement (lz4_packed.cuh); the next one follows
+            const Placement pl = chained_placement(sl, d, async_fits(sl.meta.p, m), a.dst_total_cap, k > 0 ? &c->aslot[prev] : nullptr,
+                                                   &carry->async[prev], &carry->async[s]);
+            const int32_t hc_large = a.from == Source::CUT ? (a.op == Op::ENCODE_HC && a.block_size > 65536 ? m : 0)
+                                                           : stage_hc_large(a.op, a.src_len, p.b0, p.b1);
+            const int lanes = a.from == Source::LIFTED || a.from == Source::WALKED ? 0 : stage_lanes(c, a.op, a.src_len, a.dst_cap, p.b0, p.b1);
+            rc = run_stage(c, a.kind, a.op, b, lanes, hc_large, packet_view(sl.meta.p, m), placed ? &pl : nullptr, framed ? d.aux : nullptr,
+                           sl.stream);
+            if (rc) return rc;
+            // what lands, after its scan e: `bytes` dense bytes at `from` (dof, len), behind the previous stage's landing
+            auto land = [&](cudaError_t e, const uint8_t* from, const int64_t* dof, const int32_t* len, int64_t bytes, int64_t* to_off,
+                            int32_t* to_len) -> int {
+                if (e == cudaSuccess && k > 0) e = cudaStreamWaitEvent(sl.stream, c->aslot[prev].carried, 0);
+                if (e == cudaSuccess)
+                    e = launch_land(from, dof, len, offs, m, bytes, k > 0 ? &carry->async[prev] : nullptr, a.dst_total_cap, a.dst, to_off,
+                                    to_len, &carry->async[s], c->dev, sl.stream, &c->launches);
+                if (e != cudaSuccess) return cuda_fail(e, "scan / landing launch");
+                CU(cudaEventRecord(sl.carried, sl.stream));
+                return LZ4B200_OK;
+            };
+            switch (a.kind) {
+            case Stage::STREAM_ENCODE:      // the frames land, at their scan, of their sizes
+                rc = land(write_frames(c, b, a.op == Op::ENCODE_HC, d.aux, offs, sl.scan.p, sl.scan.cap, (uint8_t*)sl.frames.p, sl.stream),
+                          (const uint8_t*)sl.frames.p, offs, d.aux, p.sp.dsum + (int64_t)m * STREAM_HEADER_MAX, nullptr, nullptr);
+                break;
+            case Stage::FRAMED_DECODE:
+                rc = launched(launch_stream_status(d.sl, d.aux, d.out, m, &carry->failed, sl.stream, &c->launches), "stream status launch");
+                break;
+            case Stage::CODEC:
+            case Stage::WRAP_ENCODE:
+                if (enc) {
+                    rc = land(launch_compact(nullptr, nullptr, d.out, nullptr, offs, m, sl.scan.p, sl.scan.cap, c->dev, sl.stream, &c->launches),
+                              (const uint8_t*)sl.io.p, d.dof, d.out, p.sp.dsum, a.out_off + p.b0, a.out_len + p.b0);
+                    break;
+                }
+                [[fallthrough]];
+            case Stage::PLACED_DECODE:
+            case Stage::UNWRAP:
+                if (a.from == Source::LIFTED)
+                    rc = launched(launch_lift_status(a.src_cap, span, m, d.aux, d.out, sl.stream, &c->launches), "lift status launch");
+                if (rc) return rc;
+                CU(cudaMemcpyAsync(a.out_len + p.b0, d.out, sizeof(int32_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
+                if (placed) {
+                    CU(cudaMemcpyAsync(a.out_off + p.b0, d.dof, sizeof(int64_t) * (size_t)m, cudaMemcpyDefault, sl.stream));
+                    if (p.b1 == a.n) CU(cudaMemcpyAsync(a.out_off + a.n, &carry->async[s], sizeof(int64_t), cudaMemcpyDefault, sl.stream));
+                }
+                break;
+            }
+            if (rc) return rc;
+        }
+        return LZ4B200_OK;
+    };
+    // whatever was enqueued, the caller's stream joins it, and the chain and the metadata block are recorded behind it; an
+    // LZ4Stream call whose stages are all in writes its size or status in between
+    auto join = [&](bool all_in) -> int {
+        for (int s = 0; s < used; s++) {
+            CU(cudaEventRecord(c->aslot[s].done, c->aslot[s].stream));
+            CU(cudaStreamWaitEvent(caller, c->aslot[s].done, 0));
+        }
+        const int last = (int)((plan.size() - 1) % NASYNC);
+        int tail = LZ4B200_OK;
+        if (all_in) switch (a.kind) {
+        case Stage::STREAM_ENCODE:
+            tail = launched(cudaMemcpyAsync(a.out_off, &carry->async[last], sizeof(int64_t), cudaMemcpyDefault, caller), "stream size copy");
+            break;
+        case Stage::FRAMED_DECODE:
+            tail = launched(a.from == Source::WALKED ? launch_stream_walk_result(&carry->failed, carry->walk[last], a.out_off, caller, &c->launches)
+                                                     : launch_stream_result(&carry->failed, a.total, a.out_off, caller, &c->launches),
+                            "stream result launch");
+            break;
+        default: break;
+        }
+        CU(c->async_done.record(caller, Capture{}));
+        if (blk) CU(cudaEventRecord(blk->done, caller));
+        return tail;
+    };
+    int rc = stages();
+    const int jr = join(rc == LZ4B200_OK);
+    return rc ? rc : jr;
+}
+
+// The way into every asynchronous call, after its argument checks: the context's lock and device, the capture refusal,
+// each pointer by the side it must be on (a packed call's out_off first, then out_off[0] = 0 if there is nothing to do;
+// an LZ4Stream's headers are walked once src is known to be page-locked), then run_async.  The kernels reach the
+// caller's memory at its device addresses; the copy engines take the caller's addresses as given.
+int enter_async(lz4b200_ctx* c, AsyncCall a, void* stream, const char* what)
+{
+    CallGuard g(c); if (g.rc) return g.rc;
+    int rc = refuse_capture(stream, what, false); if (rc) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const bool lz4s = a.kind == Stage::STREAM_ENCODE || a.kind == Stage::FRAMED_DECODE, walked = a.from == Source::WALKED;
+    const bool from_device = a.from == Source::DEVICE || a.from == Source::CUT;      // src device memory, dst page-locked
+    void* at = nullptr;
+    // p's device address, in `at`, and in p itself for a pointer the kernels take (use)
+    auto reach = [&](auto*& p, bool device_ok, const char* name, bool use) {
+        const int r = device_address(c, p, device_ok, name, &at);
+        if (!r && use) p = static_cast<std::remove_reference_t<decltype(p)>>(at);
+        return r;
+    };
+    if (a.out_off && !walked) {
+        rc = reach(a.out_off, true, lz4s ? "out_size" : "out_off", a.from != Source::COPIED || lz4s); if (rc) return rc;
+        if (lz4s ? a.stream_len == 0 : a.n == 0) { CU(cudaMemsetAsync(at, 0, sizeof(int64_t), st)); return LZ4B200_OK; }
+    }
+    if (a.n == 0 && !lz4s) return LZ4B200_OK;
+    if (from_device) rc = check_side(c, a.src, true, "src");
+    else if (a.src) rc = reach(a.src, false, "src", a.from != Source::COPIED);      // a walked call's src may be null
+    if (!rc && a.from == Source::LIFTED) rc = reach(a.src_off, true, "src_off", false);
+    if (!rc && walked) rc = reach(a.src_size, true, "src_size", true);
+    if (rc) return rc;
+    StreamEntries e;
+    if (a.from == Source::COPIED && lz4s) {
+        // src is final: a caller who knows the stream's length has its bytes in place
+        a.total = stream_entries(a.src, a.stream_len, &e);
+        if (a.total < 0) return fail((int)a.total, "malformed LZ4Stream");
+        if (a.total > a.dst_total_cap || (a.total > 0 && !a.dst)) return fail(LZ4B200_E_ARG, "dst_cap < the decoded size");
+        if (a.total == 0) { CU(cudaMemsetAsync(a.out_off, 0, sizeof(int64_t), st)); return LZ4B200_OK; }
+        if (e.so.size() > (size_t)INT32_MAX) return fail(LZ4B200_E_ARG, "more than INT32_MAX non-empty chunks");
+        a.n = (int32_t)e.so.size();
+        a.src_off = e.so.data(); a.src_len = e.len.data(); a.dst_off = e.dof.data(); a.dst_cap = e.raw.data(); a.stored = e.stored.data();
+    }
+    if (from_device) rc = reach(a.dst, false, "dst", true);
+    else if (a.dst) rc = check_side(c, a.dst, true, "dst");                            // a walked call's dst may be null
+    if (!rc && a.out_len) rc = reach(a.out_len, true, "out_len", from_device);
+    if (!rc && walked) rc = reach(a.out_off, true, "out_size", true);
+    return rc ? rc : run_async(c, a, st);
+}
+
+// The capacities of n Wrap packets, src_len[i] + 8 (the largest a packet gets), into caps; an input whose packet would not
+// fit an int32 is refused.  Packets that go into the caller's slots (slot_cap) must each fit their slot.
+int wrap_caps(const int32_t* src_len, const int32_t* slot_cap, int32_t n, std::vector<int32_t>& caps)
+{
+    caps.resize((size_t)n);
+    for (int32_t i = 0; i < n; i++) {
+        if (src_len[i] < 0 || src_len[i] > INT32_MAX - WRAP_HEADER) return fail(LZ4B200_E_ARG, "input length: negative, or a packet above INT32_MAX bytes");
+        if (slot_cap && (int64_t)slot_cap[i] < (int64_t)src_len[i] + WRAP_HEADER) return fail(LZ4B200_E_ARG, "dst_cap[i] < src_len[i] + 8");
+        caps[i] = src_len[i] + WRAP_HEADER;
+    }
+    return LZ4B200_OK;
+}
+
+// The argument checks of the asynchronous packed encodes (the codec's blocks; Wrap packets, kind WRAP_ENCODE, whose
+// capacities are their own), then enter_async.
+int encode_async(lz4b200_ctx* c, Stage kind, int mode, const void* src, const int64_t* src_off, const int32_t* src_len,
+                 const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
+                 void* stream, const char* what)
+{
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (mode != LZ4B200_MODE_FAST && mode != LZ4B200_MODE_HC) return fail(LZ4B200_E_ARG, "unknown encoder mode");
+    if (n < 0 || !out_off || dst_total_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
+    const bool wrap = kind == Stage::WRAP_ENCODE;
+    if (n > 0 && (!src || !src_off || !src_len || (!wrap && !dst_cap) || !dst || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
+    // a Wrap's dense slots hold whole packets
+    std::vector<int32_t> pcap;
+    int rc = wrap ? wrap_caps(src_len, nullptr, n, pcap) : check_lengths(src_len, dst_cap, n, "block"); if (rc) return rc;
+    return enter_async(c, {kind, encode_op(mode == LZ4B200_MODE_HC), Source::DEVICE, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst,
+                           nullptr, wrap ? pcap.data() : dst_cap, out_len, n, out_off, dst_total_cap}, stream, what);
+}
+
+// The argument checks of the asynchronous decodes (the codec's blocks; Unwrap packets, kind UNWRAP) into the caller's
+// slots or packed (out_off, dst_total_cap; no dst_off, dst_cap), then enter_async.
+int decode_async(lz4b200_ctx* c, Stage kind, Op op, bool packed, const void* src, const int64_t* src_off, const int32_t* src_len,
+                 void* dst, const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int64_t* out_off,
+                 int64_t dst_total_cap, void* stream, const char* what)
+{
+    const char* unit = kind == Stage::UNWRAP ? "packet" : "block";
+    if (!c) return fail(LZ4B200_E_ARG, "null context");
+    if (packed && (n < 0 || !out_off || dst_total_cap < 0)) return fail(LZ4B200_E_ARG, "bad argument");
+    if (n < 0) return fail(LZ4B200_E_ARG, std::string("negative ") + unit + " count");
+    if (n > 0 && (!src || !src_off || !src_len || !dst || (!packed && (!dst_off || !dst_cap)) || !out_len))
+        return fail(LZ4B200_E_ARG, "null argument");
+    int rc = check_lengths(src_len, dst_cap, n, unit); if (rc) return rc;
+    return enter_async(c, {kind, op, Source::COPIED, (const uint8_t*)src, src_off, src_len, (uint8_t*)dst, dst_off, dst_cap, out_len, n,
+                           out_off, dst_total_cap}, stream, what);
+}
+
+// The argument checks of the decode and Unwrap whose offsets src_off (n + 1) are read on the device, and each block's
+// bound (compress_bound(dst_cap[i]), or an Unwrap packet's dst_cap[i] + 8, at most INT32_MAX); then enter_async.
+int decode_at_async(lz4b200_ctx* c, Stage kind, Op op, const void* src, int64_t src_cap, const int64_t* src_off, void* dst,
                  const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream, const char* what)
 {
     const bool unwrap = kind == Stage::UNWRAP;
     if (!c) return fail(LZ4B200_E_ARG, "null context");
     if (n < 0 || src_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
     if (n > 0 && (!src || !src_off || !dst || !dst_off || !dst_cap || !out_len)) return fail(LZ4B200_E_ARG, "null argument");
-    LiftCall lc;
-    lc.src_cap = src_cap; lc.src_off = src_off; lc.bound.resize((size_t)n);
+    AsyncCall a{kind, op, Source::LIFTED, (const uint8_t*)src, src_off, nullptr, (uint8_t*)dst, dst_off, dst_cap, out_len, n, nullptr, 0,
+                src_cap};
+    a.bound.resize((size_t)n);
     for (int32_t i = 0; i < n; i++) {
         if (dst_cap[i] < 0) return fail(LZ4B200_E_ARG, std::string("negative ") + (unwrap ? "packet" : "block") + " capacity");
-        lc.bound[i] = unwrap ? (int32_t)std::min<int64_t>((int64_t)dst_cap[i] + WRAP_HEADER, INT32_MAX)
-                             : (int32_t)std::min<int64_t>((int64_t)dst_cap[i] + dst_cap[i] / 255 + 16, INT32_MAX);
+        a.bound[i] = unwrap ? (int32_t)std::min<int64_t>((int64_t)dst_cap[i] + WRAP_HEADER, INT32_MAX)
+                            : (int32_t)std::min<int64_t>((int64_t)dst_cap[i] + dst_cap[i] / 255 + 16, INT32_MAX);
     }
-    CallGuard g(c); if (g.rc) return g.rc;
-    int rc = refuse_capture(stream, what, false); if (rc) return rc;
-    if (n == 0) return LZ4B200_OK;
-    void *at = nullptr, *off_at = nullptr, *len_at = nullptr;
-    rc = device_address(c, src, false, "src", &at); if (rc) return rc;
-    rc = device_address(c, src_off, true, "src_off", &off_at); if (rc) return rc;
-    rc = check_side(c, dst, true, "dst"); if (rc) return rc;
-    rc = device_address(c, out_len, true, "out_len", &len_at); if (rc) return rc;
-    lc.src = (const uint8_t*)at;
-    // (src_off and out_len are copied at the caller's addresses, which the copy engines take for either kind)
-    return run_async(c, kind, op, (const uint8_t*)src, nullptr, nullptr, (uint8_t*)dst, dst_off, dst_cap, out_len, n, nullptr, 0,
-                     (cudaStream_t)stream, nullptr, &lc);
+    return enter_async(c, std::move(a), stream, what);
 }
 
-// The asynchronous LZ4Stream decode from page-locked host memory whose size S (*src_size, device memory or page-locked) is
-// read on the device: the argument checks, the stage plan (WalkCall), the capture refusal and the kinds of memory, then
-// run_async with the walk in place of the host's.  src may be null when src_cap == 0, dst when dst_cap == 0.
+// The argument checks of the LZ4Stream decode whose size S (*src_size) the device wrote, then enter_async.  src may be
+// null when src_cap == 0, dst when dst_cap == 0.
 int walked_async(lz4b200_ctx* c, const void* src, int64_t src_cap, const int64_t* src_size, int32_t block_size, void* dst,
                  int64_t dst_cap, int64_t* out_size, void* stream, const char* what)
 {
@@ -1286,24 +1299,8 @@ int walked_async(lz4b200_ctx* c, const void* src, int64_t src_cap, const int64_t
     if (src_cap < 0 || dst_cap < 0) return fail(LZ4B200_E_ARG, "bad argument");
     if (block_size < 1 || block_size > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "block_size: a chunk's frame must fit an int32");
     if (!src_size || !out_size || (src_cap > 0 && !src) || (dst_cap > 0 && !dst)) return fail(LZ4B200_E_ARG, "null argument");
-    WalkCall wc;
-    wc.src_cap = src_cap; wc.block_size = block_size; wc.dst_cap = dst_cap;
-    wc.chunks = dst_cap / block_size + (dst_cap % block_size != 0);
-    // the asynchronous encode's stages, as long as a stage's span (a header may take STREAM_WALK_HEADER_MAX bytes) fits an int32
-    const int64_t frame = (int64_t)block_size + STREAM_WALK_HEADER_MAX;
-    CallGuard g(c); if (g.rc) return g.rc;
-    wc.per = std::max<int64_t>(1, std::min<int64_t>({(int64_t)c->host_chunk_bytes / block_size, STREAM_RUN_CHUNKS, INT32_MAX / frame}));
-    // (the chunks' payloads add up to at most dst_cap bytes, which bounds a stage's span for a small output)
-    wc.stage_cap = std::min<int64_t>({wc.per * frame, wc.per * STREAM_WALK_HEADER_MAX + dst_cap, INT32_MAX});
-    int rc = refuse_capture(stream, what, false); if (rc) return rc;
-    void *at = nullptr, *size_at = nullptr, *out_at = nullptr;
-    if (src) { rc = device_address(c, src, false, "src", &at); if (rc) return rc; }
-    rc = device_address(c, src_size, true, "src_size", &size_at); if (rc) return rc;
-    if (dst) { rc = check_side(c, dst, true, "dst"); if (rc) return rc; }
-    rc = device_address(c, out_size, true, "out_size", &out_at); if (rc) return rc;
-    wc.src = (const uint8_t*)at; wc.src_size = (const int64_t*)size_at;
-    return run_async(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, wc.src, nullptr, nullptr, (uint8_t*)dst, nullptr, nullptr, nullptr, 0,
-                     (int64_t*)out_at, dst_cap, (cudaStream_t)stream, nullptr, nullptr, &wc);
+    return enter_async(c, {Stage::FRAMED_DECODE, Op::DECODE_KNOWN, Source::WALKED, (const uint8_t*)src, nullptr, nullptr, (uint8_t*)dst,
+                           nullptr, nullptr, nullptr, 0, out_size, dst_cap, src_cap, src_size, 0, block_size}, stream, what);
 }
 
 // Argument checks, the context's lock and its device for every batch call.  dst_off == nullptr with out_off set is the
@@ -1582,7 +1579,7 @@ int lz4b200_create(lz4b200_ctx** out, int device)
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device); c->dev.smem_per_sm = v;
     cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device); c->dev.smem_optin = v;
     cudaError_t e = cudaMalloc(&c->counters, sizeof(uint32_t) * (NCOUNTER + 4 * NCAPTURED));
-    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(int64_t) * (NSLOT + NASYNC + 1 + STREAM_WALK_CELLS * NASYNC));
+    if (e == cudaSuccess) e = cudaMalloc(&c->carry, sizeof(Carry));
     for (Chain* ch : {&c->hc_done, &c->compact_done, &c->async_done}) {
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->done, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ch->inner, cudaEventDisableTiming);
@@ -1650,7 +1647,7 @@ int lz4b200_encode_batch_packed_from_device_async(lz4b200_ctx* c, const void* sr
                                                   const int32_t* dst_cap, void* dst, int64_t dst_total_cap, int64_t* out_off,
                                                   int32_t* out_len, int32_t n, int mode, void* stream)
 {
-    return landed_async(c, Stage::CODEC, mode, src, src_off, src_len, dst_cap, dst, dst_total_cap, out_off, out_len, n, stream,
+    return encode_async(c, Stage::CODEC, mode, src, src_off, src_len, dst_cap, dst, dst_total_cap, out_off, out_len, n, stream,
                         "lz4b200_encode_batch_packed_from_device_async");
 }
 
@@ -1658,7 +1655,7 @@ int lz4b200_decode_batch_to_device_async(lz4b200_ctx* c, const void* src, const 
                                          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int known_len,
                                          void* stream)
 {
-    return staged_async(c, Stage::CODEC, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, false, src, src_off, src_len, dst, dst_off,
+    return decode_async(c, Stage::CODEC, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, false, src, src_off, src_len, dst, dst_off,
                         dst_cap, out_len, n, nullptr, 0, stream, "lz4b200_decode_batch_to_device_async");
 }
 
@@ -1666,7 +1663,7 @@ int lz4b200_decode_batch_packed_to_device_async(lz4b200_ctx* c, const void* src,
                                                 void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
                                                 void* stream)
 {
-    return staged_async(c, Stage::PLACED_DECODE, Op::DECODE_UNKNOWN, true, src, src_off, src_len, dst, nullptr, nullptr, out_len, n,
+    return decode_async(c, Stage::PLACED_DECODE, Op::DECODE_UNKNOWN, true, src, src_off, src_len, dst, nullptr, nullptr, out_len, n,
                         out_off, dst_total_cap, stream, "lz4b200_decode_batch_packed_to_device_async");
 }
 
@@ -1674,14 +1671,14 @@ int lz4b200_wrap_batch_packed_from_device_async(lz4b200_ctx* c, const void* src,
                                                 int high_compression, void* dst, int64_t dst_total_cap, int64_t* out_off,
                                                 int32_t* out_len, int32_t n, void* stream)
 {
-    return landed_async(c, Stage::WRAP_ENCODE, high_compression ? LZ4B200_MODE_HC : LZ4B200_MODE_FAST, src, src_off, src_len, nullptr,
+    return encode_async(c, Stage::WRAP_ENCODE, high_compression ? LZ4B200_MODE_HC : LZ4B200_MODE_FAST, src, src_off, src_len, nullptr,
                         dst, dst_total_cap, out_off, out_len, n, stream, "lz4b200_wrap_batch_packed_from_device_async");
 }
 
 int lz4b200_unwrap_batch_to_device_async(lz4b200_ctx* c, const void* src, const int64_t* src_off, const int32_t* src_len, void* dst,
                                          const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
 {
-    return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, false, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, nullptr, 0,
+    return decode_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, false, src, src_off, src_len, dst, dst_off, dst_cap, out_len, n, nullptr, 0,
                         stream, "lz4b200_unwrap_batch_to_device_async");
 }
 
@@ -1689,7 +1686,7 @@ int lz4b200_unwrap_batch_packed_to_device_async(lz4b200_ctx* c, const void* src,
                                                 void* dst, int64_t dst_total_cap, int64_t* out_off, int32_t* out_len, int32_t n,
                                                 void* stream)
 {
-    return staged_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, true, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
+    return decode_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, true, src, src_off, src_len, dst, nullptr, nullptr, out_len, n, out_off,
                         dst_total_cap, stream, "lz4b200_unwrap_batch_packed_to_device_async");
 }
 
@@ -1699,14 +1696,14 @@ int lz4b200_decode_batch_to_device_at_async(lz4b200_ctx* c, const void* src, int
                                             const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, int known_len,
                                             void* stream)
 {
-    return lifted_async(c, Stage::CODEC, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, src, src_cap, src_off, dst, dst_off, dst_cap,
+    return decode_at_async(c, Stage::CODEC, known_len ? Op::DECODE_KNOWN : Op::DECODE_UNKNOWN, src, src_cap, src_off, dst, dst_off, dst_cap,
                         out_len, n, stream, "lz4b200_decode_batch_to_device_at_async");
 }
 
 int lz4b200_unwrap_batch_to_device_at_async(lz4b200_ctx* c, const void* src, int64_t src_cap, const int64_t* src_off, void* dst,
                                             const int64_t* dst_off, const int32_t* dst_cap, int32_t* out_len, int32_t n, void* stream)
 {
-    return lifted_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, src, src_cap, src_off, dst, dst_off, dst_cap, out_len, n, stream,
+    return decode_at_async(c, Stage::UNWRAP, Op::DECODE_KNOWN, src, src_cap, src_off, dst, dst_off, dst_cap, out_len, n, stream,
                         "lz4b200_unwrap_batch_to_device_at_async");
 }
 
@@ -1718,21 +1715,20 @@ int lz4b200_stream_encode_from_device_async(lz4b200_ctx* c, const void* src, int
     if (block_size > INT32_MAX - STREAM_HEADER_MAX) return fail(LZ4B200_E_ARG, "block_size: a chunk's frame must fit an int32");
     if (int rc = stream_encode_args(c, src, n, block_size, dst, dst_cap)) return rc;
     if (!out_size) return fail(LZ4B200_E_ARG, "bad argument");
-    const StreamCall sc{n, block_size};
-    return landed_async(c, Stage::STREAM_ENCODE, high_compression ? LZ4B200_MODE_HC : LZ4B200_MODE_FAST, src, nullptr, nullptr, nullptr,
-                        dst, dst_cap, out_size, nullptr, 0, stream, "lz4b200_stream_encode_from_device_async", &sc);
+    return enter_async(c, {Stage::STREAM_ENCODE, encode_op(high_compression != 0), Source::CUT, (const uint8_t*)src, nullptr, nullptr,
+                           (uint8_t*)dst, nullptr, nullptr, nullptr, 0, out_size, dst_cap, 0, nullptr, n, block_size},
+                       stream, "lz4b200_stream_encode_from_device_async");
 }
 
 int lz4b200_stream_decode_to_device_async(lz4b200_ctx* c, const void* src, int64_t n, void* dst, int64_t dst_cap, int64_t* out_size,
                                           void* stream)
 {
     if (!c || n < 0 || (n > 0 && !src) || !out_size) return fail(LZ4B200_E_ARG, "bad argument");
-    return staged_async(c, Stage::FRAMED_DECODE, Op::DECODE_KNOWN, true, src, nullptr, nullptr, dst, nullptr, nullptr, nullptr, 0,
-                        out_size, dst_cap, stream, "lz4b200_stream_decode_to_device_async", n);
+    return enter_async(c, {Stage::FRAMED_DECODE, Op::DECODE_KNOWN, Source::COPIED, (const uint8_t*)src, nullptr, nullptr, (uint8_t*)dst,
+                           nullptr, nullptr, nullptr, 0, out_size, dst_cap, 0, nullptr, n}, stream, "lz4b200_stream_decode_to_device_async");
 }
 
-// The LZ4Stream decode whose size the device wrote (an asynchronous encode's out_size): its headers are walked on the
-// device (lz4_stream.cuh stream_walk_stage) and each stage's span is staged by the lift kernel (lz4_lift.cuh).
+// The LZ4Stream decode whose size an asynchronous encode wrote on the device: its headers are walked there (walked_async).
 int lz4b200_stream_decode_to_device_at_async(lz4b200_ctx* c, const void* src, int64_t src_cap, const int64_t* src_size,
                                              int32_t block_size, void* dst, int64_t dst_cap, int64_t* out_size, void* stream)
 {

@@ -80,10 +80,10 @@ SIMT_DEV void stream_stored_one(const uint8_t* payload, int32_t stored, uint8_t*
     group_copy<32, false>(dst, s, (uint32_t)stored, lane, 0xFFFFFFFFu);
 }
 
-// The asynchronous encode (capi.cu run_async) holds no per-chunk host metadata: each stage's chunk table is computed on
-// the device.  Entry i of the stage whose first chunk is `first`, in a stream of n bytes cut into block_size chunks: the
-// chunk is bytes [so, so + len) of the source, encoded into the stage's dense slot at dof with capacity cap = len.  Only
-// a stream's last chunk is short, so slot i starts at i * block_size.
+// The asynchronous encode (capi.cu run_async, Source::CUT: its stages planned by plan_chunks) holds no per-chunk host
+// metadata: each stage's chunk table is computed on the device.  Entry i of the stage whose first chunk is `first`, in a
+// stream of n bytes cut into block_size chunks: the chunk is bytes [so, so + len) of the source, encoded into the stage's
+// dense slot at dof with capacity cap = len.  Only a stream's last chunk is short, so slot i starts at i * block_size.
 SIMT_DEV void stream_cut_one(int64_t i, int64_t first, int32_t block_size, int64_t n, int64_t* so, int32_t* len, int64_t* dof,
                              int32_t* cap)
 {

@@ -23,10 +23,11 @@ void walk_fn(int lane, void* arg) { stream_walk_stage(*(const StreamWalkStage*)a
 
 extern "C" {
 
-// The walk kernel over `stages` stages of `per` chunk slots (the last one m_last), in order, as run_async chains them: the
-// first reads S from *src_size, each later one the previous stage's carry cells.  Stage k's entries go to [k * per, k * per
-// + m_k) of so / dof / sl / dc / stored, its lift descriptor (slot[2] | span[3] | bound) to lift + 8 k.  Returns the call's
-// result with the decode's failure flag clear (stream_walk_result).
+// The walk kernel over `stages` stages of `per` chunk slots (the last one m_last), in order, as run_async chains the
+// stages of a WALKED call: the first reads S from *src_size, each later one the previous stage's carry cells
+// (Carry::walk).  Stage k's entries go to [k * per, k * per + m_k) of so / dof / sl / dc / stored, its lift descriptor
+// (slot[2] | span[3] | bound) to lift + 8 k.  Returns the call's result with the decode's failure flag clear
+// (stream_walk_result).
 int64_t emu_stream_walk(const uint8_t* src, int64_t src_cap, const int64_t* src_size, int32_t block_size, int64_t dst_cap, int32_t per,
                         int32_t stages, int32_t m_last, int64_t stage_cap, int64_t* so, int64_t* dof, int32_t* sl, int32_t* dc,
                         int32_t* stored, int64_t* lift, uint64_t sched_seed)

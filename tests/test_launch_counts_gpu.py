@@ -4,8 +4,8 @@ The launch counts (`lz4b200_launch_count` before and after a call) pin what ever
 encoders, decoders and measure pass in every kind of memory a call accepts, host batches of one block and of more than
 eight (every landing mode of the host pipeline), every pinned `decode_lanes` value and the automatic pick, the LZ4Stream
 and Wrap / Unwrap calls in their host, device, mixed and packed forms, and the packed decode into device memory over
-several pipeline stages; and the six asynchronous calls between device memory and page-locked host memory in one stage and
-in several.  A change to the host code that adds, drops or reorders a step shows up here.
+several pipeline stages; and the eleven asynchronous calls between device memory and page-locked host memory in one stage
+and in several.  A change to the host code that adds, drops or reorders a step shows up here.
 
 The device calls share the context's scan scratch, capacities and packet view whatever stream they are on.  Enqueued on
 two streams with no synchronise in between, a call that grows that scratch and one that does not must both give their
@@ -23,7 +23,9 @@ LANES = (1, 4, 8, 16, 32, 104, 108, 116, 132)
 MEMS = {"host": 0, "device": 1, "device_to_host": 2, "host_to_device": 3}
 
 # Recorded on an H100 80GB HBM3; the same before and after the host pipeline named its operations and stage kinds, and
-# (the asynchronous rows) before and after the pipeline's stage kinds were dispatched in one place.
+# (the asynchronous rows) before and after the pipeline's stage kinds were dispatched in one place, and before and after
+# every asynchronous call was described by one AsyncCall and run as arrival, sequence, departure.  The rows of the
+# asynchronous LZ4Stream encode and decode and of the `_at` calls were recorded with the host code before that change.
 EXPECTED = {
     'encode/fast/host/1': 1, 'encode/hc/host/1': 2, 'decode/known/host/1': 1, 'decode/unknown/host/1': 1,
     'encode/fast/device/1': 1, 'encode/hc/device/1': 3, 'decode/known/device/1': 5, 'decode/unknown/device/1': 5,
@@ -75,7 +77,12 @@ EXPECTED = {
     'wrap_packed_async/fast/stages': 28, 'encode_packed_async/hc/stages': 28, 'wrap_packed_async/hc/stages': 36,
     'decode_async/known/stages': 3, 'decode_async/unknown/stages': 3, 'decode_packed_async/stages': 30,
     'unwrap_async/fast/stages': 21, 'unwrap_packed_async/fast/stages': 33, 'unwrap_async/hc/stages': 14,
-    'unwrap_packed_async/hc/stages': 22,
+    'unwrap_packed_async/hc/stages': 22, 'stream_encode_async/fast/1stage': 8, 'stream_encode_async/hc/1stage': 9,
+    'decode_at_async/known/1stage': 7, 'decode_at_async/unknown/1stage': 7, 'stream_decode_async/1stage': 4,
+    'stream_decode_at_async/1stage': 10, 'unwrap_at_async/fast/1stage': 9, 'unwrap_at_async/hc/1stage': 9,
+    'stream_encode_async/fast/stages': 32, 'stream_encode_async/hc/stages': 36, 'decode_at_async/known/stages': 28,
+    'decode_at_async/unknown/stages': 28, 'stream_decode_async/stages': 10, 'stream_decode_at_async/stages': 37,
+    'unwrap_at_async/fast/stages': 36, 'unwrap_at_async/hc/stages': 36,
 }
 
 
@@ -316,8 +323,9 @@ def _placed_calls(ctx, count):
 
 
 def _async_calls(ctx, count):
-    """The six asynchronous calls between device memory and page-locked host memory, each in one stage (the default
-    host_chunk_mb) and over several 1 MiB stages, in fast and HC where the call takes a mode."""
+    """The eleven asynchronous calls between device memory and page-locked host memory, each in one stage (the default
+    host_chunk_mb) and over several 1 MiB stages, in fast and HC where the call takes a mode.  The calls from offsets or a
+    size the device wrote are fed those of the packed encode, the packed Wrap and the LZ4Stream encode before them."""
     import torch
     from lz4net_b200 import native
     lib, h, st = native.lib(), ctx.handle, torch.cuda.current_stream().cuda_stream
@@ -333,6 +341,8 @@ def _async_calls(ctx, count):
                     torch.zeros(n, dtype=torch.int32, device="cuda"))
     cbuf, cso, csl = _src([oracle.encode(d)[1] for d in raws])
     comp = pin(cbuf)
+    d_want, bs = _dev(np.frombuffer(want, np.uint8).copy()), 65536
+    sbound = int(lib.lz4b200_stream_bound(len(want), bs))
     try:
         for stages, mb in (("1stage", 128), ("stages", 1)):
             ctx.set_option("host_chunk_mb", mb)
@@ -346,12 +356,20 @@ def _async_calls(ctx, count):
                         h, d_raw.data_ptr(), rso.ctypes.data, rsl.ctypes.data, ecap.ctypes.data, dst.data_ptr(), dst.numel(),
                         off.data_ptr(), out.data_ptr(), n, int(hc), st), "encode_packed_async"))
                 assert int(off[n]) <= dst.numel(), (stages, tag)
+                if not hc:
+                    encoded = (dst, off)
                 dst = pin(np.zeros(int(rsl.sum()) + 8 * n + 64, np.uint8))
                 off, out = outs()
                 count(f"wrap_packed_async/{tag}/{stages}", lambda: native.check(lib.lz4b200_wrap_batch_packed_from_device_async(
                     h, d_raw.data_ptr(), rso.ctypes.data, rsl.ctypes.data, int(hc), dst.data_ptr(), dst.numel(), off.data_ptr(),
                     out.data_ptr(), n, st), "wrap_packed_async"))
-                packets[hc] = (dst, off.cpu().numpy(), out.cpu().numpy())
+                packets[hc] = (dst, off.cpu().numpy(), out.cpu().numpy(), off)
+                wire, (size, _) = pin(np.zeros(sbound, np.uint8)), outs()
+                count(f"stream_encode_async/{tag}/{stages}", lambda: native.check(lib.lz4b200_stream_encode_from_device_async(
+                    h, d_want.data_ptr(), len(want), bs, int(hc), wire.data_ptr(), sbound, size.data_ptr(), st),
+                    "stream_encode_async"))
+                if not hc:
+                    streamed = (wire, size)
             for known in (True, False):
                 d_dst, (_, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
                 count(f"decode_async/{'known' if known else 'unknown'}/{stages}", lambda: native.check(
@@ -359,12 +377,28 @@ def _async_calls(ctx, count):
                         h, comp.data_ptr(), cso.ctypes.data, csl.ctypes.data, d_dst.data_ptr(), rdo.ctypes.data, rcap.ctypes.data,
                         out.data_ptr(), n, int(known), st), "decode_async"))
                 assert d_dst.cpu().numpy().tobytes() == want, (stages, known)
+                d_dst, (_, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
+                count(f"decode_at_async/{'known' if known else 'unknown'}/{stages}", lambda: native.check(
+                    lib.lz4b200_decode_batch_to_device_at_async(
+                        h, encoded[0].data_ptr(), encoded[0].numel(), encoded[1].data_ptr(), d_dst.data_ptr(), rdo.ctypes.data,
+                        rcap.ctypes.data, out.data_ptr(), n, int(known), st), "decode_at_async"))
+                assert d_dst.cpu().numpy().tobytes() == want, (stages, known)
+            d_dst, (size, _) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
+            count(f"stream_decode_async/{stages}", lambda: native.check(lib.lz4b200_stream_decode_to_device_async(
+                h, streamed[0].data_ptr(), int(streamed[1][0]), d_dst.data_ptr(), rtotal, size.data_ptr(), st),
+                "stream_decode_async"))
+            assert d_dst.cpu().numpy().tobytes() == want and int(size[0]) == rtotal, stages
+            d_dst, (size, _) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
+            count(f"stream_decode_at_async/{stages}", lambda: native.check(lib.lz4b200_stream_decode_to_device_at_async(
+                h, streamed[0].data_ptr(), sbound, streamed[1].data_ptr(), bs, d_dst.data_ptr(), rtotal, size.data_ptr(), st),
+                "stream_decode_at_async"))
+            assert d_dst.cpu().numpy().tobytes() == want and int(size[0]) == rtotal, stages
             d_dst, (off, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
             count(f"decode_packed_async/{stages}", lambda: native.check(lib.lz4b200_decode_batch_packed_to_device_async(
                 h, comp.data_ptr(), cso.ctypes.data, csl.ctypes.data, d_dst.data_ptr(), rtotal, off.data_ptr(), out.data_ptr(),
                 n, st), "decode_packed_async"))
             assert d_dst.cpu().numpy().tobytes() == want and int(off[n]) == rtotal, stages
-            for hc, (pk, poff, plen) in packets.items():
+            for hc, (pk, poff, plen, d_poff) in packets.items():
                 tag = "hc" if hc else "fast"
                 pso = np.ascontiguousarray(poff[:n])
                 d_dst, (_, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
@@ -378,6 +412,11 @@ def _async_calls(ctx, count):
                         h, pk.data_ptr(), pso.ctypes.data, plen.ctypes.data, d_dst.data_ptr(), rtotal, off.data_ptr(),
                         out.data_ptr(), n, st), "unwrap_packed_async"))
                 assert d_dst.cpu().numpy().tobytes() == want and int(off[n]) == rtotal, (stages, tag)
+                d_dst, (_, out) = torch.zeros(rtotal, dtype=torch.uint8, device="cuda"), outs()
+                count(f"unwrap_at_async/{tag}/{stages}", lambda: native.check(lib.lz4b200_unwrap_batch_to_device_at_async(
+                    h, pk.data_ptr(), pk.numel(), d_poff.data_ptr(), d_dst.data_ptr(), rdo.ctypes.data, rcap.ctypes.data,
+                    out.data_ptr(), n, st), "unwrap_at_async"))
+                assert d_dst.cpu().numpy().tobytes() == want, (stages, tag)
     finally:
         ctx.set_option("host_chunk_mb", 128)
 
