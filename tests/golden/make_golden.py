@@ -6,7 +6,8 @@
 golden_v1.json: encoder outputs on named inputs.  reference_v1.json: the reference's side of tests/test_oracle.py's
 port-versus-reference checks (return values and output digests), and the one input on which r93's LZ4HC gives up at
 LZ4_compressBound (tests/test_kernels_emu.py).  constructed_v1.json: what both reference decoders return on the
-constructed streams of tests/lz4seq.py, one case per line.
+constructed streams of tests/lz4seq.py, one case per line.  hc_constructed_v1.json: what the reference's LZ4HC returns
+on the constructed blocks of tests/hcedge.py, uncapped, at cap = n and at cap = ret - 1, one case per line.
 
 The reference ships no golden vectors of its own (SURVEY.md 8c); these are outputs of the reference itself on
 reproducible inputs (tests/cases.py), including the reference-defined AutoTest text (src/LZ4/LZ4Codec.cs:175-184).
@@ -19,7 +20,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 import oracle  # noqa: E402
-from tests import cases, lz4seq  # noqa: E402
+from tests import cases, hcedge, lz4seq  # noqa: E402
 
 
 def sha(b):
@@ -79,6 +80,17 @@ def main():
         f.write(",\n".join(json.dumps(r, separators=(",", ":")) for r in rows))
         f.write("\n]}\n")
     print("wrote", t.CONSTRUCTED, len(rows), "cases,", past, "known-size decodes accepted only by reading past isize")
+
+    corpus = hcedge.catalogue(t.HC_CONSTRUCTED_SEED)
+    rows = t.records_hc_constructed(corpus, "ref")
+    head = {"source": ref["source"], "generator": "tests/hcedge.py", "seed": t.HC_CONSTRUCTED_SEED,
+            "corpus": t._digest(*(p for c in corpus for p in (c.name, c.data))),
+            "row": "[name, ret, sha256, ret at cap = n, sha256, ret at cap = ret - 1 (absent when ret = 0), sha256]"}
+    with open(t.HC_CONSTRUCTED, "w") as f:
+        f.write(json.dumps(head, separators=(",", ":"))[:-1] + ',"cases":[\n')
+        f.write(",\n".join(json.dumps(r, separators=(",", ":")) for r in rows))
+        f.write("\n]}\n")
+    print("wrote", t.HC_CONSTRUCTED, len(rows), "cases")
 
 
 if __name__ == "__main__":

@@ -1,11 +1,12 @@
 """LZ4HC for blocks above 64 KiB, one warp per block over a sliding 64 KiB window (lz4net_b200/csrc/lz4hc_window.cuh), on
 the CPU warp emulator.  A block either gets the reference's (result, bytes) or is handed back (HCW_FALLBACK), nothing
-else."""
+else.  The planted blocks are tests/hcedge.py's window cases, which the H100 tests run too; each says which of the two
+the window kernel must do, and the thread kernel must give the reference's bytes on every one."""
 import numpy as np
 import pytest
 
 import oracle
-from tests import cases, emu
+from tests import cases, emu, hcedge
 
 FB = emu.HCW_FALLBACK
 
@@ -17,10 +18,6 @@ def _check(d, cap=None, **kw):
         return False
     assert (r, o) == oracle.encode_hc(d, cap=cap), (len(d), cap, kw)
     return True
-
-
-def _rand(n, seed):
-    return np.random.default_rng(seed).integers(0, 256, n, dtype=np.uint8).tobytes()
 
 
 # every model at the sizes around the segment boundaries; the emulator needs seconds per 64 KiB on the dense models, so
@@ -41,75 +38,59 @@ def test_window_corpus_matches_oracle(model):
         assert _check(d, sched_seed=n % 97 + 1), (model, n)
 
 
-def _plant(n, marks, seed=1):
-    """Random bytes (no 4-byte string repeats by chance) with the same 12-byte string at every position in `marks`."""
-    d = bytearray(_rand(n, seed))
-    s = b"\x01WINDOWEDGE\x02"
-    for p in marks:
-        d[p:p + len(s)] = s
-    return bytes(d)
+def _planted(prefix):
+    """Runs tests/hcedge.py's window cases whose names start with `prefix` through the window and the thread kernel."""
+    got = [c for c in hcedge.window_cases(1) if c.name.startswith(prefix)]
+    assert got, prefix
+    for i, c in enumerate(got):
+        want = oracle.encode_hc(c.data)
+        assert emu.encode_hc(c.data) == want, c.name
+        r, o = emu.encode_hcw_window(c.data, sched_seed=i + 1)
+        assert (r, o) == want if c.warp else r == FB, c.name
 
 
-@pytest.mark.parametrize("q", [65536 + 40, 131072, 131072 + 3, 196608 - 1, 196608 + 17])
+@pytest.mark.parametrize("q", hcedge.WINDOW_Q)
 def test_window_edges(q):
     """A candidate exactly 65535 back is taken, one 65536 back is not; a bucket whose previous position lies 65535 / 65536
     back (the reference clamps that delta); each with q on and across a segment boundary."""
-    n = q + 5000
-    for marks in ([q - 65535, q], [q - 65536, q], [q - 65536 - 65535, q - 65536, q], [q - 65536 - 65536, q - 65536, q],
-                  [q - 65536 - 1, q - 1, q], [q - 70000, q - 65535, q - 65534, q]):
-        if min(marks) >= 1:
-            assert _check(_plant(n, marks, seed=q)), (q, marks)
+    _planted(f"window-q{q}-")
 
 
 @pytest.mark.parametrize("q", [65535, 65536])
 def test_window_position_zero(q):
     """q <= 65535 with an empty bucket: position 0 is the walk's last candidate; from 65536 on it is out of the window."""
-    d = bytearray(_rand(q + 3000, q))
-    d[0:12] = d[q:q + 12] = b"\x03ZEROWINDOW\x04"
-    assert _check(bytes(d))
+    _planted(f"window-pos0-q{q}")
 
 
 def test_window_long_matches_skip_segments():
     """Runs of 100-300 KiB inside text: one match jumps one or several segments, which are never indexed."""
-    t = cases.content("mixed", 30000, seed=5).tobytes()
-    for run in (100_000, 300_000):
-        d = t + bytes(run) + t[::-1] + bytes([7]) * (run // 2) + t
-        assert _check(d), run
+    _planted("window-skip-")
 
 
 def test_window_repeat_detector_runs_longer_than_a_segment():
     for m, n in (("E100", 140000), ("runs", 150000), ("periodic", 131075)):
         assert _check(cases.content(m, n, seed=21).tobytes()), (m, n)
-    for period in (1, 2, 3, 4):
-        d = _rand(3000, period) + bytes(range(10, 10 + period)) * (200000 // period) + _rand(3000, period + 9)
-        assert _check(d), period
+    _planted("window-repeat-period")
 
 
 def test_window_one_bucket_holds_a_whole_segment():
     """Zeros over three segments: a bucket end of 65536, a segment whose counters all sit in one bucket."""
-    assert _check(bytes(196608 + 4000))
-    assert _check(bytes(200000) + cases.content("mixed", 5000, seed=3).tobytes())
-
-
-def _hash15(b4):
-    return ((int.from_bytes(b4, "little") * 2654435761) & 0xFFFFFFFF) >> 17
+    _planted("window-one-bucket-")
 
 
 def test_window_hands_back_the_colliding_triple():
     """A run of period 3 two of whose strings share a hash bucket, past 64 KiB: the repeat detector's chain is not the
     static one, so the block is handed back (and the same run with a triple that does not collide is encoded)."""
-    found = None
-    for a in range(1, 256):
-        for b in range(a + 1, 256):
-            for c in range(b + 1, 256):
-                s0, s1, s2 = bytes([a, b, c, a]), bytes([b, c, a, b]), bytes([c, a, b, c])
-                if _hash15(s1) == _hash15(s2) and _hash15(s0) != _hash15(s1):
-                    found = (a, b, c); break
-            if found: break
-        if found: break
-    d = _rand(70000, 3) + bytes(found) * 200 + _rand(500, 4)
-    assert emu.encode_hcw_window(d)[0] == FB
-    assert _check(_rand(70000, 3) + bytes([1, 2, 3]) * 200 + _rand(500, 4))
+    _planted("window-colliding-triple")
+    _planted("window-triple-not-colliding")
+
+
+def test_window_limited_output_planted():
+    """Capacities around the start and the end of the output over a planted block whose one long match is 65535 back."""
+    d = next(c for c in hcedge.window_cases(1) if c.name == "window-q131072-65535").data
+    r, _ = oracle.encode_hc(d)
+    for cap in sorted({0, 1, 2, 15, 16, 17, 270, 4096, 65535, 65536, len(d), r - 3, r - 2, r - 1, r, r + 1}):
+        assert _check(d, cap=cap), cap
 
 
 def test_window_limited_output():

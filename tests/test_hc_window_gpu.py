@@ -118,15 +118,8 @@ def test_hc_window_edge_cases(ctx):
         r, o = oracle.encode_hc(blocks[i])
         assert int(clen[i]) == r and slots[i * slot:i * slot + r].cpu().numpy().tobytes() == o, i
     # a batch where every block hands back (the colliding period-3 run, past 64 KiB): the thread kernel encodes it
-    found = None
-    h = lambda b4: ((int.from_bytes(b4, "little") * 2654435761) & 0xFFFFFFFF) >> 17
-    for a in range(1, 256):
-        for b in range(a + 1, 256):
-            for c in range(b + 1, 256):
-                if h(bytes([b, c, a, b])) == h(bytes([c, a, b, c])) and h(bytes([a, b, c, a])) != h(bytes([b, c, a, b])):
-                    found = (a, b, c); break
-            if found: break
-        if found: break
+    from tests import hcedge
+    found = hcedge.colliding_triple()
     rng = np.random.default_rng(5)
     back = [rng.integers(0, 256, 70000 + 1000 * i, dtype=np.uint8).tobytes() + bytes(found) * 200 + bytes(300) for i in range(6)]
     lens, outs = ctx.encode_blocks(back, hc=True)

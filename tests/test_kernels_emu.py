@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 import oracle
-from tests import cases, emu
+from tests import cases, emu, hcedge
 
 
 def _enc_check(blocks, caps=None, **kw):
@@ -349,24 +349,11 @@ def test_encode_hcw_upstream_fuzzer_buffers():
         assert _hcw_check(d, sched_seed=seed + 1), seed
 
 
-def _hash15(b4):
-    return ((int.from_bytes(b4, "little") * 2654435761) & 0xFFFFFFFF) >> 17
-
-
 def test_encode_hcw_hands_back_what_the_static_index_does_not_describe():
     """Larger than 64 KiB; and a run of period 3 two of whose strings share a hash bucket: the reference's repeat detector
     (original/lz4hc.c:437-455) writes chain deltas of 3 across positions whose real predecessor in the bucket is 1 back."""
     assert emu.encode_hcw(cases.content("ETEXT", 65537, seed=1).tobytes())[0] == emu.HCW_FALLBACK
-    found = None
-    for a in range(1, 256):
-        for b in range(a + 1, 256):
-            for c in range(b + 1, 256):
-                s0, s1, s2 = bytes([a, b, c, a]), bytes([b, c, a, b]), bytes([c, a, b, c])
-                if _hash15(s1) == _hash15(s2) and _hash15(s0) != _hash15(s1):
-                    found = (a, b, c); break
-            if found: break
-        if found: break
-    assert found, "no colliding triple"
+    found = hcedge.colliding_triple()
     rng = np.random.default_rng(3)
     d = rng.integers(0, 256, 500, dtype=np.uint8).tobytes() + bytes(found) * 200 + rng.integers(0, 256, 500, dtype=np.uint8).tobytes()
     assert emu.encode_hcw(d)[0] == emu.HCW_FALLBACK

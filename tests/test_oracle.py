@@ -17,6 +17,8 @@ GOLD = os.path.join(os.path.dirname(__file__), "golden", "golden_v1.json")
 REF = os.path.join(os.path.dirname(__file__), "golden", "reference_v1.json")
 CONSTRUCTED = os.path.join(os.path.dirname(__file__), "golden", "constructed_v1.json")
 CONSTRUCTED_SEED = 1                                 # tests/lz4seq.py's corpus(seed) that constructed_v1.json records
+HC_CONSTRUCTED = os.path.join(os.path.dirname(__file__), "golden", "hc_constructed_v1.json")
+HC_CONSTRUCTED_SEED = 1                              # tests/hcedge.py's catalogue(seed) that hc_constructed_v1.json records
 
 
 def _sha(b: bytes) -> str:
@@ -114,6 +116,21 @@ def records_constructed(impl):
         rows.append([max(rk, -1), max(ru, -1),
                      _digest(ok if 0 <= rk <= len(c.stream) else b"-", ou if ru >= 0 else b"-")[:8]])
     return _digest(*(p for c in corpus for p in (c.name, c.stream, c.cap))), rows
+
+
+def records_hc_constructed(corpus, impl):
+    """tests/hcedge.py's blocks: [name, ret, digest, ret and digest at cap = n, at cap = ret - 1] per case (the last
+    pair only where ret > 0)."""
+    rows = []
+    for c in corpus:
+        r, o = oracle.encode_hc(c.data, impl=impl)
+        row = [c.name, r, _sha(o)]
+        for cap in (len(c.data), r - 1):
+            if cap >= 0:
+                rc, oc = oracle.encode_hc(c.data, cap=cap, impl=impl)
+                row += [rc, _sha(oc)]
+        rows.append(row)
+    return rows
 
 
 def test_bound():
@@ -241,3 +258,19 @@ def test_port_equals_reference_on_constructed_streams():
             assert g == w, (c.name, g, w)
     past = sum(w[0] > len(c.stream) for c, w in zip(corpus, want))
     assert offset0 > 0 and past == stored["known_reads_past_isize"] > 0
+
+
+def test_port_equals_reference_on_constructed_hc_blocks():
+    """tests/hcedge.py's blocks -- candidates at the ends of the attempt budget, position 0, ties, lengths at matchlimit
+    and around the warp count's steps, backward extensions, repeats, the 64 KiB window: the port's LZ4HC returns what the
+    reference returned (hc_constructed_v1.json, made by make_golden.py), uncapped and at the two capacities LZ4Stream and
+    a one-byte shortfall give."""
+    from tests import hcedge
+    stored = json.load(open(HC_CONSTRUCTED))
+    corpus = hcedge.catalogue(HC_CONSTRUCTED_SEED)
+    assert _digest(*(p for c in corpus for p in (c.name, c.data))) == stored["corpus"], \
+        "tests/hcedge.py no longer makes the blocks the fixture was made from"
+    got = records_hc_constructed(corpus, "port")
+    assert len(got) == len(stored["cases"])
+    for g, w in zip(got, stored["cases"]):
+        assert g == w, g[0]
